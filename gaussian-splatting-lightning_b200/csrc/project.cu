@@ -11,6 +11,8 @@
 #include "common.cuh"
 #include "onesweep.cuh"
 
+#include <type_traits>
+
 namespace b200gs {
 
 namespace {
@@ -247,6 +249,22 @@ __device__ __forceinline__ void project_view(const B200gsView& v, const float* p
     g.a = xa(g.a0, R(v.eps2d));
     g.c = xa(g.c0, R(v.eps2d));
     g.det = xf(g.a, g.c, -bb);
+    if (std::is_same<R, float>::value) {
+        // The fp32 geometry (K8's) takes the determinants from forms without cancellation: a0 c0 - b^2 cancels completely
+        // for a needle (cov2D of rank ~1), and K8 would differentiate a compensation and a conic other than the ones K1
+        // rendered in fp64.  Cauchy-Binet: det0 = sum of the squared 2x2 minors of N = T M (cov2D = N N^T, M = Rm diag(s)),
+        // and det = det0 + e (a0 + c0 + e) with e = eps2d.  Not used in fp64 (K1), whose bits stay those of the form above.
+        R N[6];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            N[k] = (T[0] * g.Rm[k] + T[1] * g.Rm[3 + k] + T[2] * g.Rm[6 + k]) * g.s[k];
+            N[3 + k] = (T[3] * g.Rm[k] + T[4] * g.Rm[3 + k] + T[5] * g.Rm[6 + k]) * g.s[k];
+        }
+        const R m01 = N[0] * N[4] - N[1] * N[3], m02 = N[0] * N[5] - N[2] * N[3], m12 = N[1] * N[5] - N[2] * N[4];
+        const R e = R(v.eps2d);
+        g.det0 = m01 * m01 + m02 * m02 + m12 * m12;
+        g.det = g.det0 + e * (g.a0 + g.c0 + e);
+    }
 }
 
 // Optional fused-activation ("raw parameter") operands: the model's exp / normalize / sigmoid activations and the
@@ -674,12 +692,17 @@ __device__ __forceinline__ void geometry_backward(const B200gsView& v, const flo
     if (GSPLAT) {
         const float vc = c.vcomp;
         if (g.det0 > 0.f && vc != 0.f) {
+            // d comp / d(a, b, c) of comp = sqrt(det0 / det) is 0.5 comp (c0 / det0 - c / det, -2 b (1 / det0 - 1 / det), a0 / det0 - a / det).
+            // For a splat much larger than eps2d both quotients of each difference agree to ~eps2d / lambda, and fp32 subtraction
+            // left none of their digits (measured: 1e-2 relative errors on the scale gradients of large off-screen splats).  With
+            // det = det0 + e (a0 + c0 + e) and b^2 = a0 c0 - det0 the differences are e (c0^2 + c0 e + b^2) / (det0 det),
+            // e (a0 + c0 + e) / (det0 det) and e (a0^2 + a0 e + b^2) / (det0 det): sums of positive terms, no cancellation.
             const float comp = sqrtf(g.det0 * inv_det);
-            const float d_det0 = vc * 0.5f * comp / g.det0;
-            const float d_det = -vc * 0.5f * comp * inv_det;
-            da += d_det0 * g.c0 + d_det * g.c;
-            dc += d_det0 * g.a0 + d_det * g.a;
-            db += -2.0f * g.b * (d_det0 + d_det);
+            const float e = v.eps2d, bb = g.b * g.b;
+            const float k = vc * 0.5f * comp * e * inv_det / g.det0;
+            da += k * (g.c0 * (g.c0 + e) + bb);
+            dc += k * (g.a0 * (g.a0 + e) + bb);
+            db += -2.0f * g.b * k * (g.a0 + g.c0 + e);
         }
     }
     // symmetric gradient wrt the 2x2 cov: [[da, db/2],[db/2, dc]]
@@ -954,7 +977,9 @@ __global__ void __launch_bounds__(BWD_THREADS, (MC <= 16 ? (GSPLAT ? 7 : 6) : 3)
     c.vcomp = (GSPLAT && v_comp != nullptr) ? __ldg(v_comp + i) : 0.f;
     if (RAW) {
         // blend opacity = sigmoid(logit) [* compensation]: split dL/d(opac_out) between the logit and the compensation
-        const float o = 1.0f / (1.0f + expf(-__ldg(raw.opac_in + i)));
+        // 1 - o = sigmoid(-logit): 1.0f - o cancels at large logits (a 1e-2 relative error of the logit gradient at logit 12)
+        const float x = __ldg(raw.opac_in + i);
+        const float o = 1.0f / (1.0f + expf(-x)), o1 = 1.0f / (1.0f + expf(x));
         const float vo = __ldg(vrow + B200GS_ROW_OPACITY);
         float v_sig = vo;
         if (GSPLAT && raw.anti_aliased) {
@@ -963,7 +988,7 @@ __global__ void __launch_bounds__(BWD_THREADS, (MC <= 16 ? (GSPLAT ? 7 : 6) : 3)
             c.vcomp += vo * o;
         }
         // explicit fma: whether nvcc contracts the product into the add depends on the surrounding code (see xm / xa / xf)
-        raw.v_opac_logit[i] = fmaf(v_sig * o, 1.0f - o, ACC ? raw.v_opac_logit[i] : 0.f);
+        raw.v_opac_logit[i] = fmaf(v_sig * o, o1, ACC ? raw.v_opac_logit[i] : 0.f);
     }
     float dscale[3] = {0.f, 0.f, 0.f};
     float4 dq = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -1017,7 +1042,7 @@ __global__ void __launch_bounds__(BWD_THREADS) project_bwd_multi_kernel(const __
     for (int c = 0; c < rw; ++c) my_row[c] = 0.f;
     float dm[3] = {0.f, 0.f, 0.f}, dscale[3] = {0.f, 0.f, 0.f}, dlogit = 0.f;
     float4 dq = make_float4(0.f, 0.f, 0.f, 0.f);
-    float p[3] = {0.f, 0.f, 0.f}, sc[3] = {1.f, 1.f, 1.f}, q[4] = {1.f, 0.f, 0.f, 0.f}, inv_qn = 1.f, o = 0.f;
+    float p[3] = {0.f, 0.f, 0.f}, sc[3] = {1.f, 1.f, 1.f}, q[4] = {1.f, 0.f, 0.f, 0.f}, inv_qn = 1.f, o = 0.f, o1 = 0.f;
     bool loaded = false;
     Proj<float> g;
 #pragma unroll 1
@@ -1032,7 +1057,9 @@ __global__ void __launch_bounds__(BWD_THREADS) project_bwd_multi_kernel(const __
         if (!loaded) {
             p[0] = __ldg(means + 3 * i); p[1] = __ldg(means + 3 * i + 1); p[2] = __ldg(means + 3 * i + 2);
             load_scale_quat<true, float>(scales, quats, i, sc, q, &inv_qn);
-            o = 1.0f / (1.0f + expf(-__ldg(raw.opac_in + i)));
+            const float x = __ldg(raw.opac_in + i);
+            o = 1.0f / (1.0f + expf(-x));
+            o1 = 1.0f / (1.0f + expf(x));                            // 1 - o without cancellation
             gaussian_cov3d<float>(sc, q, vp.v[0].scale_modifier, g);      // once per Gaussian; project_view per camera
             g.qr = q[0]; g.qx = q[1]; g.qy = q[2]; g.qz = q[3];
             loaded = true;
@@ -1068,7 +1095,7 @@ __global__ void __launch_bounds__(BWD_THREADS) project_bwd_multi_kernel(const __
             v_sig = vo * comp;
             c.vcomp = vo * o;
         }
-        dlogit += v_sig * o * (1.0f - o);
+        dlogit += v_sig * o * o1;
         geometry_backward<true>(v, p, g, c, dm, dscale, dq);
     }
     if (in_range) { v_shs_dc[3 * i] = dc_acc[0]; v_shs_dc[3 * i + 1] = dc_acc[1]; v_shs_dc[3 * i + 2] = dc_acc[2]; }

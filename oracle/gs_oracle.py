@@ -197,11 +197,16 @@ def compute_cov_2d(t, tan_fovx, tan_fovy, focal_x, focal_y, cov_3d, world_to_cam
     return cov[:, :2, :2]
 
 
-def _radius_from_cov(a, b, c, det):
+def _extent_from_cov(a, b, c, det):
+    """3 sqrt(largest eigenvalue): the radius before it is rounded up to whole pixels."""
     mid = 0.5 * (a + c)
     sq = torch.sqrt(torch.clamp_min(mid * mid - det, 0.1))  # gaussian_projection.py:98-105 / dgr max(0.1, ...)
     lam = torch.maximum(mid + sq, mid - sq)
-    return torch.ceil(3.0 * torch.sqrt(lam)).to(torch.int32)
+    return 3.0 * torch.sqrt(lam)
+
+
+def _radius_from_cov(a, b, c, det):
+    return torch.ceil(_extent_from_cov(a, b, c, det)).to(torch.int32)
 
 
 def project(mode: int, means: torch.Tensor, scales: torch.Tensor, quats: torch.Tensor, view: View,
@@ -212,6 +217,8 @@ def project(mode: int, means: torch.Tensor, scales: torch.Tensor, quats: torch.T
     xy [N,2] pixel coordinates (vanilla: ((ndc+1)S-1)/2, i.e. pixel-index space; gsplat: K t/(t_z+1e-6), no +0.5),
     depth [N], radii int32 [N], conic [N,3], comp [N] (gsplat; ones in vanilla), tiles int32 [N],
     rect_min / rect_max int32 [N,2], mask bool [N], cov3d [N,3,3].  Entries of culled Gaussians are zero.
+    Unmasked, for tests that keep their scenes away from the culling decisions: t [N,3] camera-space means,
+    xy_all [N,2], extent [N] (3 sqrt(largest eigenvalue), the radius before it is rounded up).
     """
     dt = means.dtype
     v = view.to(dt)
@@ -294,6 +301,9 @@ def project(mode: int, means: torch.Tensor, scales: torch.Tensor, quats: torch.T
         "mask": mask,
         "rect_min": rmin,
         "rect_max": rmax,
+        "t": t,
+        "xy_all": xy,
+        "extent": _extent_from_cov(a, b, c, det),
     }
 
 
