@@ -114,7 +114,8 @@ class B200GSplatV1:
     @classmethod
     def isect_encode_tile_based_culling(cls, preprocessed_camera: Tuple, projection_results, opacities, tile_size: int = 16):
         """Only (tile, Gaussian) pairs whose tile can see alpha >= 1/255 are listed (exact test, binning.cu); images and gradients are
-        bit-identical to the unculled lists."""
+        bit-identical to the unculled lists for these opacities.  A rasterize call with larger opacities over the same lists (the
+        renderer's hard-depth passes) misses the pairs that only those opacities would have kept."""
         return cls._isect(preprocessed_camera, projection_results, tile_size, projection_results[3], opacities)
 
     @classmethod

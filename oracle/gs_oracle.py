@@ -347,7 +347,7 @@ def sort_and_ranges(keys: torch.Tensor, ids: torch.Tensor, n_tiles: int):
 # --------------------------------------------------------------------------------------------------------------------
 def blend(mode: int, xy: torch.Tensor, conic: torch.Tensor, opacity: torch.Tensor, colors: torch.Tensor,
           sorted_ids: torch.Tensor, ranges: torch.Tensor, bg: Optional[torch.Tensor], width: int, height: int,
-          block: int = BLOCK, margins: Optional[list] = None):
+          block: int = BLOCK, margins: Optional[list] = None, side: Optional[dict] = None):
     """Per-tile front-to-back compositing.  xy [N,2], conic [N,3], opacity [N], colors [N,D].
 
     Returns image [D,H,W], alpha [H,W] (= 1 - T_final), n_contrib int32 [H,W] (1-based index, inside the tile's
@@ -357,6 +357,20 @@ def blend(mode: int, xy: torch.Tensor, conic: torch.Tensor, opacity: torch.Tenso
     (pixel, splat) samples to a branch threshold of the loop (alpha vs 1/255, remaining T vs 1e-4, power vs 0, alpha vs the
     clamp of the gsplat backward).  A sample closer to a threshold than fp32 resolves may take the other branch in a
     float32 implementation; tests use this map to tell such pixels from real errors.
+
+    side: pass an empty dict to receive the side channels below; the returned values are the same with or without it.
+      "hit"         bool [N]: the splat is active (weight a * T_excl > 0) in at least one pixel: gsplat's has_hit_any_pixels.
+      "hit_margin"  [N]: how far "hit" is from flipping, in the units of `margins`.  A splat that is hit stays hit while one of
+                    its active samples keeps its branches: the largest margin of its active samples.  A splat that is not
+                    hit becomes hit if any sample the loop reaches flips: the smallest margin of those (inf when no pixel
+                    reaches it).  An fp32 implementation can only disagree with "hit" where this is small.  A pixel whose
+                    stop is ambiguous does not lower the margin of the splats behind it: if fp32 keeps it alive, the next
+                    valid sample (alpha >= 1/255) takes T below the cut-off and stops it with weight 0.
+      "stopped"     bool [H,W]: the pixel stopped at the 1e-4 transmittance cut-off.
+      "clamped"     int: the number of active samples whose alpha sits at the clamp (0.999 / 0.99).
+      "abs_terms"   list of (ids [L], dx [P,L], dy [P,L]) per non-empty tile: mean - pixel centre of every (pixel, splat) sample
+                    of the tile's list.  When xy requires grad they retain their gradient: after backward(), dx.grad[p, j] is
+                    pixel p's own contribution to the x gradient of splat ids[j], and absgrad() sums their magnitudes.
     """
     dt = xy.dtype
     D = colors.shape[1]
@@ -367,6 +381,14 @@ def blend(mode: int, xy: torch.Tensor, conic: torch.Tensor, opacity: torch.Tenso
     img = torch.zeros(height, width, D, dtype=dt)
     alpha_img = torch.zeros(height, width, dtype=dt)
     ncontrib = torch.zeros(height, width, dtype=torch.int32)
+    if side is not None:
+        n_splats = xy.shape[0]
+        side["hit"] = torch.zeros(n_splats, dtype=torch.bool)
+        side["hit_margin"] = torch.full((n_splats,), float("inf"), dtype=dt)
+        witness = torch.full((n_splats,), float("-inf"), dtype=dt)
+        side["clamped"] = 0
+        side["abs_terms"] = []
+        stopped_rows = []
     img_rows = []
     for ty in range(gy):
         row_tiles = []
@@ -380,6 +402,7 @@ def blend(mode: int, xy: torch.Tensor, conic: torch.Tensor, opacity: torch.Tenso
             PY = py[:, None].expand(y1 - y0, x1 - x0).reshape(-1)
             npx = PX.shape[0]
             tile_margin = torch.full((npx,), float("inf"), dtype=dt)
+            stopped = torch.zeros(npx, dtype=torch.bool)
             if e <= s:
                 C = torch.zeros(npx, D, dtype=dt)
                 Tf = torch.ones(npx, dtype=dt)
@@ -389,6 +412,11 @@ def blend(mode: int, xy: torch.Tensor, conic: torch.Tensor, opacity: torch.Tenso
                 mxy, con, op, col = xy[gid], conic[gid], opacity[gid], colors[gid]
                 dx = mxy[None, :, 0] - PX[:, None]
                 dy = mxy[None, :, 1] - PY[:, None]
+                if side is not None:
+                    if dx.requires_grad:
+                        dx.retain_grad()
+                        dy.retain_grad()
+                    side["abs_terms"].append((gid, dx, dy))
                 power = -0.5 * (con[None, :, 0] * dx * dx + con[None, :, 2] * dy * dy) - con[None, :, 1] * dx * dy
                 G = torch.exp(power)
                 raw = op[None, :] * G
@@ -402,14 +430,21 @@ def blend(mode: int, xy: torch.Tensor, conic: torch.Tensor, opacity: torch.Tenso
                     testT = torch.cumprod(1.0 - a_eff, dim=1)
                     alive = (testT > 1e-4) if mode == MODE_GSPLAT else (testT >= 1e-4)
                     active = valid & alive
-                    if margins is not None:
+                    if margins is not None or side is not None:
                         reach = torch.cat([torch.ones(npx, 1, dtype=torch.bool), alive[:, :-1]], dim=1)   # the sample is evaluated at all
                         big = torch.full((), float("inf"), dtype=dt)
                         m_alpha = torch.where(reach & (power <= 0), (raw - 1.0 / 255.0).abs() * 255.0, big)
                         m_T = torch.where(reach & valid, (testT - 1e-4).abs() / 1e-4, big)
                         m_pow = torch.where(reach, power.abs() / 1e-3, big)          # power > 0 is skipped: absolute scale 1e-3
                         m_clamp = torch.where(reach & valid, (raw - amax).abs() / amax, big)
-                        tile_margin = torch.minimum(torch.minimum(m_alpha, m_T), torch.minimum(m_pow, m_clamp)).min(dim=1).values
+                        m_sample = torch.minimum(torch.minimum(m_alpha, m_T), torch.minimum(m_pow, m_clamp))
+                        tile_margin = m_sample.min(dim=1).values
+                    if side is not None:
+                        stopped = (reach & valid & ~alive).any(dim=1)
+                        witness.scatter_reduce_(0, gid, torch.where(active, m_sample, -big).max(dim=0).values, "amax")
+                        side["hit_margin"].scatter_reduce_(0, gid, m_sample.min(dim=0).values, "amin")
+                        side["hit"][gid[active.any(dim=0)]] = True
+                        side["clamped"] += int((active & (raw > amax)).sum())
                     idx = torch.arange(1, e - s + 1, dtype=torch.int32)[None, :].expand_as(active)
                     last = torch.where(active, idx, torch.zeros((), dtype=torch.int32)).max(dim=1).values
                 a_act = torch.where(active, a, torch.zeros((), dtype=dt))
@@ -422,14 +457,29 @@ def blend(mode: int, xy: torch.Tensor, conic: torch.Tensor, opacity: torch.Tenso
             if bg is not None:
                 C = C + Tf[:, None] * bg.to(dt)[None, :]
             row_tiles.append((C.reshape(y1 - y0, x1 - x0, D), (1.0 - Tf).reshape(y1 - y0, x1 - x0),
-                              last.reshape(y1 - y0, x1 - x0), tile_margin.detach().reshape(y1 - y0, x1 - x0)))
-        img_rows.append(tuple(torch.cat([r[k] for r in row_tiles], dim=1) for k in range(4)))
+                              last.reshape(y1 - y0, x1 - x0), tile_margin.detach().reshape(y1 - y0, x1 - x0),
+                              stopped.reshape(y1 - y0, x1 - x0)))
+        img_rows.append(tuple(torch.cat([r[k] for r in row_tiles], dim=1) for k in range(5)))
     img = torch.cat([r[0] for r in img_rows], dim=0)
     alpha_img = torch.cat([r[1] for r in img_rows], dim=0)
     ncontrib = torch.cat([r[2] for r in img_rows], dim=0)
     if margins is not None:
         margins.append(torch.cat([r[3] for r in img_rows], dim=0))
+    if side is not None:
+        side["stopped"] = torch.cat([r[4] for r in img_rows], dim=0)
+        side["hit_margin"] = torch.where(side["hit"], witness, side["hit_margin"])
     return img.permute(2, 0, 1), alpha_img, ncontrib
+
+
+def absgrad(abs_terms: list, n: int) -> torch.Tensor:
+    """gsplat's means2d.absgrad [n,2] from blend(side=...)["abs_terms"] after backward(): sum over pixels of |dL_pixel/dmean2d|."""
+    out = torch.zeros(n, 2, dtype=torch.float64)
+    for gid, dx, dy in abs_terms:
+        if dx.grad is not None:
+            out[:, 0].index_add_(0, gid, dx.grad.abs().sum(dim=0).to(out.dtype))
+        if dy.grad is not None:
+            out[:, 1].index_add_(0, gid, dy.grad.abs().sum(dim=0).to(out.dtype))
+    return out
 
 
 # --------------------------------------------------------------------------------------------------------------------
