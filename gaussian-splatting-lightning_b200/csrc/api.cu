@@ -41,7 +41,7 @@ using namespace b200gs;
 extern "C" {
 
 const char* b200gs_last_error(void) { return g_error; }
-int b200gs_version(void) { return 221; }
+int b200gs_version(void) { return 222; }
 int64_t b200gs_launch_count(void) { return (int64_t)g_launches.load(std::memory_order_relaxed); }
 
 int b200gs_project_fwd(const B200gsView* view, int64_t n, const float* means, const float* scales, const float* quats,
@@ -300,7 +300,7 @@ int b200gs_blend_fwd(int32_t mode, int32_t width, int32_t height, int32_t channe
     B200GS_CHECK_ARG(mode == B200GS_MODE_VANILLA || mode == B200GS_MODE_GSPLAT, "bad mode");
     B200GS_CHECK_ARG(width > 0 && height > 0, "bad size");
     B200GS_CHECK_ARG(tile_ranges && image && final_T && n_contrib, "NULL output/range pointer");
-    return launch_blend_fwd(mode, width, height, channels, tile_ranges, sorted_ids, 0, xy, conic, opacity, colors, bg, image,
+    return launch_blend_fwd(mode, width, height, channels, tile_ranges, sorted_ids, false, xy, conic, opacity, colors, bg, image,
                             pix_stride, ch_stride, final_T, n_contrib, alpha, (cudaStream_t)stream);
 }
 
@@ -311,7 +311,7 @@ int b200gs_blend_fwd_hits(int32_t mode, int32_t width, int32_t height, int32_t c
     B200GS_CHECK_ARG(mode == B200GS_MODE_VANILLA || mode == B200GS_MODE_GSPLAT, "bad mode");
     B200GS_CHECK_ARG(width > 0 && height > 0, "bad size");
     B200GS_CHECK_ARG(tile_ranges && image && final_T && n_contrib && hit_any, "NULL output/range pointer");
-    return launch_blend_fwd(mode, width, height, channels, tile_ranges, sorted_ids, 0, xy, conic, opacity, colors, bg, image,
+    return launch_blend_fwd(mode, width, height, channels, tile_ranges, sorted_ids, false, xy, conic, opacity, colors, bg, image,
                             pix_stride, ch_stride, final_T, n_contrib, alpha, (cudaStream_t)stream, hit_any);
 }
 
@@ -325,7 +325,7 @@ int b200gs_blend_bwd(int32_t mode, int32_t width, int32_t height, int32_t channe
     B200GS_CHECK_ARG(width > 0 && height > 0, "bad size");
     B200GS_CHECK_ARG(tile_ranges && final_T && n_contrib && v_image, "NULL input pointer");
     B200GS_CHECK_ARG(v_xy && v_conic && v_opacity && v_colors, "NULL output pointer");
-    return launch_blend_bwd(mode, width, height, channels, tile_ranges, sorted_ids, 0, xy, conic, opacity, colors, bg, final_T,
+    return launch_blend_bwd(mode, width, height, channels, tile_ranges, sorted_ids, false, xy, conic, opacity, colors, bg, final_T,
                             n_contrib, v_image, pix_stride, ch_stride, v_alpha, xy_scale_x, xy_scale_y, v_xy, v_conic,
                             v_opacity, v_colors, v_xy_abs, (cudaStream_t)stream);
 }
@@ -385,7 +385,8 @@ int b200gs_blend_fwd_rows(int32_t mode, int32_t width, int32_t height, const int
                           int32_t* n_contrib, float* alpha, void* stream) {
     B200GS_CHECK_ARG(mode == B200GS_MODE_VANILLA || mode == B200GS_MODE_GSPLAT, "bad mode");
     B200GS_CHECK_ARG(width > 0 && height > 0 && tile_ranges && image && final_T && n_contrib, "bad argument");
-    return launch_blend_fwd(mode, width, height, 3, tile_ranges, sorted_ids, B200GS_ROW_FLOATS, rows + B200GS_ROW_XY,
+    B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(rows) & 15u) == 0, "rows must be 16-byte aligned");
+    return launch_blend_fwd(mode, width, height, 3, tile_ranges, sorted_ids, true, rows + B200GS_ROW_XY,
                             rows + B200GS_ROW_CONIC, rows + B200GS_ROW_OPACITY, rows + B200GS_ROW_RGB, bg, image, pix_stride,
                             ch_stride, final_T, n_contrib, alpha, (cudaStream_t)stream);
 }
@@ -396,7 +397,8 @@ int b200gs_blend_bwd_rows(int32_t mode, int32_t width, int32_t height, const int
                           float* v_rows, void* stream) {
     B200GS_CHECK_ARG(mode == B200GS_MODE_VANILLA || mode == B200GS_MODE_GSPLAT, "bad mode");
     B200GS_CHECK_ARG(width > 0 && height > 0 && tile_ranges && final_T && n_contrib && v_image && v_rows, "bad argument");
-    return launch_blend_bwd(mode, width, height, 3, tile_ranges, sorted_ids, B200GS_ROW_FLOATS, rows + B200GS_ROW_XY,
+    B200GS_CHECK_ARG(((reinterpret_cast<uintptr_t>(rows) | reinterpret_cast<uintptr_t>(v_rows)) & 15u) == 0, "rows and v_rows must be 16-byte aligned");
+    return launch_blend_bwd(mode, width, height, 3, tile_ranges, sorted_ids, true, rows + B200GS_ROW_XY,
                             rows + B200GS_ROW_CONIC, rows + B200GS_ROW_OPACITY, rows + B200GS_ROW_RGB, bg, final_T, n_contrib, v_image,
                             pix_stride, ch_stride, v_alpha, grad_scale_x, grad_scale_y, v_rows + B200GS_ROW_XY, v_rows + B200GS_ROW_CONIC,
                             v_rows + B200GS_ROW_OPACITY, v_rows + B200GS_ROW_RGB, nullptr, (cudaStream_t)stream);

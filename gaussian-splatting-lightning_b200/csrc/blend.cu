@@ -15,11 +15,11 @@
 // Forward: the conic is pre-scaled by -0.5*log2(e) / -log2(e) while staging, so the per-(pixel,splat) body is
 // 5 FP32 ops + one MUFU.EX2 + compare/blend; colours are fetched (one LDS.128) only by contributing lanes.
 //
-// Backward walks each warp's list in reverse, only up to the deepest contributor of the warp.  Each pixel evaluates RB
-// consecutive list entries and keeps their 9 partial derivatives in registers; the warp then reduces them with a
-// reduce-SCATTER butterfly (halving exchanges: RB -> RB/2 -> ... -> 1 value per lane) and one lane per splat issues
-// the atomics: 32x fewer L2 atomics than the reference's per-pixel atomicAdd.
-#include <stdlib.h>
+// Backward walks each warp's list in reverse, only up to the deepest contributor of the warp.  Each pixel stores two numbers
+// per list entry (four with the absgrad side channel) in a per-warp shared-memory tile; every 16 entries the lanes switch to one entry each, sum the entry's
+// coordinate moments and colour terms over the warp's pixels and issue its atomics: one set of L2 atomics per
+// (warp, entry) instead of one per (pixel, entry).  blend_bwd_tr_kernel has the details.
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -88,11 +88,12 @@ __device__ __forceinline__ unsigned block_mask(float mx, float my, float A, floa
 
 // Staged splats live in shared memory as 48-byte records (3 x float4): one base address per splat, immediate offsets.
 //   forward : {x, y, a', b'} {c', opacity, col0, col1} {col2, col3, -, -}     (a',b',c' = conic pre-scaled by -0.5*log2e / -log2e)
-//   backward: {x, y, A, B}   {C, opacity, col0, col1}  {col2, col3, id, -}
+//   backward: the same, and the splat id in the third float4: {col2, col3, id, -}
 // Record DUMMY (index 256) has opacity 0: it fails the alpha test in every lane and pads the per-warp lists to a
 // multiple of the unroll factor, so the pixel loops are straight-line code.
 constexpr int DUMMY = BLOCK_PIX;
 constexpr int LIST_PAD = 8;
+constexpr int REC_SLAB = (BLOCK_PIX + 1) * 3;   // float4s of one staging buffer, DUMMY included
 
 // Every warp compacts the staged slab [0,top) into the ascending list of entries whose mask has its bit set.
 // my_list[LIST_PAD + k] = k-th entry; the LIST_PAD slots in front and the slots after the end hold DUMMY.
@@ -113,61 +114,148 @@ __device__ __forceinline__ int build_list(const unsigned char* __restrict__ s_ma
     return n;
 }
 
-#ifndef B200GS_FWD_MINBLOCKS
-#define B200GS_FWD_MINBLOCKS 1
-#endif
+// The tile of this CTA and the pixel of this thread, with the sample positions of the mode (gsplat samples pixel centres).
+struct TilePixel {
+    int tile, px, py;
+    bool inside;      // the pixel lies in the image
+    float pxf, pyf;   // sample position of the pixel
+    float ox, oy;     // sample position of the tile's first pixel
+    float amax;       // alpha clamp
+};
+
+template <bool GSPLAT>
+__device__ __forceinline__ TilePixel tile_pixel(int tid, int grid_x, int width, int height) {
+    TilePixel t;
+    // 1-D grid over the tiles, row-major.  (A longest-list-first order, from a counting sort of the tile counts, gained nothing in
+    // K6 or K7 and cost an extra ordering kernel — the kernels' tails are not what limits them.)
+    t.tile = (int)blockIdx.x;
+    const int tile_y = t.tile / grid_x, tile_x = t.tile - tile_y * grid_x;
+    int lx, ly;
+    pixel_of_thread(tid, lx, ly);
+    t.px = tile_x * TILE + lx;
+    t.py = tile_y * TILE + ly;
+    t.inside = (t.px < width) && (t.py < height);
+    const float off = GSPLAT ? 0.5f : 0.0f;
+    t.pxf = float(t.px) + off;
+    t.pyf = float(t.py) + off;
+    t.ox = float(tile_x * TILE) + off;
+    t.oy = float(tile_y * TILE) + off;
+    t.amax = GSPLAT ? 0.999f : 0.99f;
+    return t;
+}
+
+// Writes the staged record of splat slot i (conic pre-scaled; ID: the splat id in the third float4) and its block mask for the
+// tile at (ox, oy).
+template <int CH, bool ID>
+__device__ __forceinline__ void stage_record(float4* s_rec, unsigned char* s_mask, int i, float mx, float my, float A, float B, float C,
+                                             float o, const float (&col)[4], int id, float ox, float oy) {
+    s_rec[i * 3 + 0] = make_float4(mx, my, (-0.5f * LOG2E) * A, -LOG2E * B);
+    s_rec[i * 3 + 1] = make_float4((-0.5f * LOG2E) * C, o, col[0], col[1]);
+    if (CH > 2 || ID) s_rec[i * 3 + 2] = make_float4(col[2], col[3], ID ? __int_as_float(id) : 0.f, 0.f);
+    s_mask[i] = (unsigned char)block_mask(mx, my, A, B, C, o, ox, oy);
+}
+
+// Synchronous staging (K6 without cp.async, K7): reads splat g through the strides.  col[CH..3] stay as the caller set them (zero).
+// The outputs are the caller's locals: gathering into locals of this helper changes nvcc's instruction schedule of the 2-4 channel K6.
+template <int CH>
+__device__ __forceinline__ void gather_splat(int g, const SplatStrides& st, const float* __restrict__ xy, const float* __restrict__ conic,
+                                             const float* __restrict__ opacity, const float* __restrict__ colors, float2& m, float& A,
+                                             float& B, float& C, float& o, float (&col)[4]) {
+    m = __ldg(reinterpret_cast<const float2*>(xy + int64_t(g) * st.xs));
+    const float* cq = conic + int64_t(g) * st.cs;
+    A = __ldg(cq);
+    B = __ldg(cq + 1);
+    C = __ldg(cq + 2);
+    o = __ldg(opacity + int64_t(g) * st.os);
+#pragma unroll
+    for (int c = 0; c < CH; ++c) col[c] = __ldg(colors + int64_t(g) * st.ks + c);
+}
+
+// Composites the four list entries list[0..3] of the batch that starts at slab index `base` into the pixel.
+// HITS: also mark every splat that contributed to at least one pixel (gsplat's `means2d.has_hit_any_pixels`, read by
+// SelectiveAdam, optimizers.py:39, and exported as `acc_vis`, gsplat_v1_renderer.py:287): one byte store per (warp, contributing entry).
+template <int CH, bool GSPLAT, bool HITS>
+__device__ __forceinline__ void composite4(float& T, float& Tc, int& last, float (&C)[4], const TilePixel& t, const float4* s_rec,
+                                           const unsigned short* list, int base, const int32_t* s_gid, uint8_t* __restrict__ hit_any,
+                                           unsigned lane) {
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+        const int j = list[u];                         // entries past the list's end are DUMMY (alpha 0)
+        const float4 r0 = s_rec[j * 3 + 0];
+        const float4 r1 = s_rec[j * 3 + 1];
+        const float dx = r0.x - t.pxf, dy = r0.y - t.pyf;
+        // power * log2(e) = a' dx^2 + b' dx dy + c' dy^2
+        const float p2 = fmaf(r1.x * dy, dy, fmaf(r0.w, dy, r0.z * dx) * dx);
+        float a = fminf(t.amax, r1.y * ex2_approx(p2));
+        a = (!(p2 > 0.0f) && !(a < ALPHA_MIN)) ? a : 0.f;             // a sample that fails the alpha test composites nothing
+        // Tc is the transmittance used for compositing; it drops to exactly 0 when the pixel stops, so every later sample
+        // weighs nothing without a `done` predicate in the arithmetic; T keeps the value in front of the stopping sample
+        const float nT = fmaf(-a, Tc, Tc);
+        const bool stop = GSPLAT ? (nT <= T_STOP) : (nT < T_STOP);
+        const float w = stop ? 0.f : a * Tc;
+        C[0] = fmaf(r1.z, w, C[0]);
+        if (CH > 1) C[1] = fmaf(r1.w, w, C[1]);
+        if (CH > 2) {
+            const float2 r2 = *reinterpret_cast<const float2*>(&s_rec[j * 3 + 2]);
+            C[2] = fmaf(r2.x, w, C[2]);
+            if (CH > 3) C[3] = fmaf(r2.y, w, C[3]);
+        }
+        last = (w > 0.f) ? base + j + 1 : last;
+        T = stop ? T : nT;
+        Tc = stop ? 0.f : nT;
+        if (HITS) {
+            if (__any_sync(FULL, w > 0.f) && lane == 0) hit_any[s_gid[j]] = 1;
+        }
+    }
+}
+
+template <int CH>
+__device__ __forceinline__ void write_pixel(const TilePixel& t, float T, int last, const float (&C)[4], int width, const float* __restrict__ bg,
+                                            float* __restrict__ image, int64_t pix_stride, int64_t ch_stride, float* __restrict__ final_T,
+                                            int32_t* __restrict__ n_contrib, float* __restrict__ alpha_out) {
+    if (t.inside) {
+        const int64_t pix = int64_t(t.py) * width + t.px;
+        final_T[pix] = T;
+        n_contrib[pix] = last;
+        if (alpha_out) alpha_out[pix] = 1.0f - T;
+#pragma unroll
+        for (int c = 0; c < CH; ++c) image[pix * pix_stride + c * ch_stride] = C[c] + (bg ? T * __ldg(bg + c) : 0.f);
+    }
+}
 
 template <int CH, bool GSPLAT>
-__global__ void __launch_bounds__(BLOCK_PIX, B200GS_FWD_MINBLOCKS) blend_fwd_kernel(int width, int height, int grid_x, const int2* __restrict__ ranges,
+__global__ void __launch_bounds__(BLOCK_PIX, 1) blend_fwd_kernel(int width, int height, int grid_x, const int2* __restrict__ ranges,
                                                               const int32_t* __restrict__ ids, const SplatStrides st, const float* __restrict__ xy,
                                                               const float* __restrict__ conic, const float* __restrict__ opacity,
                                                               const float* __restrict__ colors, const float* __restrict__ bg,
                                                               float* __restrict__ image, int64_t pix_stride, int64_t ch_stride,
                                                               float* __restrict__ final_T, int32_t* __restrict__ n_contrib,
                                                               float* __restrict__ alpha_out) {
-    __shared__ float4 s_rec[(BLOCK_PIX + 1) * 3];
+    __shared__ float4 s_rec[REC_SLAB];
     __shared__ unsigned char s_mask[BLOCK_PIX];
     __shared__ unsigned short s_list[NWARP][BLOCK_PIX + 2 * LIST_PAD];
 
     const int tid = threadIdx.x;
     const int warp = tid >> 5;
     const unsigned lane = tid & 31u;
-    // 1-D grid over the tiles, row-major.  (A longest-list-first order, from a counting sort of the tile counts, gained nothing in
-    // K6 or K7 and cost an extra ordering kernel — the kernels' tails are not what limits them.)
-    const int tile = (int)blockIdx.x;
-    const int tile_y = tile / grid_x, tile_x = tile - tile_y * grid_x;
-    int lx, ly;
-    pixel_of_thread(tid, lx, ly);
-    const int px = tile_x * TILE + lx, py = tile_y * TILE + ly;
-    const bool inside = (px < width) && (py < height);
-    const float off = GSPLAT ? 0.5f : 0.0f;
-    const float pxf = float(px) + off, pyf = float(py) + off;
-    const float ox = float(tile_x * TILE) + off, oy = float(tile_y * TILE) + off;
-    const float amax = GSPLAT ? 0.999f : 0.99f;
-    if (tid < 3) s_rec[DUMMY * 3 + tid] = make_float4(0.f, 0.f, 0.f, 0.f);
-
-    const int2 range = ranges[tile];
-    int todo = range.y - range.x;
-    float T = 1.0f, Tc = inside ? 1.0f : 0.0f;     // Tc == 0: this pixel is finished (or outside the image)
     int last = 0;
     float C[4] = {0.f, 0.f, 0.f, 0.f};
+    const TilePixel t = tile_pixel<GSPLAT>(tid, grid_x, width, height);
+    if (tid < 3) s_rec[DUMMY * 3 + tid] = make_float4(0.f, 0.f, 0.f, 0.f);
+
+    const int2 range = ranges[t.tile];
+    int todo = range.y - range.x;
+    float T = 1.0f, Tc = t.inside ? 1.0f : 0.0f;     // Tc == 0: this pixel is finished (or outside the image)
 
     for (int base = 0; todo > 0; base += BLOCK_PIX, todo -= BLOCK_PIX) {
         if (__syncthreads_and(Tc == 0.0f)) break;
         const int cnt = min(BLOCK_PIX, todo);
         if (tid < cnt) {
             const int g = __ldg(ids + range.x + base + tid);
-            const float2 m = __ldg(reinterpret_cast<const float2*>(xy + int64_t(g) * st.xs));
-            const float* cq = conic + int64_t(g) * st.cs;
-            const float A = __ldg(cq), B = __ldg(cq + 1), Cc = __ldg(cq + 2);
-            const float o = __ldg(opacity + int64_t(g) * st.os);
-            float col[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-            for (int c = 0; c < CH; ++c) col[c] = __ldg(colors + int64_t(g) * st.ks + c);
-            s_rec[tid * 3 + 0] = make_float4(m.x, m.y, (-0.5f * LOG2E) * A, -LOG2E * B);
-            s_rec[tid * 3 + 1] = make_float4((-0.5f * LOG2E) * Cc, o, col[0], col[1]);
-            if (CH > 2) s_rec[tid * 3 + 2] = make_float4(col[2], col[3], 0.f, 0.f);
-            s_mask[tid] = (unsigned char)block_mask(m.x, m.y, A, B, Cc, o, ox, oy);
+            float2 m;
+            float A, B, Cc, o, col[4] = {0.f, 0.f, 0.f, 0.f};
+            gather_splat<CH>(g, st, xy, conic, opacity, colors, m, A, B, Cc, o, col);
+            stage_record<CH, false>(s_rec, s_mask, tid, m.x, m.y, A, B, Cc, o, col, g, t.ox, t.oy);
         }
         __syncthreads();
         if (__all_sync(FULL, Tc == 0.0f)) continue;  // warp finished: only keeps the block barriers company
@@ -175,42 +263,10 @@ __global__ void __launch_bounds__(BLOCK_PIX, B200GS_FWD_MINBLOCKS) blend_fwd_ker
         const int nl = build_list(s_mask, s_list[warp], cnt, warp, lane);
         for (int i0 = 0; i0 < nl; i0 += 4) {
             if (__all_sync(FULL, Tc == 0.0f)) break;
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const int j = my_list[i0 + u];                 // entries past nl are DUMMY (alpha 0)
-                const float4 r0 = s_rec[j * 3 + 0];
-                const float4 r1 = s_rec[j * 3 + 1];
-                const float dx = r0.x - pxf, dy = r0.y - pyf;
-                // power * log2(e) = a' dx^2 + b' dx dy + c' dy^2
-                const float p2 = fmaf(r1.x * dy, dy, fmaf(r0.w, dy, r0.z * dx) * dx);
-                float a = fminf(amax, r1.y * ex2_approx(p2));
-                a = (!(p2 > 0.0f) && !(a < ALPHA_MIN)) ? a : 0.f;             // a sample that fails the alpha test composites nothing
-                // Tc is the transmittance used for compositing; it drops to exactly 0 when the pixel stops, so every later sample
-                // weighs nothing without a `done` predicate in the arithmetic; T keeps the value in front of the stopping sample
-                const float nT = fmaf(-a, Tc, Tc);
-                const bool stop = GSPLAT ? (nT <= T_STOP) : (nT < T_STOP);
-                const float w = stop ? 0.f : a * Tc;
-                C[0] = fmaf(r1.z, w, C[0]);
-                if (CH > 1) C[1] = fmaf(r1.w, w, C[1]);
-                if (CH > 2) {
-                    const float2 r2 = *reinterpret_cast<const float2*>(&s_rec[j * 3 + 2]);
-                    C[2] = fmaf(r2.x, w, C[2]);
-                    if (CH > 3) C[3] = fmaf(r2.y, w, C[3]);
-                }
-                last = (w > 0.f) ? base + j + 1 : last;
-                T = stop ? T : nT;
-                Tc = stop ? 0.f : nT;
-            }
+            composite4<CH, GSPLAT, false>(T, Tc, last, C, t, s_rec, my_list + i0, base, nullptr, nullptr, lane);
         }
     }
-    if (inside) {
-        const int64_t pix = int64_t(py) * width + px;
-        final_T[pix] = T;
-        n_contrib[pix] = last;
-        if (alpha_out) alpha_out[pix] = 1.0f - T;
-#pragma unroll
-        for (int c = 0; c < CH; ++c) image[pix * pix_stride + c * ch_stride] = C[c] + (bg ? T * __ldg(bg + c) : 0.f);
-    }
+    write_pixel<CH>(t, T, last, C, width, bg, image, pix_stride, ch_stride, final_T, n_contrib, alpha_out);
 }
 
 // ---- forward with asynchronous slab staging -----------------------------------------------------------------------------
@@ -260,8 +316,7 @@ __device__ __forceinline__ void stage_async(float4* slot, int g, const SplatStri
     }
 }
 
-// HITS: also mark every splat that contributed to at least one pixel (gsplat's `means2d.has_hit_any_pixels`, read by
-// SelectiveAdam, optimizers.py:39, and exported as `acc_vis`, gsplat_v1_renderer.py:287): one byte store per (warp, contributing entry).
+// ROWS: the splats are [n,12] rows (CH == 3); HITS: also fill hit_any (see composite4).
 template <int CH, bool GSPLAT, bool ROWS, bool HITS>
 __global__ void __launch_bounds__(BLOCK_PIX, 3) blend_fwd_async_kernel(int width, int height, int grid_x, const int2* __restrict__ ranges,
                                                               const int32_t* __restrict__ ids, const SplatStrides st, const float* __restrict__ xy,
@@ -270,7 +325,7 @@ __global__ void __launch_bounds__(BLOCK_PIX, 3) blend_fwd_async_kernel(int width
                                                               float* __restrict__ image, int64_t pix_stride, int64_t ch_stride,
                                                               float* __restrict__ final_T, int32_t* __restrict__ n_contrib,
                                                               float* __restrict__ alpha_out, uint8_t* __restrict__ hit_any) {
-    __shared__ float4 s_buf[2][(BLOCK_PIX + 1) * 3];
+    __shared__ float4 s_buf[2][REC_SLAB];
     __shared__ int32_t s_gid[HITS ? BLOCK_PIX + 1 : 1];
     __shared__ unsigned char s_mask[BLOCK_PIX];
     __shared__ unsigned short s_list[NWARP][BLOCK_PIX + 2 * LIST_PAD];
@@ -278,23 +333,14 @@ __global__ void __launch_bounds__(BLOCK_PIX, 3) blend_fwd_async_kernel(int width
     const int tid = threadIdx.x;
     const int warp = tid >> 5;
     const unsigned lane = tid & 31u;
-    const int tile = (int)blockIdx.x;
-    const int tile_y = tile / grid_x, tile_x = tile - tile_y * grid_x;
-    int lx, ly;
-    pixel_of_thread(tid, lx, ly);
-    const int px = tile_x * TILE + lx, py = tile_y * TILE + ly;
-    const bool inside = (px < width) && (py < height);
-    const float off = GSPLAT ? 0.5f : 0.0f;
-    const float pxf = float(px) + off, pyf = float(py) + off;
-    const float ox = float(tile_x * TILE) + off, oy = float(tile_y * TILE) + off;
-    const float amax = GSPLAT ? 0.999f : 0.99f;
-    if (tid < 6) s_buf[tid / 3][DUMMY * 3 + tid % 3] = make_float4(0.f, 0.f, 0.f, 0.f);
-
-    const int2 range = ranges[tile];
-    const int total = range.y - range.x;
-    float T = 1.0f, Tc = inside ? 1.0f : 0.0f;
     int last = 0;
     float C[4] = {0.f, 0.f, 0.f, 0.f};
+    const TilePixel t = tile_pixel<GSPLAT>(tid, grid_x, width, height);
+    if (tid < 6) s_buf[tid / 3][DUMMY * 3 + tid % 3] = make_float4(0.f, 0.f, 0.f, 0.f);
+
+    const int2 range = ranges[t.tile];
+    const int total = range.y - range.x;
+    float T = 1.0f, Tc = t.inside ? 1.0f : 0.0f;     // Tc == 0: this pixel is finished (or outside the image)
 
     // prologue: batch 0 in flight, ids of batch 1 in a register
     int cur_id = (tid < total) ? __ldg(ids + range.x + tid) : 0;
@@ -309,13 +355,13 @@ __global__ void __launch_bounds__(BLOCK_PIX, 3) blend_fwd_async_kernel(int width
         float4* s_rec = s_buf[buf];
         if (tid < cnt) {
             const float4 q0 = s_rec[tid * 3 + 0], q1 = s_rec[tid * 3 + 1], q2 = s_rec[tid * 3 + 2];
-            float mx, my, A, B, Cc, o, c0, c1, c2, c3;
-            if (ROWS) { mx = q0.x; my = q0.y; A = q0.w; B = q1.x; Cc = q1.y; o = q1.w; c0 = q2.x; c1 = q2.y; c2 = q2.z; c3 = 0.f; }
-            else      { mx = q0.x; my = q0.y; A = q0.z; B = q0.w; Cc = q1.x; o = q1.y; c0 = q1.z; c1 = q1.w; c2 = q2.x; c3 = q2.y; }
-            s_rec[tid * 3 + 0] = make_float4(mx, my, (-0.5f * LOG2E) * A, -LOG2E * B);
-            s_rec[tid * 3 + 1] = make_float4((-0.5f * LOG2E) * Cc, o, c0, CH > 1 ? c1 : 0.f);
-            if (CH > 2) s_rec[tid * 3 + 2] = make_float4(c2, CH > 3 ? c3 : 0.f, 0.f, 0.f);
-            s_mask[tid] = (unsigned char)block_mask(mx, my, A, B, Cc, o, ox, oy);
+            if (ROWS) {
+                const float col[4] = {q2.x, q2.y, q2.z, 0.f};
+                stage_record<CH, false>(s_rec, s_mask, tid, q0.x, q0.y, q0.w, q1.x, q1.y, q1.w, col, cur_id, t.ox, t.oy);
+            } else {
+                const float col[4] = {q1.z, CH > 1 ? q1.w : 0.f, q2.x, CH > 3 ? q2.y : 0.f};
+                stage_record<CH, false>(s_rec, s_mask, tid, q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, col, cur_id, t.ox, t.oy);
+            }
             if (HITS) s_gid[tid] = cur_id;
         }
         cur_id = next_id;
@@ -329,43 +375,11 @@ __global__ void __launch_bounds__(BLOCK_PIX, 3) blend_fwd_async_kernel(int width
         const int nl = build_list(s_mask, s_list[warp], cnt, warp, lane);
         for (int i0 = 0; i0 < nl; i0 += 4) {
             if (__all_sync(FULL, Tc == 0.0f)) break;
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const int j = my_list[i0 + u];                 // entries past nl are DUMMY (alpha 0)
-                const float4 r0 = s_rec[j * 3 + 0];
-                const float4 r1 = s_rec[j * 3 + 1];
-                const float dx = r0.x - pxf, dy = r0.y - pyf;
-                const float p2 = fmaf(r1.x * dy, dy, fmaf(r0.w, dy, r0.z * dx) * dx);
-                float a = fminf(amax, r1.y * ex2_approx(p2));
-                a = (!(p2 > 0.0f) && !(a < ALPHA_MIN)) ? a : 0.f;
-                const float nT = fmaf(-a, Tc, Tc);             // same arithmetic as blend_fwd_kernel: see there
-                const bool stop = GSPLAT ? (nT <= T_STOP) : (nT < T_STOP);
-                const float w = stop ? 0.f : a * Tc;
-                C[0] = fmaf(r1.z, w, C[0]);
-                if (CH > 1) C[1] = fmaf(r1.w, w, C[1]);
-                if (CH > 2) {
-                    const float2 r2 = *reinterpret_cast<const float2*>(&s_rec[j * 3 + 2]);
-                    C[2] = fmaf(r2.x, w, C[2]);
-                    if (CH > 3) C[3] = fmaf(r2.y, w, C[3]);
-                }
-                last = (w > 0.f) ? base + j + 1 : last;
-                T = stop ? T : nT;
-                Tc = stop ? 0.f : nT;
-                if (HITS) {
-                    if (__any_sync(FULL, w > 0.f) && lane == 0) hit_any[s_gid[j]] = 1;
-                }
-            }
+            composite4<CH, GSPLAT, HITS>(T, Tc, last, C, t, s_rec, my_list + i0, base, s_gid, hit_any, lane);
         }
     }
     cp_async_wait_all();
-    if (inside) {
-        const int64_t pix = int64_t(py) * width + px;
-        final_T[pix] = T;
-        n_contrib[pix] = last;
-        if (alpha_out) alpha_out[pix] = 1.0f - T;
-#pragma unroll
-        for (int c = 0; c < CH; ++c) image[pix * pix_stride + c * ch_stride] = C[c] + (bg ? T * __ldg(bg + c) : 0.f);
-    }
+    write_pixel<CH>(t, T, last, C, width, bg, image, pix_stride, ch_stride, final_T, n_contrib, alpha_out);
 }
 
 // ---- backward: transpose-reduce --------------------------------------------------------------------------------------------
@@ -391,7 +405,7 @@ template <bool ABS>
 struct TrSmem {
     static constexpr int VAL_BYTES = ABS ? 16 : 8;              // per (entry, pixel): {go, fac} or {go, fac, |gx|, |gy|}
     static constexpr int VAL_ROW = 32 * VAL_BYTES + 16;         // bytes per entry row of the value tile (+ pad)
-    float4 rec[(BLOCK_PIX + 1) * 3];
+    float4 rec[REC_SLAB];
     float4 vo[NWARP][33];                                        // v_image of the warp's pixels; pixel p at slot p + (p >> 4): the two halves
                                                                  // of a warp read different banks in the same instruction
     unsigned char val[NWARP][GE * VAL_ROW];
@@ -424,31 +438,22 @@ __global__ void __launch_bounds__(BLOCK_PIX, ABS ? 3 : 4) blend_bwd_tr_kernel(in
     const int tid = threadIdx.x;
     const int warp = tid >> 5;
     const unsigned lane = tid & 31u;
-    const int tile = (int)blockIdx.x;
-    const int tile_y = tile / grid_x, tile_x = tile - tile_y * grid_x;
-    int lx, ly;
-    pixel_of_thread(tid, lx, ly);
-    const int px = tile_x * TILE + lx, py = tile_y * TILE + ly;
-    const bool inside = (px < width) && (py < height);
-    const float off = GSPLAT ? 0.5f : 0.0f;
-    const float pxf = float(px) + off, pyf = float(py) + off;
-    const float ox = float(tile_x * TILE) + off, oy = float(tile_y * TILE) + off;
-    const float amax = GSPLAT ? 0.999f : 0.99f;
-    const int64_t pix = int64_t(py) * width + px;
+    const TilePixel t = tile_pixel<GSPLAT>(tid, grid_x, width, height);
+    const int64_t pix = int64_t(t.py) * width + t.px;
     if (tid < 3) s_rec[DUMMY * 3 + tid] = make_float4(0.f, 0.f, 0.f, 0.f);
 
-    const int2 range = ranges[tile];
-    const float Tf = inside ? final_T[pix] : 0.f;
-    const int last = inside ? n_contrib[pix] : 0;
+    const int2 range = ranges[t.tile];
+    const float Tf = t.inside ? final_T[pix] : 0.f;
+    const int last = t.inside ? n_contrib[pix] : 0;
     float vo[4] = {0.f, 0.f, 0.f, 0.f};
     float bg_dot = 0.f;
 #pragma unroll
     for (int c = 0; c < CH; ++c) {
-        vo[c] = inside ? __ldg(v_image + pix * pix_stride + c * ch_stride) : 0.f;
+        vo[c] = t.inside ? __ldg(v_image + pix * pix_stride + c * ch_stride) : 0.f;
         if (bg) bg_dot += __ldg(bg + c) * vo[c];
     }
     sm.vo[warp][lane + (lane >> 4)] = make_float4(vo[0], vo[1], vo[2], vo[3]);
-    const float va = (v_alpha && inside) ? __ldg(v_alpha + pix) : 0.f;
+    const float va = (v_alpha && t.inside) ? __ldg(v_alpha + pix) : 0.f;
     const float tail = Tf * (va - bg_dot);  // d(out)/d(alpha_i) through everything behind the last contributor
 
     const int wmax = __reduce_max_sync(FULL, last);
@@ -466,7 +471,7 @@ __global__ void __launch_bounds__(BLOCK_PIX, ABS ? 3 : 4) blend_bwd_tr_kernel(in
     const float4* my_row = reinterpret_cast<const float4*>(sm.val[warp] + re * VAL_ROW + rh * 16 * VAL_BYTES);
     const float4* my_vo = sm.vo[warp] + rh * 17;
     // origin of the warp's 8x4 block of pixel samples; the reduce lane's pixels are rows 2 rh, 2 rh + 1 of it
-    const float bx0 = ox + float((warp & 1) << 3), by0 = oy + float((warp >> 1) << 2);
+    const float bx0 = t.ox + float((warp & 1) << 3), by0 = t.oy + float((warp >> 1) << 2);
     const float hh = float(2 * rh);
 
     for (int hi = max_last; hi > 0; hi -= BLOCK_PIX) {
@@ -475,17 +480,10 @@ __global__ void __launch_bounds__(BLOCK_PIX, ABS ? 3 : 4) blend_bwd_tr_kernel(in
         __syncthreads();
         if (tid < cnt) {
             const int g = __ldg(ids + range.x + lo + tid);
-            const float2 m = __ldg(reinterpret_cast<const float2*>(xy + int64_t(g) * st.xs));
-            const float* cq = conic + int64_t(g) * st.cs;
-            const float A = __ldg(cq), B = __ldg(cq + 1), Cc = __ldg(cq + 2);
-            const float o = __ldg(opacity + int64_t(g) * st.os);
-            float col[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-            for (int c = 0; c < CH; ++c) col[c] = __ldg(colors + int64_t(g) * st.ks + c);
-            s_rec[tid * 3 + 0] = make_float4(m.x, m.y, (-0.5f * LOG2E) * A, -LOG2E * B);
-            s_rec[tid * 3 + 1] = make_float4((-0.5f * LOG2E) * Cc, o, col[0], col[1]);
-            s_rec[tid * 3 + 2] = make_float4(col[2], col[3], __int_as_float(g), 0.f);
-            sm.mask[tid] = (unsigned char)block_mask(m.x, m.y, A, B, Cc, o, ox, oy);
+            float2 m;
+            float A, B, Cc, o, col[4] = {0.f, 0.f, 0.f, 0.f};
+            gather_splat<CH>(g, st, xy, conic, opacity, colors, m, A, B, Cc, o, col);
+            stage_record<CH, true>(s_rec, sm.mask, tid, m.x, m.y, A, B, Cc, o, col, g, t.ox, t.oy);
         }
         __syncthreads();
         if (wmax <= lo) continue;  // this warp has no contributor in the batch
@@ -499,12 +497,12 @@ __global__ void __launch_bounds__(BLOCK_PIX, ABS ? 3 : 4) blend_bwd_tr_kernel(in
                 const int j = my_list[ii - u];
                 const float4 r0 = s_rec[j * 3 + 0];
                 const float4 r1 = s_rec[j * 3 + 1];
-                const float dx = r0.x - pxf, dy = r0.y - pyf;
+                const float dx = r0.x - t.pxf, dy = r0.y - t.pyf;
                 // same arithmetic as the forward: power * log2(e) = a' dx^2 + b' dx dy + c' dy^2
                 const float p2 = fmaf(r1.x * dy, dy, fmaf(r0.w, dy, r0.z * dx) * dx);
                 const float G = ex2_approx(p2);
                 const float oG = r1.y * G;
-                const float a = fminf(amax, oG);
+                const float a = fminf(t.amax, oG);
                 const bool valid = (j < rel_last) && !(p2 > 0.0f) && (a >= ALPHA_MIN);
                 float go = 0.f, fac = 0.f, gax = 0.f, gay = 0.f;
                 if (valid) {
@@ -626,138 +624,117 @@ __global__ void __launch_bounds__(BLOCK_PIX, ABS ? 3 : 4) blend_bwd_tr_kernel(in
     }
 }
 
+// Strides of the splat columns (and of the gradient columns in the backward): one [n,12] row buffer, or separate arrays.
 template <int CH>
-int fwd_dispatch(int mode, int width, int height, const int32_t* ranges, const int32_t* ids, int row_stride, const float* xy, const float* conic,
+SplatStrides splat_strides(bool rows) {
+    return rows ? SplatStrides{B200GS_ROW_FLOATS, B200GS_ROW_FLOATS, B200GS_ROW_FLOATS, B200GS_ROW_FLOATS} : SplatStrides{2, 3, 1, CH};
+}
+
+// Two stagings of the tile slab.  Synchronous: ids -> gathered records -> registers -> shared memory, the latency covered by the other
+// CTAs of the SM.  Asynchronous: cp.async (LDGSTS) double buffer.  At 1 M Gaussians / 1080p the asynchronous kernel only wins
+// when capped at 80 registers (3 blocks per SM) and reading [n,12] rows (3 x 16 B); at 81 registers (2 blocks per SM) it lost,
+// so the asynchronous staging serves the row layout (what the fused renderers and the sharded renderer use) and the
+// has_hit_any_pixels variant; the separate-array layout (eight 4/8-byte LDGSTS per splat) stays synchronous.
+template <int CH, bool GSPLAT>
+int fwd_dispatch(bool rows, int width, int height, const int32_t* ranges, const int32_t* ids, const float* xy, const float* conic,
                  const float* opacity, const float* colors, const float* bg, float* image, int64_t ps, int64_t cs, float* final_T,
                  int32_t* n_contrib, float* alpha, uint8_t* hit_any, cudaStream_t s) {
-    const int gx = div_up(width, TILE), gy = div_up(height, TILE);
-    dim3 grid(gx * gy);
-    const SplatStrides st = row_stride > 0 ? SplatStrides{row_stride, row_stride, row_stride, row_stride} : SplatStrides{2, 3, 1, CH};
-    // Two stagings of the tile slab.  Synchronous: ids -> gathered records -> registers -> shared memory, the latency covered by the other
-    // CTAs of the SM.  Asynchronous: cp.async (LDGSTS) double buffer.  At 1 M Gaussians / 1080p the asynchronous kernel only wins
-    // when capped at 80 registers (3 blocks per SM) and reading [n,12] rows (3 x 16 B); at 81 registers (2 blocks per SM) it lost,
-    // so the asynchronous staging is the default for the row layout (what the fused renderers and the sharded renderer use) and for the
-    // has_hit_any_pixels variant; the separate-array layout (eight 4/8-byte LDGSTS per splat) stays synchronous.
-    // B200GS_FWD_ASYNC=1 / =0 forces one or the other everywhere.
-    static const int async_env = []() { const char* e = getenv("B200GS_FWD_ASYNC"); return (e && e[0] == '1') ? 1 : (e && e[0] == '0') ? 0 : -1; }();
-    // the row layout is [x, y, depth, A, B, C, comp, opacity, r, g, b, radius] (include/b200gs.h); 16-byte copies need 16-byte aligned rows
-    const bool rows16 = row_stride == 12 && CH == 3 && conic == xy + 3 && opacity == xy + 7 && colors == xy + 8 && (reinterpret_cast<uintptr_t>(xy) & 15) == 0;
-    const bool use_async = async_env == 1 || (async_env == -1 && rows16);
-    if (use_async || hit_any != nullptr) {
-#define B200GS_FWD_ARGS width, height, gx, (const int2*)ranges, ids, st, xy, conic, opacity, colors, bg, image, ps, cs, final_T, n_contrib, alpha, hit_any
-#define B200GS_FWD_LAUNCH(G, R)                                                                                                   \
-    do {                                                                                                                           \
-        if (hit_any) blend_fwd_async_kernel<CH, G, R, true><<<grid, BLOCK_PIX, 0, s>>>(B200GS_FWD_ARGS);                          \
-        else blend_fwd_async_kernel<CH, G, R, false><<<grid, BLOCK_PIX, 0, s>>>(B200GS_FWD_ARGS);                                 \
-    } while (0)
-        if (rows16) {
-            if constexpr (CH == 3) {
-                if (mode == B200GS_MODE_GSPLAT) B200GS_FWD_LAUNCH(true, true);
-                else B200GS_FWD_LAUNCH(false, true);
-            }
-        } else {
-            if (mode == B200GS_MODE_GSPLAT) B200GS_FWD_LAUNCH(true, false);
-            else B200GS_FWD_LAUNCH(false, false);
-        }
-#undef B200GS_FWD_LAUNCH
-#undef B200GS_FWD_ARGS
-        B200GS_LAUNCH_CHECK();
-        return B200GS_OK;
+    const int gx = div_up(width, TILE);
+    const dim3 grid(gx * div_up(height, TILE));
+    const SplatStrides st = splat_strides<CH>(rows);
+    const auto launch = [&](auto kernel, auto... hit_any_arg) {   // the asynchronous kernels take hit_any last
+        kernel<<<grid, BLOCK_PIX, 0, s>>>(width, height, gx, reinterpret_cast<const int2*>(ranges), ids, st, xy, conic, opacity, colors, bg,
+                                          image, ps, cs, final_T, n_contrib, alpha, hit_any_arg...);
+    };
+    if (hit_any) {
+        launch(blend_fwd_async_kernel<CH, GSPLAT, false, true>, hit_any);
+    } else if (!rows) {
+        launch(blend_fwd_kernel<CH, GSPLAT>);
+    } else if constexpr (CH == 3) {
+        // three 16-byte copies per row: the entry point checks that the rows are 16-byte aligned
+        launch(blend_fwd_async_kernel<3, GSPLAT, true, false>, hit_any);
+    } else {
+        set_error("blend_fwd: [n,12] rows carry 3 colour channels, not %d", CH);
+        return B200GS_EINVAL;
     }
-    if (mode == B200GS_MODE_GSPLAT)
-        blend_fwd_kernel<CH, true><<<grid, BLOCK_PIX, 0, s>>>(width, height, gx, (const int2*)ranges, ids, st, xy, conic,
-                                                              opacity, colors, bg, image, ps, cs, final_T, n_contrib, alpha);
-    else
-        blend_fwd_kernel<CH, false><<<grid, BLOCK_PIX, 0, s>>>(width, height, gx, (const int2*)ranges, ids, st, xy, conic,
-                                                               opacity, colors, bg, image, ps, cs, final_T, n_contrib, alpha);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-template <int CH>
-int bwd_dispatch(int mode, int width, int height, const int32_t* ranges, const int32_t* ids, int row_stride, const float* xy, const float* conic,
-                 const float* opacity, const float* colors, const float* bg, const float* final_T, const int32_t* n_contrib,
-                 const float* v_image, int64_t ps, int64_t cs, const float* v_alpha, float sx, float sy, float* v_xy,
-                 float* v_conic, float* v_opacity, float* v_colors, float* v_xy_abs, cudaStream_t s) {
-    const int gx = div_up(width, TILE), gy = div_up(height, TILE);
-    dim3 grid(gx * gy);
-    const SplatStrides st = row_stride > 0 ? SplatStrides{row_stride, row_stride, row_stride, row_stride} : SplatStrides{2, 3, 1, CH};
-    // gradient outputs that are the columns of one 16-byte aligned [n,12] row buffer leave as 128-bit reductions
-    const bool vrows = CH == 3 && row_stride == B200GS_ROW_FLOATS && v_conic == v_xy + B200GS_ROW_CONIC && v_opacity == v_xy + B200GS_ROW_OPACITY &&
-                       v_colors == v_xy + B200GS_ROW_RGB && (reinterpret_cast<uintptr_t>(v_xy) & 15) == 0;
-#define B200GS_BWD_ARGS width, height, gx, (const int2*)ranges, ids, st, xy, conic, opacity, colors, bg, final_T, n_contrib, \
-                        v_image, ps, cs, v_alpha, sx, sy, v_xy, v_conic, v_opacity, v_colors, v_xy_abs
-    static const cudaError_t attr_rc = []() {
-        cudaError_t e = cudaSuccess;
-        auto set = [&e](const void* f, size_t bytes) {
-            if (e == cudaSuccess) e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-            if (e == cudaSuccess) e = cudaFuncSetAttribute(f, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-        };
-        set((const void*)blend_bwd_tr_kernel<CH, true, false, false>, sizeof(TrSmem<false>));
-        set((const void*)blend_bwd_tr_kernel<CH, false, false, false>, sizeof(TrSmem<false>));
-        set((const void*)blend_bwd_tr_kernel<CH, true, true, false>, sizeof(TrSmem<true>));
-        set((const void*)blend_bwd_tr_kernel<CH, false, true, false>, sizeof(TrSmem<true>));
-        if constexpr (CH == 3) {
-            set((const void*)blend_bwd_tr_kernel<CH, true, false, true>, sizeof(TrSmem<false>));
-            set((const void*)blend_bwd_tr_kernel<CH, false, false, true>, sizeof(TrSmem<false>));
-            set((const void*)blend_bwd_tr_kernel<CH, true, true, true>, sizeof(TrSmem<true>));
-            set((const void*)blend_bwd_tr_kernel<CH, false, true, true>, sizeof(TrSmem<true>));
-        }
+// Launches K7 instantiation <CH, GSPLAT, ABS, VROWS>.  Its first launch also sets the kernel's dynamic shared-memory limit.
+template <int CH, bool GSPLAT, bool ABS, bool VROWS, typename... Args>
+int bwd_launch(dim3 grid, cudaStream_t s, Args... args) {
+    const auto kernel = blend_bwd_tr_kernel<CH, GSPLAT, ABS, VROWS>;
+    static const cudaError_t attr_rc = [kernel]() {
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TrSmem<ABS>));
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
         return e;
     }();
     if (attr_rc != cudaSuccess) {
         set_error("blend_bwd: cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_rc));
         return B200GS_ECUDA;
     }
-#define B200GS_BWD_LAUNCH(G, A, V) blend_bwd_tr_kernel<CH, G, A, V><<<grid, BLOCK_PIX, sizeof(TrSmem<A>), s>>>(B200GS_BWD_ARGS)
-    const bool gs = mode == B200GS_MODE_GSPLAT, ab = v_xy_abs != nullptr;
-    if (vrows) {
-        if constexpr (CH == 3) {
-            if (gs) { if (ab) B200GS_BWD_LAUNCH(true, true, true); else B200GS_BWD_LAUNCH(true, false, true); }
-            else    { if (ab) B200GS_BWD_LAUNCH(false, true, true); else B200GS_BWD_LAUNCH(false, false, true); }
-        }
-    } else {
-        if (gs) { if (ab) B200GS_BWD_LAUNCH(true, true, false); else B200GS_BWD_LAUNCH(true, false, false); }
-        else    { if (ab) B200GS_BWD_LAUNCH(false, true, false); else B200GS_BWD_LAUNCH(false, false, false); }
-    }
-#undef B200GS_BWD_LAUNCH
-#undef B200GS_BWD_ARGS
+    kernel<<<grid, BLOCK_PIX, sizeof(TrSmem<ABS>), s>>>(args...);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
+template <int CH, bool GSPLAT>
+int bwd_dispatch(bool rows, int width, int height, const int32_t* ranges, const int32_t* ids, const float* xy, const float* conic,
+                 const float* opacity, const float* colors, const float* bg, const float* final_T, const int32_t* n_contrib,
+                 const float* v_image, int64_t ps, int64_t cs, const float* v_alpha, float sx, float sy, float* v_xy,
+                 float* v_conic, float* v_opacity, float* v_colors, float* v_xy_abs, cudaStream_t s) {
+    const int gx = div_up(width, TILE);
+    const dim3 grid(gx * div_up(height, TILE));
+    const SplatStrides st = splat_strides<CH>(rows);
+    const auto launch = [&](auto abs, auto vrows) {
+        return bwd_launch<CH, GSPLAT, decltype(abs)::value, decltype(vrows)::value>(
+            grid, s, width, height, gx, reinterpret_cast<const int2*>(ranges), ids, st, xy, conic, opacity, colors, bg, final_T, n_contrib,
+            v_image, ps, cs, v_alpha, sx, sy, v_xy, v_conic, v_opacity, v_colors, v_xy_abs);
+    };
+    if (v_xy_abs) return launch(std::true_type{}, std::false_type{});
+    if (!rows) return launch(std::false_type{}, std::false_type{});
+    if constexpr (CH == 3) {
+        // 128-bit reductions into the gradient rows: the entry point checks that they are 16-byte aligned
+        return launch(std::false_type{}, std::true_type{});
+    } else {
+        set_error("blend_bwd: [n,12] rows carry 3 colour channels, not %d", CH);
+        return B200GS_EINVAL;
+    }
+}
+
 }  // namespace
 
-int launch_blend_fwd(int mode, int width, int height, int channels, const int32_t* ranges, const int32_t* ids, int row_stride, const float* xy,
+int launch_blend_fwd(int mode, int width, int height, int channels, const int32_t* ranges, const int32_t* ids, bool rows, const float* xy,
                      const float* conic, const float* opacity, const float* colors, const float* bg, float* image,
                      int64_t pix_stride, int64_t ch_stride, float* final_T, int32_t* n_contrib, float* alpha, cudaStream_t s,
                      uint8_t* hit_any) {
-    switch (channels) {
-        case 1: return fwd_dispatch<1>(mode, width, height, ranges, ids, row_stride, xy, conic, opacity, colors, bg, image, pix_stride, ch_stride, final_T, n_contrib, alpha, hit_any, s);
-        case 2: return fwd_dispatch<2>(mode, width, height, ranges, ids, row_stride, xy, conic, opacity, colors, bg, image, pix_stride, ch_stride, final_T, n_contrib, alpha, hit_any, s);
-        case 3: return fwd_dispatch<3>(mode, width, height, ranges, ids, row_stride, xy, conic, opacity, colors, bg, image, pix_stride, ch_stride, final_T, n_contrib, alpha, hit_any, s);
-        case 4: return fwd_dispatch<4>(mode, width, height, ranges, ids, row_stride, xy, conic, opacity, colors, bg, image, pix_stride, ch_stride, final_T, n_contrib, alpha, hit_any, s);
+    static constexpr decltype(&fwd_dispatch<1, false>) by_channels[4][2] = {
+        {fwd_dispatch<1, false>, fwd_dispatch<1, true>}, {fwd_dispatch<2, false>, fwd_dispatch<2, true>},
+        {fwd_dispatch<3, false>, fwd_dispatch<3, true>}, {fwd_dispatch<4, false>, fwd_dispatch<4, true>}};
+    if (channels < 1 || channels > 4) {
+        set_error("blend_fwd: unsupported channel count %d (1..4)", channels);
+        return B200GS_EINVAL;
     }
-    set_error("blend_fwd: unsupported channel count %d (1..4)", channels);
-    return B200GS_EINVAL;
+    return by_channels[channels - 1][mode == B200GS_MODE_GSPLAT](rows, width, height, ranges, ids, xy, conic, opacity, colors, bg, image,
+                                                                  pix_stride, ch_stride, final_T, n_contrib, alpha, hit_any, s);
 }
 
-int launch_blend_bwd(int mode, int width, int height, int channels, const int32_t* ranges, const int32_t* ids, int row_stride, const float* xy,
+int launch_blend_bwd(int mode, int width, int height, int channels, const int32_t* ranges, const int32_t* ids, bool rows, const float* xy,
                      const float* conic, const float* opacity, const float* colors, const float* bg, const float* final_T,
                      const int32_t* n_contrib, const float* v_image, int64_t pix_stride, int64_t ch_stride, const float* v_alpha,
                      float sx, float sy, float* v_xy, float* v_conic, float* v_opacity, float* v_colors, float* v_xy_abs,
                      cudaStream_t s) {
-#define B200GS_BWD_CALL(C) bwd_dispatch<C>(mode, width, height, ranges, ids, row_stride, xy, conic, opacity, colors, bg, final_T, n_contrib, v_image, \
-                                           pix_stride, ch_stride, v_alpha, sx, sy, v_xy, v_conic, v_opacity, v_colors, v_xy_abs, s)
-    switch (channels) {
-        case 1: return B200GS_BWD_CALL(1);
-        case 2: return B200GS_BWD_CALL(2);
-        case 3: return B200GS_BWD_CALL(3);
-        case 4: return B200GS_BWD_CALL(4);
+    static constexpr decltype(&bwd_dispatch<1, false>) by_channels[4][2] = {
+        {bwd_dispatch<1, false>, bwd_dispatch<1, true>}, {bwd_dispatch<2, false>, bwd_dispatch<2, true>},
+        {bwd_dispatch<3, false>, bwd_dispatch<3, true>}, {bwd_dispatch<4, false>, bwd_dispatch<4, true>}};
+    if (channels < 1 || channels > 4) {
+        set_error("blend_bwd: unsupported channel count %d (1..4)", channels);
+        return B200GS_EINVAL;
     }
-#undef B200GS_BWD_CALL
-    set_error("blend_bwd: unsupported channel count %d (1..4)", channels);
-    return B200GS_EINVAL;
+    return by_channels[channels - 1][mode == B200GS_MODE_GSPLAT](rows, width, height, ranges, ids, xy, conic, opacity, colors, bg, final_T,
+                                                                  n_contrib, v_image, pix_stride, ch_stride, v_alpha, sx, sy, v_xy, v_conic,
+                                                                  v_opacity, v_colors, v_xy_abs, s);
 }
 
 }  // namespace b200gs

@@ -129,12 +129,13 @@ int launch_loss_fwd(int channels, int width, int height, const float* img, const
 int launch_loss_bwd(int channels, int width, int height, const float* img, const float* gt, const float* dmaps, float lambda_dssim,
                     const float* v_loss, float* v_img, cudaStream_t s);
 
+// rows: xy, conic, opacity and colors (and the gradient outputs) are columns of 16-byte aligned [n,12] row buffers, channels == 3
 int launch_blend_fwd(int mode, int width, int height, int channels, const int32_t* ranges, const int32_t* ids,
-                     int row_stride, const float* xy, const float* conic, const float* opacity, const float* colors, const float* bg,
+                     bool rows, const float* xy, const float* conic, const float* opacity, const float* colors, const float* bg,
                      float* image, int64_t pix_stride, int64_t ch_stride, float* final_T, int32_t* n_contrib,
                      float* alpha, cudaStream_t s, uint8_t* hit_any = nullptr);
 int launch_blend_bwd(int mode, int width, int height, int channels, const int32_t* ranges, const int32_t* ids,
-                     int row_stride, const float* xy, const float* conic, const float* opacity, const float* colors, const float* bg,
+                     bool rows, const float* xy, const float* conic, const float* opacity, const float* colors, const float* bg,
                      const float* final_T, const int32_t* n_contrib, const float* v_image, int64_t pix_stride,
                      int64_t ch_stride, const float* v_alpha, float sx, float sy, float* v_xy, float* v_conic,
                      float* v_opacity, float* v_colors, float* v_xy_abs, cudaStream_t s);

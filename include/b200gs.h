@@ -223,7 +223,9 @@ B200GS_API int b200gs_loss_bwd(int32_t channels, int32_t width, int32_t height, 
  *     = the row of entry i, kept for the backward; *d_count <- number of rows.
  * b200gs_bin_count_rows (then b200gs_bin_sort) / blend_fwd_rows / blend_bwd_rows: K2-K7 reading the rows IN PLACE (strided
  *     access, no split copies); blend_bwd_rows accumulates into a zero-filled [n,12] gradient row buffer that goes
- *     straight back through the all-to-all.  3 colour channels; cull != 0 enables exact tile culling. */
+ *     straight back through the all-to-all.  3 colour channels; cull != 0 enables exact tile culling.
+ *     blend_fwd_rows / blend_bwd_rows read rows (and blend_bwd_rows accumulates into v_rows) with 16-byte accesses: both buffers
+ *     must be 16-byte aligned (an allocation base is), or the call fails with B200GS_EINVAL. */
 #define B200GS_MAX_VIEWS 8      /* cameras per multi-view launch / destination ranks per peer-mode pack (one NVSwitch box) */
 #define B200GS_ROW_FLOATS 12
 #define B200GS_ROW_XY 0

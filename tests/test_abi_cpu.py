@@ -64,6 +64,13 @@ def test_argument_validation_without_gpu(lib):
     assert b"sh_stride" in L.b200gs_last_error()
     # unsupported channel count / bad image size in the blend entry points
     assert L.b200gs_blend_fwd(0, 0, 64, 3, *([None] * 7), None, 1, 1, None, None, None, None) == -1
+    # [n,12] row buffers that are not 16-byte aligned (every other pointer is a non-NULL dummy)
+    d16, d8 = ctypes.c_void_p(16), ctypes.c_void_p(8)
+    assert L.b200gs_blend_fwd_rows(0, 64, 64, d16, d16, d8, d16, d16, 3, 1, d16, d16, d16, None) == -1
+    assert b"aligned" in L.b200gs_last_error()
+    for rows, v_rows in ((d8, d16), (d16, d8)):
+        assert L.b200gs_blend_bwd_rows(0, 64, 64, d16, d16, rows, d16, d16, d16, d16, 3, 1, d16, 1.0, 1.0, v_rows, None) == -1
+        assert b"aligned" in L.b200gs_last_error()
     # n = 0 is a valid no-op everywhere that takes a count
     v.sh_stride = 16
     assert L.b200gs_project_fwd(ctypes.byref(v), 0, *([None] * 13), None) == 0
