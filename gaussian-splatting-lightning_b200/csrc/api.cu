@@ -182,7 +182,7 @@ int b200gs_project_bwd_rows_multi(const B200gsView* views, int32_t n_views, int6
         B200GS_CHECK_ARG(views[0].sh_stride == 1 || (shs_rest && v_shs_rest), "shs_rest / v_shs_rest required when sh_stride > 1");
         B200GS_CHECK_ARG(v_means && v_log_scales && v_raw_quats && v_opacity_logits && v_shs_dc, "NULL output pointer");
     }
-    return launch_project_bwd_multi(views, n_views, n, means, log_scales, raw_quats, opacity_logits, shs_dc, shs_rest, anti_aliased, radii, clamped,
+    return launch_project_bwd_multi(views, n_views, n, means, log_scales, raw_quats, opacity_logits, shs_rest, anti_aliased, radii, clamped,
                                     row_index, v_rows, v_means, v_log_scales, v_raw_quats, v_opacity_logits, v_shs_dc, v_shs_rest,
                                     (cudaStream_t)stream);
 }

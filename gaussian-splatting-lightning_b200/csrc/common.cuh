@@ -96,9 +96,9 @@ int launch_project_pack_multi(const B200gsView* views, int n_views, int64_t n, c
                               uint8_t* clamped, int32_t* row_index, float* const* dst_rows, int64_t cap, void* workspace, size_t workspace_bytes,
                               int64_t* d_count, cudaStream_t s);
 int launch_project_bwd_multi(const B200gsView* views, int n_views, int64_t n, const float* means, const float* scales, const float* quats,
-                             const float* opac_logits, const float* shs_dc, const float* shs_rest, int anti_aliased, const int32_t* radii,
-                             const uint8_t* clamped, const int32_t* row_index, const float* const* v_rows, float* v_means, float* v_scales,
-                             float* v_quats, float* v_opac_logit, float* v_shs_dc, float* v_shs_rest, cudaStream_t s);
+                             const float* opac_logits, const float* shs_rest, int anti_aliased, const int32_t* radii, const uint8_t* clamped,
+                             const int32_t* row_index, const float* const* v_rows, float* v_means, float* v_scales, float* v_quats,
+                             float* v_opac_logit, float* v_shs_dc, float* v_shs_rest, cudaStream_t s);
 int launch_sh_fwd(int degree, int stride, int64_t n, const float* dirs, const float* coeffs, float* rgb, cudaStream_t s);
 int launch_sh_bwd(int degree, int stride, int64_t n, const float* dirs, const float* coeffs, const float* v_rgb,
                   float* v_coeffs, float* v_dirs, cudaStream_t s);

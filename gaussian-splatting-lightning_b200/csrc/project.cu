@@ -28,7 +28,8 @@ __device__ constexpr float SH_C4[9] = {2.5033429417967046f, -1.7701307697799304f
                                        0.6258357354491761f};
 
 // Every kernel that touches SH coefficients is instantiated for MC = 16 (degrees 0..3, the common case: 48 coefficient
-// registers) and MC = 25 (degree 4, sh_utils.py:102-111: 75 registers); the launchers pick by the view's sh_degree.
+// registers) and MC = 25 (degree 4, sh_utils.py:102-111: 75 registers); each launcher at the end of this file picks the
+// instantiation in one place, by the view's sh_degree (K8-multi also by the storage width).
 
 // Loads the first ncoef*3 floats of one Gaussian's SH block into registers. 128-bit path when the block is 16B aligned.
 template <int MC>
@@ -157,7 +158,6 @@ struct Proj {
     R T[6];              // T = J * Rw, rows 0,1 (2x3)
     R a, b, c, det;      // blurred cov2D and determinant
     R a0, c0, det0;      // un-blurred diag and determinant (gsplat compensation)
-    R qr, qx, qy, qz;    // the unit quaternion Rm was built from (filled by the backward kernels)
 };
 
 template <typename R>
@@ -187,15 +187,6 @@ __device__ __forceinline__ void gaussian_cov3d(const R* sc, const R* q, float sc
     g.S3[3] = xf(M[5], M[5], xf(M[4], M[4], xm(M[3], M[3])));
     g.S3[4] = xf(M[5], M[8], xf(M[4], M[7], xm(M[3], M[6])));
     g.S3[5] = xf(M[8], M[8], xf(M[7], M[7], xm(M[6], M[6])));
-}
-
-template <bool GSPLAT, typename R>
-__device__ __forceinline__ void project_view(const B200gsView& v, const float* p, Proj<R>& g);
-
-template <bool GSPLAT, typename R>
-__device__ __forceinline__ void project_geometry(const B200gsView& v, const float* p, const R* sc, const R* q, Proj<R>& g) {
-    gaussian_cov3d<R>(sc, q, v.scale_modifier, g);
-    project_view<GSPLAT, R>(v, p, g);
 }
 
 // The per-camera half: camera-space mean, Jacobian, cov2D (+ blur), determinants.  g.S3 (and Rm, s for the backward) are inputs.
@@ -323,9 +314,22 @@ __device__ __forceinline__ float near_of(const B200gsView& v) {
     return v.near_plane > 0.f ? v.near_plane : (GSPLAT ? 0.01f : 0.2f);
 }
 
+// K1's per-Gaussian prologue: mean p and camera-independent geometry g (gaussian_cov3d, with v's scale_modifier) of Gaussian i.
+// A lane past the end (live == false) leaves p as it is and gets the geometry of a unit Gaussian.
+template <bool RAW>
+__device__ __forceinline__ void load_gaussian(const B200gsView& v, const float* __restrict__ means, const float* __restrict__ scales,
+                                              const float* __restrict__ quats, int64_t i, bool live, float* p, Proj<double>& g) {
+    double sc[3] = {1.0, 1.0, 1.0}, q[4] = {1.0, 0.0, 0.0, 0.0}, inv_qn;
+    if (live) {
+        p[0] = __ldg(means + 3 * i); p[1] = __ldg(means + 3 * i + 1); p[2] = __ldg(means + 3 * i + 2);
+        load_scale_quat<RAW, double>(scales, quats, i, sc, q, &inv_qn);
+    }
+    gaussian_cov3d<double>(sc, q, v.scale_modifier, g);
+}
+
 // Destination of one view's projection outputs (element index `o` of every array).
 struct ProjOut {
-    float2* xy; float* depth; int32_t* radii; float* conic; float* comp; int32_t* tiles; float* cov3d; float* rgb; uint8_t* clamped;
+    float2* xy; float* depth; int32_t* radii; float* conic; float* comp; int32_t* tiles;
 };
 
 // What one (view, Gaussian) projection produces (all zero when the Gaussian is culled)
@@ -334,20 +338,8 @@ struct ProjVals {
     int32_t radius, ntiles;
 };
 
-// Projection of Gaussian (p, sc, q) into view v -> pv; returns the visibility.  cov3d (optional) is written at index o.
-template <bool GSPLAT, bool RAW>
-__device__ __forceinline__ bool project_one_view(const B200gsView& v, const RawIO& raw, int64_t i, int64_t o, const float* p, Proj<double>& g,
-                                                 float* cov3d_out, ProjVals& pv);
-
-template <bool GSPLAT, bool RAW>
-__device__ __forceinline__ bool project_one(const B200gsView& v, const RawIO& raw, int64_t i, int64_t o, const float* p, const double* sc,
-                                            const double* q, float* cov3d_out, ProjVals& pv) {
-    Proj<double> g;
-    gaussian_cov3d<double>(sc, q, v.scale_modifier, g);
-    return project_one_view<GSPLAT, RAW>(v, raw, i, o, p, g, cov3d_out, pv);
-}
-
-// g: gaussian_cov3d already evaluated
+// Projection of Gaussian i (mean p, gaussian_cov3d already in g) into view v -> pv; returns the visibility.  cov3d_out (optional)
+// receives cov3D at element o.
 template <bool GSPLAT, bool RAW>
 __device__ __forceinline__ bool project_one_view(const B200gsView& v, const RawIO& raw, int64_t i, int64_t o, const float* p, Proj<double>& g,
                                                  float* cov3d_out, ProjVals& pv) {
@@ -460,12 +452,12 @@ __global__ void __launch_bounds__(256, 3) project_fwd_kernel(const __grid_consta
                                                           uint8_t* __restrict__ clamped_out, float* __restrict__ rows_out) {
     const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const float p[3] = {__ldg(means + 3 * i), __ldg(means + 3 * i + 1), __ldg(means + 3 * i + 2)};
-    double sc[3], q[4], inv_qn;
-    load_scale_quat<RAW, double>(scales, quats, i, sc, q, &inv_qn);
-    const ProjOut out{xy_out, depth_out, radii_out, conic_out, comp_out, tiles_out, cov3d_out, rgb_out, clamped_out};
+    float p[3];
+    Proj<double> g;
+    load_gaussian<RAW>(v, means, scales, quats, i, true, p, g);
+    const ProjOut out{xy_out, depth_out, radii_out, conic_out, comp_out, tiles_out};
     ProjVals pv;
-    const bool vis = project_one<GSPLAT, RAW>(v, raw, i, i, p, sc, q, cov3d_out, pv);
+    const bool vis = project_one_view<GSPLAT, RAW>(v, raw, i, i, p, g, cov3d_out, pv);
     if (!RAW) store_soa<false>(out, nullptr, i, pv);
     float r = 0.f, gc = 0.f, bc = 0.f;
     uint8_t cl = 0;
@@ -496,6 +488,25 @@ struct ViewPack {
     B200gsView v[B200GS_MAX_VIEWS];
 };
 
+// SH colour of Gaussian i in each of the nviews cameras: the SH block is read once, if any camera sees the Gaussian (bit j of
+// vismask), and store(j, r, g, b, clamped) receives camera j's colour (zeros for a camera that does not see it).
+template <int MC, typename Store>
+__device__ __forceinline__ void color_views(const ViewPack& vp, int nviews, const float* __restrict__ shs_dc, const float* __restrict__ shs_rest,
+                                            int64_t i, const float* p, unsigned vismask, Store store) {
+    float sh[MC * 3];
+    if (vismask) {
+        const int deg = vp.v[0].sh_degree;
+        load_sh_any<true, MC>(shs_dc, shs_rest, i, vp.v[0].sh_stride, (deg + 1) * (deg + 1), sh);
+    }
+#pragma unroll 1
+    for (int j = 0; j < nviews; ++j) {
+        uint8_t cl = 0;
+        float r = 0.f, gc = 0.f, bc = 0.f;
+        if ((vismask >> j) & 1u) sh_color_one<MC>(vp.v[j], p, sh, r, gc, bc, cl);
+        store(j, r, gc, bc, cl);
+    }
+}
+
 template <int MC>
 __global__ void __launch_bounds__(256) project_fwd_multi_kernel(const __grid_constant__ ViewPack vp, int nviews, const RawIO raw, int64_t n,
                                                                 const float* __restrict__ means, const float* __restrict__ scales,
@@ -505,12 +516,10 @@ __global__ void __launch_bounds__(256) project_fwd_multi_kernel(const __grid_con
                                                                 float* __restrict__ rgb_out, uint8_t* __restrict__ clamped_out) {
     const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const float p[3] = {__ldg(means + 3 * i), __ldg(means + 3 * i + 1), __ldg(means + 3 * i + 2)};
-    double sc[3], q[4], inv_qn;
-    load_scale_quat<true, double>(scales, quats, i, sc, q, &inv_qn);
+    float p[3];
     Proj<double> g3;
-    gaussian_cov3d<double>(sc, q, vp.v[0].scale_modifier, g3);      // once per Gaussian; project_one_view per camera
-    const ProjOut out{xy_out, depth_out, radii_out, conic_out, nullptr, nullptr, nullptr, rgb_out, clamped_out};
+    load_gaussian<true>(vp.v[0], means, scales, quats, i, true, p, g3);      // once per Gaussian; project_one_view per camera
+    const ProjOut out{xy_out, depth_out, radii_out, conic_out, nullptr, nullptr};
     unsigned vismask = 0;
 #pragma unroll 1
     for (int j = 0; j < nviews; ++j) {
@@ -518,20 +527,11 @@ __global__ void __launch_bounds__(256) project_fwd_multi_kernel(const __grid_con
         if (project_one_view<true, true>(vp.v[j], raw, i, int64_t(j) * n + i, p, g3, nullptr, pv)) vismask |= 1u << j;
         store_soa<true>(out, raw.opac_out, int64_t(j) * n + i, pv);
     }
-    float sh[MC * 3];
-    if (vismask) {
-        const int deg = vp.v[0].sh_degree;
-        load_sh_any<true, MC>(shs_dc, raw.shs_rest, i, vp.v[0].sh_stride, (deg + 1) * (deg + 1), sh);
-    }
-#pragma unroll 1
-    for (int j = 0; j < nviews; ++j) {
-        float r = 0.f, gc = 0.f, bc = 0.f;
-        uint8_t cl = 0;
-        if ((vismask >> j) & 1u) sh_color_one<MC>(vp.v[j], p, sh, r, gc, bc, cl);
+    color_views<MC>(vp, nviews, shs_dc, raw.shs_rest, i, p, vismask, [&](int j, float r, float gc, float bc, uint8_t cl) {
         const int64_t o = int64_t(j) * n + i;
         rgb_out[3 * o + 0] = r; rgb_out[3 * o + 1] = gc; rgb_out[3 * o + 2] = bc;
         clamped_out[o] = cl;
-    }
+    });
 }
 
 // K1 of a shard for all W cameras FUSED with the exchange's packing: the visible splats of camera j leave this kernel as [.,12]
@@ -570,13 +570,8 @@ __global__ void __launch_bounds__(PACK_THREADS, (MC <= 16 ? 3 : 2)) project_pack
     const int64_t i = int64_t(t) * PACK_THREADS + tid;
     const bool live = i < n;
     float p[3] = {0.f, 0.f, 0.f};
-    double sc[3] = {1.0, 1.0, 1.0}, q[4] = {1.0, 0.0, 0.0, 0.0}, inv_qn;
-    if (live) {
-        p[0] = __ldg(means + 3 * i); p[1] = __ldg(means + 3 * i + 1); p[2] = __ldg(means + 3 * i + 2);
-        load_scale_quat<true, double>(scales, quats, i, sc, q, &inv_qn);
-    }
     Proj<double> g3;
-    gaussian_cov3d<double>(sc, q, vp.v[0].scale_modifier, g3);      // once per Gaussian; project_one_view per camera
+    load_gaussian<true>(vp.v[0], means, scales, quats, i, live, p, g3);      // once per Gaussian; project_one_view per camera
     unsigned vismask = 0;
     unsigned long long kpos = 0;            // 8 bits per camera: this lane's rank among the warp's visible lanes
 #pragma unroll 1
@@ -601,22 +596,13 @@ __global__ void __launch_bounds__(PACK_THREADS, (MC <= 16 ? 3 : 2)) project_pack
             row[2].w = __int_as_float(pv.radius);
         }
     }
-    float sh[MC * 3];
-    if (vismask) {
-        const int deg = vp.v[0].sh_degree;
-        load_sh_any<true, MC>(shs_dc, raw.shs_rest, i, vp.v[0].sh_stride, (deg + 1) * (deg + 1), sh);
-    }
-#pragma unroll 1
-    for (int j = 0; j < nviews; ++j) {
-        uint8_t cl = 0;
+    color_views<MC>(vp, nviews, shs_dc, raw.shs_rest, i, p, vismask, [&](int j, float r, float gc, float bc, uint8_t cl) {
         if ((vismask >> j) & 1u) {
-            float r, gc, bc;
-            sh_color_one<MC>(vp.v[j], p, sh, r, gc, bc, cl);
             float* row2 = reinterpret_cast<float*>(s_rows + (size_t(j) * PACK_THREADS + w * 32 + (int)((kpos >> (8 * j)) & 255ull)) * 3 + 2);
             row2[0] = r; row2[1] = gc; row2[2] = bc;
         }
         if (live) clamped_out[int64_t(j) * n + i] = cl;
-    }
+    });
     __syncthreads();
     // warp j: camera j's block total -> chained scan over the blocks -> first row of every warp's run
     if ((int)w < nviews) {
@@ -673,10 +659,11 @@ struct ProjCot {
 };
 
 // Adds view v's contribution to dL/dmean (dm), dL/dM-chain outputs: dL/dscale (activated scale, before the exp chain) and dL/dq
-// (unit quaternion, before the normalisation chain).  g = project_geometry<GSPLAT, float>(v, p, sc, q).
+// (unit quaternion, before the normalisation chain).  g: gaussian_cov3d<float>(sc, q) and project_view<GSPLAT, float>(v, p) of the
+// Gaussian with mean p, scales sc and unit quaternion q.
 template <bool GSPLAT>
-__device__ __forceinline__ void geometry_backward(const B200gsView& v, const float* p, const Proj<float>& g, const ProjCot& c, float* dm,
-                                                  float* dscale, float4& dq) {
+__device__ __forceinline__ void geometry_backward(const B200gsView& v, const float* p, const float* q, const Proj<float>& g, const ProjCot& c,
+                                                  float* dm, float* dscale, float4& dq) {
     const float* V = v.viewmatrix;
     float dtx = 0.f, dty = 0.f, dtz = 0.f;  // dL/dt (camera)
     // ---- conic (+ compensation) -> blurred cov2D (a, b, c) ----------------------------------------------------
@@ -783,19 +770,58 @@ __device__ __forceinline__ void geometry_backward(const B200gsView& v, const flo
 #pragma unroll
         for (int r = 0; r < 3; ++r) dR[r * 3 + k] = dM[r * 3 + k] * g.s[k];
     }
-    // Rm was built from the (unit) quaternion (r, x, y, z): recover it from the caller
-    const float r = g.qr, x = g.qx, y = g.qy, z = g.qz;
+    const float r = q[0], x = q[1], y = q[2], z = q[3];
     dq.x += 2.f * (-z * dR[1] + y * dR[2] + z * dR[3] - x * dR[5] - y * dR[6] + x * dR[7]);
     dq.y += 2.f * (y * dR[1] + z * dR[2] + y * dR[3] - 2.f * x * dR[4] - r * dR[5] + z * dR[6] + r * dR[7] - 2.f * x * dR[8]);
     dq.z += 2.f * (-2.f * y * dR[0] + x * dR[1] + r * dR[2] + x * dR[3] + z * dR[5] - r * dR[6] + z * dR[7] - 2.f * y * dR[8]);
     dq.w += 2.f * (-2.f * z * dR[0] - r * dR[1] + x * dR[2] + r * dR[3] - 2.f * z * dR[4] + y * dR[5] + x * dR[6] + y * dR[7]);
 }
 
-// SH-gradient rows of a warp's 32 Gaussians: staged in shared memory (odd row stride: conflict-free) and written back with
-// fully coalesced 128-bit stores: every row must be written (zeros for culled Gaussians), so the warp's 32 rows are one
-// contiguous 5.6-6 KB span of the output.  out[] holds this lane's 48 values (dc first); RAW: dc goes to v_shs, rest to dst_base.
-// second half of store_sh_rows: the warp's staged rows (row of lane l at s_rows_warp + l * (rw | 1)) -> global memory, coalesced
-template <bool RAW>
+// Opacity logit x: o = sigmoid(x) and 1 - o, taken as o1 = sigmoid(-x) (1.0f - o cancels at large logits: a 1e-2 relative error of
+// the logit gradient at logit 12)
+__device__ __forceinline__ void logit_sigmoid(float x, float& o, float& o1) {
+    o = 1.0f / (1.0f + expf(-x));
+    o1 = 1.0f / (1.0f + expf(x));
+}
+
+// The blend opacity is sigmoid(logit), times the compensation when anti-aliased: splits its cotangent vo, adding the compensation's
+// share to c.vcomp and returning the sigmoid's (dL/dlogit is that times o o1).
+template <bool GSPLAT>
+__device__ __forceinline__ float sigmoid_cotangent(float vo, float o, int anti_aliased, const Proj<float>& g, ProjCot& c) {
+    if (!(GSPLAT && anti_aliased)) return vo;
+    c.vcomp += vo * o;
+    return vo * sqrtf(fmaxf(g.det0 / g.det, 0.f));
+}
+
+// Through the fused activations of the raw parameters: scale = exp(log scale) (d exp(x) = exp(x)) and unit quaternion
+// q = raw / |raw| (inv_qn = 1 / |raw|).
+__device__ __forceinline__ void raw_param_backward(const float* sc, const float* q, float inv_qn, float* dscale, float4& dq) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) dscale[k] *= sc[k];
+    const float dot = dq.x * q[0] + dq.y * q[1] + dq.z * q[2] + dq.w * q[3];
+    dq.x = (dq.x - q[0] * dot) * inv_qn; dq.y = (dq.y - q[1] * dot) * inv_qn;
+    dq.z = (dq.z - q[2] * dot) * inv_qn; dq.w = (dq.w - q[3] * dot) * inv_qn;
+}
+
+// Gradient of the SH colour with respect to the point the unit view direction (dx, dy, dz) = (p - campos) * inv_len starts from, given
+// the weights w[k] = <SH coefficient k, dL/drgb> for k >= 1: sum_k w[k] d(basis_k)/d(dir), less its radial component, times inv_len.
+template <int MC>
+__device__ __forceinline__ float3 view_dir_grad(int deg, float dx, float dy, float dz, float inv_len, const float* w) {
+    const int ncoef = (deg + 1) * (deg + 1);
+    float bx[MC], by[MC], bz[MC];
+    sh_basis_grad<MC>(deg, dx, dy, dz, bx, by, bz);
+    float ddx = 0.f, ddy = 0.f, ddz = 0.f;
+#pragma unroll
+    for (int k = 1; k < MC; ++k) {
+        if (k < ncoef) { ddx += bx[k] * w[k]; ddy += by[k] * w[k]; ddz += bz[k] * w[k]; }
+    }
+    const float dot = dx * ddx + dy * ddy + dz * ddz;
+    return make_float3((ddx - dx * dot) * inv_len, (ddy - dy * dot) * inv_len, (ddz - dz * dot) * inv_len);
+}
+
+// SH-gradient rows of a warp's 32 Gaussians, staged in shared memory (row of lane l at s_rows_warp + l * (rw | 1); the odd stride
+// keeps the staging conflict-free), written back with fully coalesced 128-bit stores.  Every row is written (zeros for culled
+// Gaussians), so the warp's rows are one contiguous span of the output (5.6-6 KB at 45-48 floats per row).  ACC: added to dst_base.
 __device__ __forceinline__ void flush_sh_rows(const float* s_rows_warp, int rw, int64_t i, int64_t n, unsigned lane, float* __restrict__ dst_base,
                                               bool ACC) {
     const int rwp = rw | 1;
@@ -823,33 +849,6 @@ __device__ __forceinline__ void flush_sh_rows(const float* s_rows_warp, int rw, 
         for (int f = (total & ~3) + lane; f < total; f += 32) dst[f] = sw[(f / rw) * rwp + f % rw] + (ACC ? dst[f] : 0.f);
     } else {
         for (int f = lane; f < total; f += 32) dst[f] = sw[(f / rw) * rwp + f % rw] + (ACC ? dst[f] : 0.f);
-    }
-}
-
-template <bool RAW, int MC>
-__device__ __forceinline__ void store_sh_rows(float* s_rows_warp, const float* out, int64_t i, int64_t n, bool in_range, int stride3, unsigned lane,
-                                              float* __restrict__ v_shs, float* __restrict__ v_shs_rest, bool ACC) {
-    const int rw = RAW ? stride3 - 3 : stride3;          // floats per output row
-    float* dst_base = RAW ? v_shs_rest : v_shs;
-    if (RAW && in_range) {
-        float o0 = out[0], o1 = out[1], o2 = out[2];
-        if (ACC) { o0 += v_shs[3 * i]; o1 += v_shs[3 * i + 1]; o2 += v_shs[3 * i + 2]; }
-        v_shs[3 * i] = o0; v_shs[3 * i + 1] = o1; v_shs[3 * i + 2] = o2;
-    }
-    if (rw <= MC * 3) {
-        const int rwp = rw | 1;
-        float* row = s_rows_warp + lane * rwp;
-#pragma unroll
-        for (int k = 0; k < MC * 3; ++k) {
-            const int c = RAW ? k - 3 : k;
-            if (c >= 0 && c < rw) row[c] = out[k];
-        }
-        flush_sh_rows<RAW>(s_rows_warp, rw, i, n, lane, dst_base, ACC);
-    } else if (in_range) {  // wider coefficient storage than the kernel evaluates: plain per-thread rows
-        float* o = dst_base + i * int64_t(rw);
-#pragma unroll
-        for (int k = RAW ? 3 : 0; k < MC * 3; ++k) o[RAW ? k - 3 : k] = out[k];
-        for (int c = MC * 3 - (RAW ? 3 : 0); c < rw; ++c) o[c] = 0.f;
     }
 }
 
@@ -905,27 +904,21 @@ __global__ void __launch_bounds__(BWD_THREADS, (MC <= 16 ? (GSPLAT ? 7 : 6) : 3)
             float w[MC];
 #pragma unroll
             for (int k = 1; k < MC; ++k) w[k] = (k < ncoef) ? __ldg(c0 + 3 * k) * gr + __ldg(c0 + 3 * k + 1) * gg + __ldg(c0 + 3 * k + 2) * gb : 0.f;
-            float bx[MC], by[MC], bz[MC];
-            sh_basis_grad<MC>(deg, dx, dy, dz, bx, by, bz);
-            float ddx = 0.f, ddy = 0.f, ddz = 0.f;
-#pragma unroll
-            for (int k = 1; k < MC; ++k) {
-                if (k < ncoef) { ddx += bx[k] * w[k]; ddy += by[k] * w[k]; ddz += bz[k] * w[k]; }
-            }
-            const float dot = dx * ddx + dy * ddy + dz * ddz;
-            dm[0] += (ddx - dx * dot) * inv_len;
-            dm[1] += (ddy - dy * dot) * inv_len;
-            dm[2] += (ddz - dz * dot) * inv_len;
+            const float3 d = view_dir_grad<MC>(deg, dx, dy, dz, inv_len, w);
+            dm[0] += d.x; dm[1] += d.y; dm[2] += d.z;
         }
-        // SH-gradient row of this Gaussian (coefficient k, channel c: basis_k * v_rgb_c; zeros when culled) straight into the warp's
-        // staging rows — 48 values that used to sit in registers until the store (96 registers, 5 blocks per SM) — then out coalesced
+        // SH-gradient row of this Gaussian (coefficient k, channel c: basis_k * v_rgb_c; zeros when culled).  RAW: the dc coefficient
+        // goes to v_shs, the rest to the row of v_shs_rest.
         const int rw = RAW ? stride3 - 3 : stride3;          // floats per output row
+        float* dst = RAW ? raw.v_shs_rest : v_shs;
+        if (RAW && in_range) {
+            float o0 = bs[0] * gr, o1 = bs[0] * gg, o2 = bs[0] * gb;
+            if (ACC) { o0 += v_shs[3 * i]; o1 += v_shs[3 * i + 1]; o2 += v_shs[3 * i + 2]; }
+            v_shs[3 * i] = o0; v_shs[3 * i + 1] = o1; v_shs[3 * i + 2] = o2;
+        }
         if (rw <= MC * 3) {
-            if (RAW && in_range) {
-                float o0 = bs[0] * gr, o1 = bs[0] * gg, o2 = bs[0] * gb;
-                if (ACC) { o0 += v_shs[3 * i]; o1 += v_shs[3 * i + 1]; o2 += v_shs[3 * i + 2]; }
-                v_shs[3 * i] = o0; v_shs[3 * i + 1] = o1; v_shs[3 * i + 2] = o2;
-            }
+            // straight into the warp's staging rows (48 values would otherwise sit in registers until the store: 96 registers,
+            // 5 blocks per SM), then out coalesced
             float* row = s_rows[warp] + lane * (rw | 1);
 #pragma unroll
             for (int k = RAW ? 1 : 0; k < MC; ++k) {
@@ -935,15 +928,21 @@ __global__ void __launch_bounds__(BWD_THREADS, (MC <= 16 ? (GSPLAT ? 7 : 6) : 3)
                     row[c] = bk * gr; row[c + 1] = bk * gg; row[c + 2] = bk * gb;
                 }
             }
-            flush_sh_rows<RAW>(s_rows[warp], rw, i, n, lane, RAW ? raw.v_shs_rest : v_shs, ACC);
-        } else {   // wider coefficient storage than the kernel evaluates: the register path of store_sh_rows
-            float out[MC * 3];
+            flush_sh_rows(s_rows[warp], rw, i, n, lane, dst, ACC);
+        } else if (in_range) {   // wider coefficient storage than the kernel evaluates: plain per-thread rows (ACC: add the evaluated ones)
+            float* row = dst + i * int64_t(rw);
 #pragma unroll
-            for (int k = 0; k < MC; ++k) {
+            for (int k = RAW ? 1 : 0; k < MC; ++k) {
+                const int c = RAW ? 3 * k - 3 : 3 * k;
                 const float bk = (k < ncoef) ? bs[k] : 0.f;
-                out[3 * k + 0] = bk * gr; out[3 * k + 1] = bk * gg; out[3 * k + 2] = bk * gb;
+                if (!ACC) {
+                    row[c] = bk * gr; row[c + 1] = bk * gg; row[c + 2] = bk * gb;
+                } else if (k < ncoef) {
+                    row[c] += bk * gr; row[c + 1] += bk * gg; row[c + 2] += bk * gb;
+                }
             }
-            store_sh_rows<RAW, MC>(s_rows[warp], out, i, n, in_range, stride3, lane, v_shs, raw.v_shs_rest, ACC);
+            if (!ACC)
+                for (int c = MC * 3 - (RAW ? 3 : 0); c < rw; ++c) row[c] = 0.f;
         }
     }
     if (!in_range) return;
@@ -965,8 +964,8 @@ __global__ void __launch_bounds__(BWD_THREADS, (MC <= 16 ? (GSPLAT ? 7 : 6) : 3)
     float sc[3], q[4], inv_qn;
     load_scale_quat<RAW, float>(scales, quats, i, sc, q, &inv_qn);
     Proj<float> g;
-    project_geometry<GSPLAT, float>(v, p, sc, q, g);
-    g.qr = q[0]; g.qx = q[1]; g.qy = q[2]; g.qz = q[3];
+    gaussian_cov3d<float>(sc, q, v.scale_modifier, g);
+    project_view<GSPLAT, float>(v, p, g);
 
     ProjCot c;
     const float* ccon = RAW ? vrow + B200GS_ROW_CONIC : v_conic + 3 * i;
@@ -976,33 +975,21 @@ __global__ void __launch_bounds__(BWD_THREADS, (MC <= 16 ? (GSPLAT ? 7 : 6) : 3)
     if (GSPLAT) c.vdepth = RAW ? __ldg(vrow + B200GS_ROW_DEPTH) : (v_depth ? __ldg(v_depth + i) : 0.f);
     c.vcomp = (GSPLAT && v_comp != nullptr) ? __ldg(v_comp + i) : 0.f;
     if (RAW) {
-        // blend opacity = sigmoid(logit) [* compensation]: split dL/d(opac_out) between the logit and the compensation
-        // 1 - o = sigmoid(-logit): 1.0f - o cancels at large logits (a 1e-2 relative error of the logit gradient at logit 12)
-        const float x = __ldg(raw.opac_in + i);
-        const float o = 1.0f / (1.0f + expf(-x)), o1 = 1.0f / (1.0f + expf(x));
-        const float vo = __ldg(vrow + B200GS_ROW_OPACITY);
-        float v_sig = vo;
-        if (GSPLAT && raw.anti_aliased) {
-            const float comp = sqrtf(fmaxf(g.det0 / g.det, 0.f));
-            v_sig = vo * comp;
-            c.vcomp += vo * o;
-        }
+        float o, o1;
+        logit_sigmoid(__ldg(raw.opac_in + i), o, o1);
+        const float v_sig = sigmoid_cotangent<GSPLAT>(__ldg(vrow + B200GS_ROW_OPACITY), o, raw.anti_aliased, g, c);
         // explicit fma: whether nvcc contracts the product into the add depends on the surrounding code (see xm / xa / xf)
         raw.v_opac_logit[i] = fmaf(v_sig * o, o1, ACC ? raw.v_opac_logit[i] : 0.f);
     }
     float dscale[3] = {0.f, 0.f, 0.f};
     float4 dq = make_float4(0.f, 0.f, 0.f, 0.f);
-    geometry_backward<GSPLAT>(v, p, g, c, dm, dscale, dq);
+    geometry_backward<GSPLAT>(v, p, q, g, c, dm, dscale, dq);
+    if (RAW) raw_param_backward(sc, q, inv_qn, dscale, dq);
 
     if (ACC) { dm[0] += v_means[3 * i]; dm[1] += v_means[3 * i + 1]; dm[2] += v_means[3 * i + 2]; }
     v_means[3 * i] = dm[0]; v_means[3 * i + 1] = dm[1]; v_means[3 * i + 2] = dm[2];
 #pragma unroll
-    for (int k = 0; k < 3; ++k) v_scales[3 * i + k] = (RAW ? dscale[k] * sc[k] : dscale[k]) + (ACC ? v_scales[3 * i + k] : 0.f);   // d exp(x) = exp(x)
-    if (RAW) {  // through q / |q|
-        const float dot = dq.x * q[0] + dq.y * q[1] + dq.z * q[2] + dq.w * q[3];
-        dq.x = (dq.x - q[0] * dot) * inv_qn; dq.y = (dq.y - q[1] * dot) * inv_qn;
-        dq.z = (dq.z - q[2] * dot) * inv_qn; dq.w = (dq.w - q[3] * dot) * inv_qn;
-    }
+    for (int k = 0; k < 3; ++k) v_scales[3 * i + k] = dscale[k] + (ACC ? v_scales[3 * i + k] : 0.f);
     if (ACC) {
         const float4 old = v_quats[i];
         dq.x += old.x; dq.y += old.y; dq.z += old.z; dq.w += old.w;
@@ -1035,7 +1022,7 @@ __global__ void __launch_bounds__(BWD_THREADS) project_bwd_multi_kernel(const __
     const int deg = vp.v[0].sh_degree;
     const int ncoef = (deg + 1) * (deg + 1);
     // SH-gradient accumulators over the cameras: the dc coefficient in registers, the rest in this lane's row of the staging buffer
-    // (48 accumulator registers kept the kernel at 183 registers = 8 warps per SM); rows wider than the buffer keep the register path
+    // (48 accumulator registers kept the kernel at 183 registers = 8 warps per SM)
     const int rw = stride3 - 3;                      // <= MC * 3: the launcher picks MC by the storage width
     float* my_row = s_rows[warp] + lane * (rw | 1);
     float dc_acc[3] = {0.f, 0.f, 0.f};
@@ -1057,11 +1044,8 @@ __global__ void __launch_bounds__(BWD_THREADS) project_bwd_multi_kernel(const __
         if (!loaded) {
             p[0] = __ldg(means + 3 * i); p[1] = __ldg(means + 3 * i + 1); p[2] = __ldg(means + 3 * i + 2);
             load_scale_quat<true, float>(scales, quats, i, sc, q, &inv_qn);
-            const float x = __ldg(raw.opac_in + i);
-            o = 1.0f / (1.0f + expf(-x));
-            o1 = 1.0f / (1.0f + expf(x));                            // 1 - o without cancellation
+            logit_sigmoid(__ldg(raw.opac_in + i), o, o1);
             gaussian_cov3d<float>(sc, q, vp.v[0].scale_modifier, g);      // once per Gaussian; project_view per camera
-            g.qr = q[0]; g.qx = q[1]; g.qy = q[2]; g.qz = q[3];
             loaded = true;
         }
         const B200gsView& v = vp.v[j];
@@ -1088,24 +1072,16 @@ __global__ void __launch_bounds__(BWD_THREADS) project_bwd_multi_kernel(const __
         c.vdepth = w0.z;
         c.vA = w0.w; c.vB = w1.x; c.vC = w1.y;
         c.vcomp = 0.f;
-        const float vo = w1.w;
-        float v_sig = vo;
-        if (raw.anti_aliased) {
-            const float comp = sqrtf(fmaxf(g.det0 / g.det, 0.f));
-            v_sig = vo * comp;
-            c.vcomp = vo * o;
-        }
-        dlogit += v_sig * o * o1;
-        geometry_backward<true>(v, p, g, c, dm, dscale, dq);
+        dlogit += sigmoid_cotangent<true>(w1.w, o, raw.anti_aliased, g, c) * o * o1;
+        geometry_backward<true>(v, p, q, g, c, dm, dscale, dq);
     }
     if (in_range) { v_shs_dc[3 * i] = dc_acc[0]; v_shs_dc[3 * i + 1] = dc_acc[1]; v_shs_dc[3 * i + 2] = dc_acc[2]; }
-    flush_sh_rows<true>(s_rows[warp], rw, i, n, lane, raw.v_shs_rest, false);
+    flush_sh_rows(s_rows[warp], rw, i, n, lane, raw.v_shs_rest, false);
     if (!in_range) return;
+    raw_param_backward(sc, q, inv_qn, dscale, dq);
     v_means[3 * i] = dm[0]; v_means[3 * i + 1] = dm[1]; v_means[3 * i + 2] = dm[2];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) v_scales[3 * i + k] = dscale[k] * sc[k];
-    const float dot = dq.x * q[0] + dq.y * q[1] + dq.z * q[2] + dq.w * q[3];
-    v_quats[i] = make_float4((dq.x - q[0] * dot) * inv_qn, (dq.y - q[1] * dot) * inv_qn, (dq.z - q[2] * dot) * inv_qn, (dq.w - q[3] * dot) * inv_qn);
+    v_scales[3 * i] = dscale[0]; v_scales[3 * i + 1] = dscale[1]; v_scales[3 * i + 2] = dscale[2];
+    v_quats[i] = dq;
     raw.v_opac_logit[i] = dlogit;
 }
 
@@ -1157,16 +1133,11 @@ __global__ void __launch_bounds__(256) sh_bwd_kernel(int deg, int stride, int64_
         if (deg > 0) {
             float sh[MC * 3];
             load_sh<MC>(coeffs + i * int64_t(stride3), ncoef, vec4, sh);
-            float bx[MC], by[MC], bz[MC];
-            sh_basis_grad<MC>(deg, dx, dy, dz, bx, by, bz);
+            float w[MC];
 #pragma unroll
-            for (int k = 1; k < MC; ++k)
-                if (k < ncoef) {
-                    const float w = sh[3 * k] * gr + sh[3 * k + 1] * gg + sh[3 * k + 2] * gb;
-                    ddx += bx[k] * w; ddy += by[k] * w; ddz += bz[k] * w;
-                }
-            const float dot = dx * ddx + dy * ddy + dz * ddz;
-            ddx = (ddx - dx * dot) * inv_len; ddy = (ddy - dy * dot) * inv_len; ddz = (ddz - dz * dot) * inv_len;
+            for (int k = 1; k < MC; ++k) w[k] = (k < ncoef) ? sh[3 * k] * gr + sh[3 * k + 1] * gg + sh[3 * k + 2] * gb : 0.f;
+            const float3 d = view_dir_grad<MC>(deg, dx, dy, dz, inv_len, w);
+            ddx = d.x; ddy = d.y; ddz = d.z;
         }
         v_dirs[3 * i] = ddx; v_dirs[3 * i + 1] = ddy; v_dirs[3 * i + 2] = ddz;
     }
@@ -1174,19 +1145,17 @@ __global__ void __launch_bounds__(256) sh_bwd_kernel(int deg, int stride, int64_
 
 }  // namespace
 
-// K1 / K8 launch: constant set from the view's mode, SH registers for 16 or 25 coefficients from its degree
+// Single-view K1 / K8 launch: the kernel comes from a table indexed by the view's mode (constant set) and by whether it needs 25 SH
+// coefficients (MC = 25 iff SH is given and sh_degree > 3)
 template <bool RAW>
 static int project_fwd_launch(const B200gsView& v, const RawIO& raw, int64_t n, const float* means, const float* scales, const float* quats,
                               const float* shs, float* xy, float* depth, int32_t* radii, float* conic, float* comp, int32_t* tiles,
                               float* cov3d, float* rgb, uint8_t* clamped, float* rows, cudaStream_t s) {
+    static constexpr decltype(&project_fwd_kernel<false, RAW, 16>) kernels[2][2] = {
+        {project_fwd_kernel<false, RAW, 16>, project_fwd_kernel<false, RAW, 25>}, {project_fwd_kernel<true, RAW, 16>, project_fwd_kernel<true, RAW, 25>}};
     if (n == 0) return B200GS_OK;
-    const unsigned blocks = (unsigned)div_up64(n, 256);
-    const bool gs = v.mode == B200GS_MODE_GSPLAT, deg4 = shs != nullptr && v.sh_degree > 3;
-#define B200GS_PF_LAUNCH(G, MC) project_fwd_kernel<G, RAW, MC><<<blocks, 256, 0, s>>>(v, raw, n, means, scales, quats, shs, (float2*)xy, depth, \
-                                                                                    radii, conic, comp, tiles, cov3d, rgb, clamped, rows)
-    if (gs) { if (deg4) B200GS_PF_LAUNCH(true, 25); else B200GS_PF_LAUNCH(true, 16); }
-    else    { if (deg4) B200GS_PF_LAUNCH(false, 25); else B200GS_PF_LAUNCH(false, 16); }
-#undef B200GS_PF_LAUNCH
+    kernels[v.mode == B200GS_MODE_GSPLAT][shs != nullptr && v.sh_degree > 3]<<<(unsigned)div_up64(n, 256), 256, 0, s>>>(
+        v, raw, n, means, scales, quats, shs, (float2*)xy, depth, radii, conic, comp, tiles, cov3d, rgb, clamped, rows);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
@@ -1196,15 +1165,12 @@ static int project_bwd_launch(const B200gsView& v, const RawIO& raw, int64_t n, 
                               const float* shs, const int32_t* radii, const uint8_t* clamped, const float* v_xy, const float* v_depth,
                               const float* v_conic, const float* v_comp, const float* v_rgb, float* v_means, float* v_scales, float* v_quats,
                               float* v_shs, cudaStream_t s) {
+    static constexpr decltype(&project_bwd_kernel<false, RAW, 16>) kernels[2][2] = {
+        {project_bwd_kernel<false, RAW, 16>, project_bwd_kernel<false, RAW, 25>}, {project_bwd_kernel<true, RAW, 16>, project_bwd_kernel<true, RAW, 25>}};
     if (n == 0) return B200GS_OK;
-    const unsigned blocks = (unsigned)div_up64(n, BWD_THREADS);
-    const bool gs = v.mode == B200GS_MODE_GSPLAT, deg4 = v_shs != nullptr && v.sh_degree > 3;
-#define B200GS_PB_LAUNCH(G, MC) project_bwd_kernel<G, RAW, MC><<<blocks, BWD_THREADS, 0, s>>>(v, raw, n, means, scales, quats, shs, radii, clamped, \
-                                                                                             (const float2*)v_xy, v_depth, v_conic, v_comp, v_rgb, \
-                                                                                             v_means, v_scales, (float4*)v_quats, v_shs)
-    if (gs) { if (deg4) B200GS_PB_LAUNCH(true, 25); else B200GS_PB_LAUNCH(true, 16); }
-    else    { if (deg4) B200GS_PB_LAUNCH(false, 25); else B200GS_PB_LAUNCH(false, 16); }
-#undef B200GS_PB_LAUNCH
+    kernels[v.mode == B200GS_MODE_GSPLAT][v_shs != nullptr && v.sh_degree > 3]<<<(unsigned)div_up64(n, BWD_THREADS), BWD_THREADS, 0, s>>>(
+        v, raw, n, means, scales, quats, shs, radii, clamped, (const float2*)v_xy, v_depth, v_conic, v_comp, v_rgb, v_means, v_scales,
+        (float4*)v_quats, v_shs);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
@@ -1256,12 +1222,8 @@ int launch_project_fwd_multi(const B200gsView* views, int n_views, int64_t n, co
     for (int j = n_views; j < B200GS_MAX_VIEWS; ++j) vp.v[j] = views[0];
     RawIO raw{};
     raw.opac_in = opac_logits; raw.shs_rest = shs_rest; raw.opac_out = opac_out; raw.anti_aliased = anti_aliased;
-    if (views[0].sh_degree > 3)
-        project_fwd_multi_kernel<25><<<(unsigned)div_up64(n, 256), 256, 0, s>>>(vp, n_views, raw, n, means, scales, quats, shs_dc, (float2*)xy, depth,
-                                                                                radii, conic, rgb, clamped);
-    else
-        project_fwd_multi_kernel<16><<<(unsigned)div_up64(n, 256), 256, 0, s>>>(vp, n_views, raw, n, means, scales, quats, shs_dc, (float2*)xy, depth,
-                                                                                radii, conic, rgb, clamped);
+    const auto kernel = views[0].sh_degree > 3 ? project_fwd_multi_kernel<25> : project_fwd_multi_kernel<16>;
+    kernel<<<(unsigned)div_up64(n, 256), 256, 0, s>>>(vp, n_views, raw, n, means, scales, quats, shs_dc, (float2*)xy, depth, radii, conic, rgb, clamped);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
@@ -1297,30 +1259,30 @@ int launch_project_pack_multi(const B200gsView* views, int n_views, int64_t n, c
     uint32_t* state = ticket + 64;
     const unsigned blocks = (unsigned)div_up64(n, PACK_THREADS);
     const size_t smem = (size_t)n_views * PACK_THREADS * 3 * sizeof(float4);
-    static bool configured = false;         // raise the dynamic shared-memory limit once (8 cameras: 96 KB)
-    if (!configured) {
-        B200GS_CUDA(cudaFuncSetAttribute((const void*)project_pack_multi_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         B200GS_MAX_VIEWS * PACK_THREADS * 3 * (int)sizeof(float4)));
-        B200GS_CUDA(cudaFuncSetAttribute((const void*)project_pack_multi_kernel<25>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         B200GS_MAX_VIEWS * PACK_THREADS * 3 * (int)sizeof(float4)));
-        configured = true;
+    // The first launch of each instantiation also raises its dynamic shared-memory limit (8 cameras: 96 KB)
+    const auto launch = [&](auto mc) {
+        const auto kernel = project_pack_multi_kernel<decltype(mc)::value>;
+        static const cudaError_t attr_rc = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                                B200GS_MAX_VIEWS * PACK_THREADS * 3 * (int)sizeof(float4));
+        if (attr_rc == cudaSuccess)
+            kernel<<<blocks, PACK_THREADS, smem, s>>>(vp, n_views, raw, n, means, scales, quats, shs_dc, (float2*)xy, radii, clamped, row_index, dst,
+                                                      cap, ticket, state, d_count);
+        return attr_rc;
+    };
+    const cudaError_t attr_rc = views[0].sh_degree > 3 ? launch(std::integral_constant<int, 25>{}) : launch(std::integral_constant<int, 16>{});
+    if (attr_rc != cudaSuccess) {
+        set_error("project_pack_multi: cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_rc));
+        return B200GS_ECUDA;
     }
-    if (views[0].sh_degree > 3)
-        project_pack_multi_kernel<25><<<blocks, PACK_THREADS, smem, s>>>(vp, n_views, raw, n, means, scales, quats, shs_dc, (float2*)xy, radii, clamped,
-                                                                         row_index, dst, cap, ticket, state, d_count);
-    else
-        project_pack_multi_kernel<16><<<blocks, PACK_THREADS, smem, s>>>(vp, n_views, raw, n, means, scales, quats, shs_dc, (float2*)xy, radii, clamped,
-                                                                         row_index, dst, cap, ticket, state, d_count);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
 int launch_project_bwd_multi(const B200gsView* views, int n_views, int64_t n, const float* means, const float* scales, const float* quats,
-                             const float* opac_logits, const float* shs_dc, const float* shs_rest, int anti_aliased, const int32_t* radii,
-                             const uint8_t* clamped, const int32_t* row_index, const float* const* v_rows, float* v_means, float* v_scales,
-                             float* v_quats, float* v_opac_logit, float* v_shs_dc, float* v_shs_rest, cudaStream_t s) {
+                             const float* opac_logits, const float* shs_rest, int anti_aliased, const int32_t* radii, const uint8_t* clamped,
+                             const int32_t* row_index, const float* const* v_rows, float* v_means, float* v_scales, float* v_quats,
+                             float* v_opac_logit, float* v_shs_dc, float* v_shs_rest, cudaStream_t s) {
     if (n == 0 || n_views == 0) return B200GS_OK;
-    (void)shs_dc;
     ViewPack vp;
     RowSources src;
     static const float dummy[B200GS_ROW_FLOATS] = {0.f};
@@ -1336,22 +1298,17 @@ int launch_project_bwd_multi(const B200gsView* views, int n_views, int64_t n, co
         set_error("project_bwd_multi: sh_stride %d exceeds 25 coefficients", views[0].sh_stride);
         return B200GS_EINVAL;
     }
-    if (views[0].sh_degree > 3 || views[0].sh_stride > 16)
-        project_bwd_multi_kernel<25><<<(unsigned)div_up64(n, BWD_THREADS), BWD_THREADS, 0, s>>>(vp, n_views, raw, src, n, means, scales, quats, radii,
-                                                                                                clamped, row_index, v_means, v_scales, (float4*)v_quats,
-                                                                                                v_shs_dc);
-    else
-        project_bwd_multi_kernel<16><<<(unsigned)div_up64(n, BWD_THREADS), BWD_THREADS, 0, s>>>(vp, n_views, raw, src, n, means, scales, quats, radii,
-                                                                                                clamped, row_index, v_means, v_scales, (float4*)v_quats,
-                                                                                                v_shs_dc);
+    const auto kernel = views[0].sh_degree > 3 || views[0].sh_stride > 16 ? project_bwd_multi_kernel<25> : project_bwd_multi_kernel<16>;
+    kernel<<<(unsigned)div_up64(n, BWD_THREADS), BWD_THREADS, 0, s>>>(vp, n_views, raw, src, n, means, scales, quats, radii, clamped, row_index,
+                                                                      v_means, v_scales, (float4*)v_quats, v_shs_dc);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
 int launch_sh_fwd(int degree, int stride, int64_t n, const float* dirs, const float* coeffs, float* rgb, cudaStream_t s) {
     if (n == 0) return B200GS_OK;
-    if (degree > 3) sh_fwd_kernel<25><<<(unsigned)div_up64(n, 256), 256, 0, s>>>(degree, stride, n, dirs, coeffs, rgb);
-    else sh_fwd_kernel<16><<<(unsigned)div_up64(n, 256), 256, 0, s>>>(degree, stride, n, dirs, coeffs, rgb);
+    const auto kernel = degree > 3 ? sh_fwd_kernel<25> : sh_fwd_kernel<16>;
+    kernel<<<(unsigned)div_up64(n, 256), 256, 0, s>>>(degree, stride, n, dirs, coeffs, rgb);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
@@ -1359,8 +1316,8 @@ int launch_sh_fwd(int degree, int stride, int64_t n, const float* dirs, const fl
 int launch_sh_bwd(int degree, int stride, int64_t n, const float* dirs, const float* coeffs, const float* v_rgb,
                   float* v_coeffs, float* v_dirs, cudaStream_t s) {
     if (n == 0) return B200GS_OK;
-    if (degree > 3) sh_bwd_kernel<25><<<(unsigned)div_up64(n, 256), 256, 0, s>>>(degree, stride, n, dirs, coeffs, v_rgb, v_coeffs, v_dirs);
-    else sh_bwd_kernel<16><<<(unsigned)div_up64(n, 256), 256, 0, s>>>(degree, stride, n, dirs, coeffs, v_rgb, v_coeffs, v_dirs);
+    const auto kernel = degree > 3 ? sh_bwd_kernel<25> : sh_bwd_kernel<16>;
+    kernel<<<(unsigned)div_up64(n, 256), 256, 0, s>>>(degree, stride, n, dirs, coeffs, v_rgb, v_coeffs, v_dirs);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }

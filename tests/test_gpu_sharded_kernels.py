@@ -13,11 +13,15 @@ DEV = "cuda"
 COLS = ["x", "y", "depth", "conicA", "conicB", "conicC", "comp", "opacity", "r", "g", "b", "radius"]
 
 
-def _scene(n, seed, W, H, poses, sh_degree=3, aa=True):
+# (storage degree, active degree): SH stored with stride 16 or 25.  The multi-view K1 kernels take MC = 25 for an active degree of 4.
+SH_DEGREES = pytest.mark.parametrize(("storage_degree", "sh_degree"), [(3, 3), (4, 4), (4, 2)])
+
+
+def _scene(n, seed, W, H, poses, sh_degree=3, aa=True, storage_degree=3):
     from b200gs import ops
     from b200gs._lib import MODE_GSPLAT
     from b200gs.scene import make_ring_cameras, make_scene
-    raw = {k: v.to(DEV).contiguous() for k, v in make_scene(n, seed, mean_scale=0.03).items()}
+    raw = {k: v.to(DEV).contiguous() for k, v in make_scene(n, seed, mean_scale=0.03, sh_degree=storage_degree).items()}
     cams = [make_ring_cameras(W, H)[p].to_device(DEV) for p in poses]
     stride = int(raw["shs_dc"].shape[1] + raw["shs_rest"].shape[1])
     views = [ops.make_view(MODE_GSPLAT, W, H, fx=float(c.fx), fy=float(c.fy), cx=float(c.cx), cy=float(c.cy), viewmatrix=c.world_to_camera,
@@ -61,13 +65,14 @@ def _assert_camera_arrays_match_rows(j, n, xy, depth, conic, opac, rgb, radii, c
     assert not bad, f"camera {j}: multi-view arrays differ from the single-view rows: {bad}"
 
 
+@SH_DEGREES
 @pytest.mark.parametrize("aa", [True, False])
-def test_multi_view_kernels_match_single_view_rows_bitwise(aa):
+def test_multi_view_kernels_match_single_view_rows_bitwise(aa, storage_degree, sh_degree):
     from b200gs import ops
     from b200gs._lib import B200gsView, check, lib, ptr
     L = lib()
     n, W, H = 20000, 400, 304
-    raw, views = _scene(n, 21, W, H, [0, 3, 4])
+    raw, views = _scene(n, 21, W, H, [0, 3, 4], sh_degree, storage_degree=storage_degree)
     nv = len(views)
     ol = raw["opacities"].reshape(-1).contiguous()
     single = [_single_rows(raw, v, aa) for v in views]
@@ -161,14 +166,12 @@ def test_compacted_and_blocked_rows_render_bit_identically():
     assert torch.equal(img_b, img_full), float((img_b - img_full).abs().max())
 
 
-def test_multi_view_backward_matches_accumulated_single_view_backward():
-    """K8 for all cameras in one launch (project_bwd_multi_kernel: gradients summed per Gaussian, SH-gradient rows accumulated in the shared-memory
-    staging buffer) against the single-view K8 called once per camera with accumulate (b200gs_project_bwd_rows), same gradient rows."""
+def _check_multi_view_backward_against_accumulated_single_view(storage_degree, sh_degree):
     from b200gs import ops
     from b200gs._lib import B200gsView, check, lib, ptr
     L = lib()
     n, W, H = 20000, 400, 304
-    raw, views = _scene(n, 21, W, H, [0, 3, 4])
+    raw, views = _scene(n, 21, W, H, [0, 3, 4], sh_degree, storage_degree=storage_degree)
     nv = len(views)
     ol = raw["opacities"].reshape(-1).contiguous()
     single = [_single_rows(raw, v, True) for v in views]
@@ -198,3 +201,16 @@ def test_multi_view_backward_matches_accumulated_single_view_backward():
         assert bool(torch.isfinite(a).all())
         err = float((a - b).abs().max() / b.abs().max().clamp_min(1e-30))
         assert err < 2e-5, (name, err)
+
+
+def test_multi_view_backward_matches_accumulated_single_view_backward():
+    """K8 for all cameras in one launch (project_bwd_multi_kernel: gradients summed per Gaussian, SH-gradient rows accumulated in the shared-memory
+    staging buffer) against the single-view K8 called once per camera with accumulate (b200gs_project_bwd_rows), same gradient rows."""
+    _check_multi_view_backward_against_accumulated_single_view(3, 3)
+
+
+@pytest.mark.parametrize(("storage_degree", "sh_degree"), [(4, 4), (4, 2)])
+def test_multi_view_backward_matches_accumulated_single_view_backward_sh_stride_25(storage_degree, sh_degree):
+    """The same with SH stored with stride 25: the multi-view K8 takes its MC = 25 instantiation for both active degrees.  At active degree 2
+    the single-view K8 evaluates 16 coefficients and writes the wider rows per thread, where accumulate must add to them."""
+    _check_multi_view_backward_against_accumulated_single_view(storage_degree, sh_degree)
