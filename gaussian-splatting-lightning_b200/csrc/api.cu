@@ -41,7 +41,7 @@ using namespace b200gs;
 extern "C" {
 
 const char* b200gs_last_error(void) { return g_error; }
-int b200gs_version(void) { return 222; }
+int b200gs_version(void) { return 223; }
 int64_t b200gs_launch_count(void) { return (int64_t)g_launches.load(std::memory_order_relaxed); }
 
 int b200gs_project_fwd(const B200gsView* view, int64_t n, const float* means, const float* scales, const float* quats,
@@ -277,7 +277,7 @@ int b200gs_bin_count(int32_t mode, int32_t width, int32_t height, int64_t n, con
     B200GS_CHECK_ARG(n == 0 || (xy && depth && radii), "NULL pointer");
     B200GS_CHECK_ARG(n < (int64_t(1) << 31), "n >= 2^31");
     B200GS_CHECK_ARG((cull_conic == nullptr) == (cull_opacity == nullptr), "cull_conic and cull_opacity go together");
-    return bin_count(mode, width, height, n, 0, xy, depth, radii, cull_conic, cull_opacity, workspace, workspace_bytes, d_counts,
+    return bin_count(mode, width, height, n, false, xy, depth, radii, cull_conic, cull_opacity, workspace, workspace_bytes, d_counts,
                      host_counts, sync_host, (cudaStream_t)stream);
 }
 
@@ -374,9 +374,9 @@ int b200gs_bin_count_rows(int32_t mode, int32_t width, int32_t height, int64_t n
     B200GS_CHECK_ARG(mode == B200GS_MODE_VANILLA || mode == B200GS_MODE_GSPLAT, "bad mode");
     B200GS_CHECK_ARG(width > 0 && height > 0 && n >= 0 && n < (int64_t(1) << 31), "bad size");
     B200GS_CHECK_ARG(workspace && d_counts && (n == 0 || rows), "NULL pointer");
-    return bin_count(mode, width, height, n, B200GS_ROW_FLOATS, rows + B200GS_ROW_XY, rows + B200GS_ROW_DEPTH,
-                     (const int32_t*)(rows + B200GS_ROW_RADIUS), cull ? rows + B200GS_ROW_CONIC : nullptr,
-                     cull ? rows + B200GS_ROW_OPACITY : nullptr, workspace, workspace_bytes, d_counts, host_counts, sync_host,
+    B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(rows) & 15u) == 0, "rows must be 16-byte aligned");
+    return bin_count(mode, width, height, n, true, rows + B200GS_ROW_XY, rows + B200GS_ROW_DEPTH, (const int32_t*)(rows + B200GS_ROW_RADIUS),
+                     rows + B200GS_ROW_CONIC, rows + B200GS_ROW_OPACITY, workspace, workspace_bytes, d_counts, host_counts, sync_host,
                      (cudaStream_t)stream, block_counts, block_rows);
 }
 

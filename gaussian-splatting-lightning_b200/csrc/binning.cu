@@ -18,9 +18,9 @@
 // A stable multi-split keeps the depth order inside every tile, so the result equals the oracle's torch.sort(stable)
 // of the 64-bit keys element for element (tests/test_gpu_parity.py::test_binning_exact).
 //
-// Every kernel here is ours, including the device-wide primitives (onesweep.cuh: chained scan, onesweep radix passes):
+// Every kernel here is ours, including the device-wide primitives (onesweep.cuh: block and chained scans, onesweep radix passes):
 //   phase A  depth_keys (order-preserving compaction of the visible Gaussians through a chained scan; {depth key, id} records
-//            + the 32-byte record)  ->  hist4  ->  4 onesweep passes over the V visible records
+//            + the 32-byte record + the key-byte histograms)  ->  4 onesweep passes over the V visible records
 //   phase B  emit_cells (chained scan of the coarse-cell counts in depth order; per-cell histogram)  ->  cell_table (cell
 //            ranges, chunk table, digit histograms)  ->  1 onesweep pass by cell (2 above 256 cells)  ->  chunk_counts  ->
 //            chunk_prefix  ->  scatter_ids
@@ -52,66 +52,8 @@ constexpr int CELL_IPT = 4;                          // records per thread of a 
 constexpr int DEPTH_TILE = sweep::PASS_THREADS * DEPTH_IPT;
 constexpr int CELL_TILE = sweep::PASS_THREADS * CELL_IPT;
 
-struct LayoutA {
-    size_t rec_a, rec_b, recs, zero, zero_bytes, hist, tickets, scan_state, lookback, total;
-    int64_t tiles, blocks;
-};
-struct LayoutB {
-    size_t entries_in, entries, offsets, zero, zero_bytes, cell_hist, tickets, scan_state, lookback, digit_hist, cell_ranges, chunk_base, chunk_cell,
-        chunk_cnt, chunk_pre, tile_start, total;
-    int64_t max_chunks, tiles, blocks, scan_blocks;
-};
-
-inline int bits_for(int n_values) {
-    int b = 1;
-    while ((1 << b) < n_values) ++b;
-    return b;
-}
-
-struct Taker {
-    size_t off = 0;
-    size_t operator()(size_t bytes) {
-        size_t o = off;
-        off = align_up(off + bytes, 256);
-        return o;
-    }
-};
-
-LayoutA make_layout_a(int64_t n) {
-    static thread_local int64_t cached_n = -1;
-    static thread_local LayoutA cached{};
-    if (n == cached_n) return cached;
-    LayoutA L{};
-    Taker take;
-    const size_t nn = (size_t)(n > 0 ? n : 1);
-    L.tiles = (int64_t)div_up64((int64_t)nn, DEPTH_TILE);
-    L.blocks = (int64_t)div_up64((int64_t)nn, 256 * 8);      // depth_keys_kernel: 256 threads x DK_ITEMS Gaussians
-    L.rec_a = take(nn * 8);
-    L.rec_b = take(nn * 8);
-    L.recs = take(nn * sizeof(SplatRec));
-    // one contiguous zero-initialised region: digit histograms, tickets, chained-scan state, look-back words of the 4 passes
-    L.zero = take(0);
-    L.hist = take(4 * sweep::RADIX * 4);
-    L.tickets = take(16 * 4);
-    L.scan_state = take((size_t)L.blocks * 4);
-    L.lookback = take((size_t)4 * L.tiles * sweep::RADIX * 4);
-    L.zero_bytes = take.off - L.zero;
-    L.total = take.off;
-    cached = L;
-    cached_n = n;
-    return L;
-}
-
-// The sort payload is the Gaussian id; when the id fits 24 bits and a rect can cover at most 255 coarse cells, the cell count of the
-// rect rides in the top byte ({key, ncells << 24 | id}): rank_offsets then reads its counts from the sorted records it streams through
-// anyway instead of gathering one random 32-byte sector per rank (one L2 request per rank: most of that kernel's time).  Decided from
-// (n, width, height) alone, so bin_count and bin_sort agree.
-inline bool pack_ncells(int64_t n, int width, int height) {
-    const int gx = div_up(width, TILE), gy = div_up(height, TILE);
-    const int cells = div_up(gx, 1 << 3) * div_up(gy, 1 << 3);
-    return n < (int64_t(1) << 24) && cells <= 255;
-}
-constexpr uint32_t ID_MASK = (1u << 24) - 1u;
+constexpr int DK_ITEMS = 8;                          // Gaussians per thread of depth_keys_kernel
+constexpr int RO_ITEMS = 8;                          // ranks per thread of rank_offsets_kernel
 
 inline void cell_grid(int width, int height, int& grid_x, int& grid_y, int& cgrid_x, int& cgrid_y) {
     grid_x = div_up(width, TILE);
@@ -120,44 +62,95 @@ inline void cell_grid(int width, int height, int& grid_x, int& grid_y, int& cgri
     cgrid_y = div_up(grid_y, SUPER);
 }
 
-LayoutB make_layout_b(int64_t n, int64_t max_coarse, int width, int height) {
-    static thread_local int64_t cached_p = -1, cached_n = -1;
-    static thread_local int cached_w = -1, cached_h = -1;
-    static thread_local LayoutB cached{};
-    if (max_coarse == cached_p && n == cached_n && width == cached_w && height == cached_h) return cached;
+// The sort payload is the Gaussian id; when the id fits 24 bits and a rect can cover at most 255 coarse cells, the cell count of the
+// rect rides in the top byte ({key, ncells << 24 | id}): rank_offsets then reads its counts from the sorted records it streams through
+// anyway instead of gathering one random 32-byte sector per rank (one L2 request per rank: most of that kernel's time).  Decided from
+// (n, width, height) alone, so bin_count and bin_sort agree.
+inline bool pack_ncells(int64_t n, int width, int height) {
+    int grid_x, grid_y, cgrid_x, cgrid_y;
+    cell_grid(width, height, grid_x, grid_y, cgrid_x, cgrid_y);
+    return n < (int64_t(1) << 24) && cgrid_x * cgrid_y <= 255;
+}
+constexpr uint32_t ID_MASK = (1u << 24) - 1u;
+
+// Hands out consecutive 256-byte aligned pieces of a workspace.  With a null base only `off`, the size so far, is meaningful.
+struct Carver {
+    uintptr_t base;
+    size_t off = 0;
+    template <typename T>
+    T* take(size_t count) {
+        T* p = reinterpret_cast<T*>(base + off);
+        off = align_up(off + count * sizeof(T), 256);
+        return p;
+    }
+};
+
+// Workspace of phase A (n Gaussians).  Phase B reads the sorted records (rec_a after the four passes) and the 32-byte records.
+struct WorkspaceA {
+    uint2* rec_a; uint2* rec_b; SplatRec* recs;
+    uint32_t* hist; uint32_t* tickets; uint32_t* scan_state; uint32_t* lookback;   // one zero-initialised region of zero_bytes from hist
+    size_t zero_bytes, bytes;
+    int64_t tiles, blocks;
+};
+
+WorkspaceA carve_a(void* base, int64_t n) {
+    WorkspaceA W;
+    Carver c{reinterpret_cast<uintptr_t>(base)};
+    const size_t nn = (size_t)(n > 0 ? n : 1);
+    W.tiles = div_up64((int64_t)nn, DEPTH_TILE);
+    W.blocks = div_up64((int64_t)nn, 256 * DK_ITEMS);
+    W.rec_a = c.take<uint2>(nn);
+    W.rec_b = c.take<uint2>(nn);
+    W.recs = c.take<SplatRec>(nn);
+    const size_t zero = c.off;
+    W.hist = c.take<uint32_t>(4 * sweep::RADIX);      // digit histograms, tickets, chained-scan state, look-back words of the 4 passes
+    W.tickets = c.take<uint32_t>(16);
+    W.scan_state = c.take<uint32_t>((size_t)W.blocks);
+    W.lookback = c.take<uint32_t>((size_t)4 * W.tiles * sweep::RADIX);
+    W.zero_bytes = c.off - zero;
+    W.bytes = c.off;
+    return W;
+}
+
+// Workspace of phase B (n Gaussians, up to max_coarse coarse entries).
+struct WorkspaceB {
+    CellEntry* entries_in; CellEntry* entries; uint32_t* offsets;
+    uint32_t* cell_hist; uint32_t* tickets; uint32_t* scan_state; uint32_t* lookback;   // one zero-initialised region of zero_bytes from cell_hist
+    uint32_t* digit_hist; int2* cell_ranges; int32_t* chunk_base; int32_t* chunk_cell; uint16_t* chunk_cnt; uint32_t* chunk_pre;
+    int64_t* tile_start;
+    size_t zero_bytes, bytes;
+    int64_t max_chunks, tiles, blocks, scan_blocks;
+};
+
+WorkspaceB carve_b(void* base, int64_t n, int64_t max_coarse, int width, int height) {
     int grid_x, grid_y, cgrid_x, cgrid_y;
     cell_grid(width, height, grid_x, grid_y, cgrid_x, cgrid_y);
     const size_t n_cells = (size_t)cgrid_x * cgrid_y, n_tiles = (size_t)grid_x * grid_y;
-    LayoutB L{};
-    Taker take;
-    const size_t pp = (size_t)(max_coarse > 0 ? max_coarse : 1);
-    L.max_chunks = (int64_t)(pp / CHUNK + n_cells + 1);
-    L.tiles = (int64_t)div_up64((int64_t)pp, CELL_TILE);
-    L.blocks = (int64_t)div_up64(n > 0 ? n : 1, 256);
-    L.scan_blocks = (int64_t)div_up64(n > 0 ? n : 1, 256 * 8);   // rank_offsets_kernel: 256 threads x RO_ITEMS ranks
-    L.entries_in = take(pp * sizeof(CellEntry));
-    L.entries = take(pp * sizeof(CellEntry));
-    L.offsets = take((size_t)(n > 0 ? n : 1) * 4);
-    L.zero = take(0);
-    L.cell_hist = take(n_cells * 4);
-    L.tickets = take(16 * 4);
-    L.scan_state = take((size_t)L.scan_blocks * 4);
-    L.lookback = take((size_t)2 * L.tiles * sweep::RADIX * 4);
-    L.zero_bytes = take.off - L.zero;
-    L.digit_hist = take(2 * sweep::RADIX * 4);
-    L.cell_ranges = take(n_cells * 8);
-    L.chunk_base = take((n_cells + 1) * 4);
-    L.chunk_cell = take((size_t)L.max_chunks * 4);
-    L.chunk_cnt = take((size_t)L.max_chunks * CELL_TILES * 2);
-    L.chunk_pre = take((size_t)L.max_chunks * CELL_TILES * 4);
-    L.tile_start = take(n_tiles * 8);
-    L.total = take.off;
-    cached = L;
-    cached_p = max_coarse;
-    cached_n = n;
-    cached_w = width;
-    cached_h = height;
-    return cached;
+    WorkspaceB W;
+    Carver c{reinterpret_cast<uintptr_t>(base)};
+    const size_t pp = (size_t)(max_coarse > 0 ? max_coarse : 1), nn = (size_t)(n > 0 ? n : 1);
+    W.max_chunks = (int64_t)(pp / CHUNK + n_cells + 1);
+    W.tiles = div_up64((int64_t)pp, CELL_TILE);
+    W.blocks = div_up64((int64_t)nn, 256);
+    W.scan_blocks = div_up64((int64_t)nn, 256 * RO_ITEMS);
+    W.entries_in = c.take<CellEntry>(pp);
+    W.entries = c.take<CellEntry>(pp);
+    W.offsets = c.take<uint32_t>(nn);
+    const size_t zero = c.off;
+    W.cell_hist = c.take<uint32_t>(n_cells);
+    W.tickets = c.take<uint32_t>(16);
+    W.scan_state = c.take<uint32_t>((size_t)W.scan_blocks);
+    W.lookback = c.take<uint32_t>((size_t)2 * W.tiles * sweep::RADIX);
+    W.zero_bytes = c.off - zero;
+    W.digit_hist = c.take<uint32_t>(2 * sweep::RADIX);
+    W.cell_ranges = c.take<int2>(n_cells);
+    W.chunk_base = c.take<int32_t>(n_cells + 1);
+    W.chunk_cell = c.take<int32_t>((size_t)W.max_chunks);
+    W.chunk_cnt = c.take<uint16_t>((size_t)W.max_chunks * CELL_TILES);
+    W.chunk_pre = c.take<uint32_t>((size_t)W.max_chunks * CELL_TILES);
+    W.tile_start = c.take<int64_t>(n_tiles);
+    W.bytes = c.off;
+    return W;
 }
 
 // ---- exact tile culling ------------------------------------------------------------------------------------------------
@@ -171,23 +164,13 @@ LayoutB make_layout_b(int64_t n, int64_t max_coarse, int width, int height) {
 // relative margin of 1e-4 (+1e-3), the interval a 0.01 px slack — orders of magnitude above the error of the
 // approximate sqrt used here and of the fp32 / ex2.approx rounding of the blend loop.  Each pair's verdict is computed
 // exactly once (emit_cells_kernel) and travels with the pair, so no two kernels ever have to agree on it.
-// Per-Gaussian inputs of phase A, with element strides: separate contiguous arrays ({2,1,1,3,1}) or columns of one
-// [n,12] row buffer ({12,12,12,12,12}).
+// Per-Gaussian inputs of phase A: separate contiguous arrays xy[n,2], depth[n], radii[n], conic[n,3], opacity[n] (conic and
+// opacity NULL without culling), or the columns of one [n,12] row buffer.  Rows may arrive in fixed-size blocks (the sharded
+// exchange): block b holds blk_cnt[b] valid rows, the rest of its blk_rows rows is stale memory and reads as culled — no padding
+// pass over the receive buffer.
 struct BinSrc {
     const float* xy; const float* depth; const int32_t* radii; const float* conic; const float* opacity;
-    int xs, ds, rs, cs, os;
-    // rows that arrive in fixed-size blocks (the sharded exchange): block b holds blk_cnt[b] valid rows, the rest of its blk_rows
-    // rows is stale memory and reads as culled — no padding pass over the receive buffer
     const int64_t* blk_cnt; int blk_rows;
-    __device__ __forceinline__ float2 get_xy(int64_t i) const { return *reinterpret_cast<const float2*>(xy + i * xs); }
-    __device__ __forceinline__ float get_depth(int64_t i) const { return depth[i * ds]; }
-    __device__ __forceinline__ int get_radius(int64_t i) const {
-        if (blk_cnt != nullptr) {
-            const int b = (int)i / blk_rows;
-            if ((int)i - b * blk_rows >= (int)blk_cnt[b]) return 0;
-        }
-        return radii[i * rs];
-    }
 };
 
 struct CullE {
@@ -272,10 +255,8 @@ __device__ __forceinline__ void coarsen_rect(int x0, int y0, int x1, int y1, int
 // only a handful of values in a scene, with warp-aggregated increments (match.any), the low bytes with plain shared-memory atomics.
 // counts[0] += tiles of the rect (the reference's pair count I: an upper bound of the culled count, exact without culling),
 // counts[1] += coarse cells, counts[3] = V.
-constexpr int DK_ITEMS = 8;
-
-// ROWS16: the inputs are the columns of one 16-byte aligned [n,12] row buffer (b200gs.h row layout): three 128-bit loads per Gaussian
-template <bool GSPLAT, bool ROWS16>
+// ROWS: the inputs are the columns of one 16-byte aligned [n,12] row buffer (b200gs.h row layout): three 128-bit loads per Gaussian
+template <bool GSPLAT, bool ROWS>
 __global__ void __launch_bounds__(256) depth_keys_kernel(int64_t n, int grid_x, int grid_y, int pack, const BinSrc src, uint2* __restrict__ keyrec,
                                                          SplatRec* __restrict__ recs, uint32_t* __restrict__ ticket,
                                                          uint32_t* __restrict__ scan_state, uint32_t* __restrict__ hist,
@@ -305,7 +286,7 @@ __global__ void __launch_bounds__(256) depth_keys_kernel(int64_t n, int grid_x, 
         if (i < n) {
             float px, py, dep, A = 1.f, B = 0.f, C = 1.f, o = 1.f;
             int r;
-            if (ROWS16) {
+            if (ROWS) {
                 const float4* row = reinterpret_cast<const float4*>(src.xy + i * B200GS_ROW_FLOATS);
                 const float4 q0 = row[0], q1 = row[1], q2 = row[2];
                 px = q0.x; py = q0.y; dep = q0.z; A = q0.w; B = q1.x; C = q1.y; o = q1.w;
@@ -315,14 +296,13 @@ __global__ void __launch_bounds__(256) depth_keys_kernel(int64_t n, int grid_x, 
                     if ((int)i - b * src.blk_rows >= (int)src.blk_cnt[b]) r = 0;
                 }
             } else {
-                r = src.get_radius(i);
-                const float2 pp = src.get_xy(i);
+                r = src.radii[i];
+                const float2 pp = reinterpret_cast<const float2*>(src.xy)[i];
                 px = pp.x; py = pp.y;
-                dep = src.get_depth(i);
+                dep = src.depth[i];
                 if (src.conic != nullptr) {
-                    const float* q = src.conic + i * src.cs;
-                    A = q[0]; B = q[1]; C = q[2];
-                    o = src.opacity[i * src.os];
+                    A = src.conic[3 * i]; B = src.conic[3 * i + 1]; C = src.conic[3 * i + 2];
+                    o = src.opacity[i];
                 }
             }
             if (r > 0) {
@@ -361,12 +341,7 @@ __global__ void __launch_bounds__(256) depth_keys_kernel(int64_t n, int grid_x, 
     __syncthreads();
     if (threadIdx.x < 32) {     // warp 0: scan of the 64 (round, warp) counts, then the warp-wide look-back over the preceding blocks
         const int c0 = s_cnt[2 * lane], c1 = s_cnt[2 * lane + 1];
-        int inc = c0 + c1;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int v = __shfl_up_sync(0xffffffffu, inc, o);
-            if ((int)lane >= o) inc += v;
-        }
+        const int inc = sweep::warp_inclusive(c0 + c1);
         const int block_vis = __shfl_sync(0xffffffffu, inc, 31);
         s_cnt[2 * lane] = inc - c0 - c1;
         s_cnt[2 * lane + 1] = inc - c1;
@@ -406,17 +381,10 @@ __global__ void __launch_bounds__(256) depth_keys_kernel(int64_t n, int grid_x, 
 
 // Exclusive prefix of the coarse-cell counts over the depth-ranked Gaussians: offsets[rank] = first entry slot of that rank.  Big
 // tiles (RO_ITEMS consecutive ranks per thread) for the same reason as above; the cell count of a rank is gathered from its record.
-constexpr int RO_ITEMS = 8;
-
 __global__ void __launch_bounds__(256) rank_offsets_kernel(const int64_t* __restrict__ d_visible, int pack, const uint2* __restrict__ order,
                                                           const SplatRec* __restrict__ recs, uint32_t* __restrict__ offsets,
                                                           uint32_t* __restrict__ ticket, uint32_t* __restrict__ scan_state) {
-    __shared__ int s_scan[sweep::WARPS + 1];
-    __shared__ int s_tile;
-    __shared__ uint32_t s_excl;
-    if (threadIdx.x == 0) s_tile = (int)atomicAdd(ticket, 1u);
-    __syncthreads();
-    const int t = s_tile;
+    const int t = sweep::block_ticket(ticket);
     const int64_t n = *d_visible;
     const int64_t r0 = (int64_t(t) * blockDim.x + threadIdx.x) * RO_ITEMS;
     if (int64_t(t) * blockDim.x * RO_ITEMS >= n) return;
@@ -431,14 +399,7 @@ __global__ void __launch_bounds__(256) rank_offsets_kernel(const int64_t* __rest
         }
         mine += nc[k];
     }
-    int block_total;
-    int local = sweep::block_exclusive(mine, s_scan, &block_total);
-    if (threadIdx.x < 32) {
-        const uint32_t excl = sweep::chained_exclusive(scan_state, t, (uint32_t)block_total);
-        if (threadIdx.x == 0) s_excl = excl;
-    }
-    __syncthreads();
-    uint32_t run = s_excl + (uint32_t)local;
+    uint32_t run = sweep::chained_block_exclusive<8>(mine, scan_state, t);
 #pragma unroll
     for (int k = 0; k < RO_ITEMS; ++k) {
         if (r0 + k < n) offsets[r0 + k] = run;
@@ -467,12 +428,11 @@ __global__ void __launch_bounds__(256) emit_cells_kernel(const int64_t* __restri
     __shared__ unsigned long long s_mask[EMIT_SLOTS];
     __shared__ float s_f[8][256];        // mx, my, B, iA, two_tA, det, ymax, yR
     __shared__ int s_mode[256], s_xr[256], s_yr[256], s_start[256];   // x0 | x1 << 16, y0 | y1 << 16, first slot - block_lo
-    __shared__ int s_rowoff[260];
+    __shared__ int s_rowoff[256];
     __shared__ unsigned char s_item[EMIT_ITEMS];   // work item -> rank of the block (when the block has <= EMIT_ITEMS tile rows)
-    __shared__ int s_warp[8];
+    __shared__ int s_warp[9];
     __shared__ uint32_t s_hist[EMIT_HIST];
     const int tid = threadIdx.x;
-    const unsigned lane = tid & 31u, w = tid >> 5;
     const int64_t n = *d_visible;
     const int64_t rank0 = int64_t(blockIdx.x) * blockDim.x;
     if (rank0 >= n) return;
@@ -502,22 +462,8 @@ __global__ void __launch_bounds__(256) emit_cells_kernel(const int64_t* __restri
     const uint32_t last_y = order[last_rank].y;
     const int block_cells = (int)((int64_t)offsets[last_rank] + (pack ? (int)(last_y >> 24) : __ldg(&recs[last_y].ncells)) - block_lo);
     const int local_start = (rnk < n) ? (int)((int64_t)offsets[rnk] - block_lo) : block_cells;
-    // exclusive scan of the row counts
-    int inc = nrows;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int v = __shfl_up_sync(0xffffffffu, inc, o);
-        if ((int)lane >= o) inc += v;
-    }
-    if (lane == 31) s_warp[w] = inc;
-    __syncthreads();
-    int wbase = 0;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) wbase += (k < (int)w) ? s_warp[k] : 0;
-    __syncthreads();   // every warp has read s_warp before anything below is stored (racecheck: a slow warp's read of
-                       // s_warp raced with the stores that follow in a fast warp)
-    s_rowoff[tid] = wbase + inc - nrows;
-    if (tid == 255) s_rowoff[256] = wbase + inc;
+    int total_rows;
+    s_rowoff[tid] = sweep::block_exclusive<int, 8>(nrows, s_warp, &total_rows);   // exclusive scan of the row counts
     s_f[0][tid] = e.mx; s_f[1][tid] = e.my; s_f[2][tid] = e.B; s_f[3][tid] = e.iA;
     s_f[4][tid] = e.two_tA; s_f[5][tid] = e.det; s_f[6][tid] = e.ymax; s_f[7][tid] = e.yR;
     s_mode[tid] = e.mode;
@@ -527,7 +473,6 @@ __global__ void __launch_bounds__(256) emit_cells_kernel(const int64_t* __restri
     const int cx0 = x0 >> SUPER_SHIFT, cy0 = y0 >> SUPER_SHIFT;
     const int cw = t > 0 ? ((x1 - 1) >> SUPER_SHIFT) - cx0 + 1 : 1;
     __syncthreads();
-    const int total_rows = s_rowoff[256];
     const bool item_table = total_rows <= EMIT_ITEMS;
     if (item_table) {     // rank tid owns items [s_rowoff[tid], s_rowoff[tid] + nrows)
         const int o = s_rowoff[tid];
@@ -603,13 +548,12 @@ __global__ void __launch_bounds__(256) emit_cells_kernel(const int64_t* __restri
 __global__ void __launch_bounds__(1024) cell_table_kernel(int n_cells, const uint32_t* __restrict__ cell_hist, int2* __restrict__ cell_ranges,
                                                           int32_t* __restrict__ chunk_base, int32_t* __restrict__ chunk_cell,
                                                           uint32_t* __restrict__ digit_hist, int n_tiles, int64_t* __restrict__ tile_total) {
-    __shared__ int s_warp[32], s_warp2[32];
-    __shared__ int s_carry, s_carry2;
+    __shared__ int s_warp[33];
     __shared__ uint32_t s_dh[2][sweep::RADIX];
-    const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-    if (tid == 0) { s_carry = 0; s_carry2 = 0; }
+    const int tid = threadIdx.x;
     for (int i = tid; i < 2 * sweep::RADIX; i += 1024) (&s_dh[0][0])[i] = 0;
     __syncthreads();
+    int total = 0, entries = 0;     // chunks / entries of the cells before this round
     for (int base = 0; base < n_cells; base += 1024) {
         const int i = base + tid;
         int cnt = 0, v = 0;
@@ -618,38 +562,16 @@ __global__ void __launch_bounds__(1024) cell_table_kernel(int n_cells, const uin
             v = (cnt + CHUNK - 1) / CHUNK;
             if (cnt) { atomicAdd(&s_dh[0][i & 255], (uint32_t)cnt); atomicAdd(&s_dh[1][(i >> 8) & 255], (uint32_t)cnt); }
         }
-        int inc = v, inc2 = cnt;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int t = __shfl_up_sync(0xffffffffu, inc, o);
-            const int t2 = __shfl_up_sync(0xffffffffu, inc2, o);
-            if (lane >= o) { inc += t; inc2 += t2; }
-        }
-        if (lane == 31) { s_warp[w] = inc; s_warp2[w] = inc2; }
-        __syncthreads();
-        if (w == 0) {
-            int ws = s_warp[lane], winc = ws, ws2 = s_warp2[lane], winc2 = ws2;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int t = __shfl_up_sync(0xffffffffu, winc, o);
-                const int t2 = __shfl_up_sync(0xffffffffu, winc2, o);
-                if (lane >= o) { winc += t; winc2 += t2; }
-            }
-            s_warp[lane] = winc - ws;
-            s_warp2[lane] = winc2 - ws2;
-        }
-        __syncthreads();
-        const int excl = s_carry + s_warp[w] + inc - v;
-        const int excl2 = s_carry2 + s_warp2[w] + inc2 - cnt;
+        int round_chunks, round_entries;
+        const int excl = total + sweep::block_exclusive<int, 32>(v, s_warp, &round_chunks);
+        const int excl2 = entries + sweep::block_exclusive<int, 32>(cnt, s_warp, &round_entries);
         if (i < n_cells) {
             chunk_base[i] = excl;
             cell_ranges[i] = cnt > 0 ? make_int2(excl2, excl2 + cnt) : make_int2(0, 0);
         }
-        __syncthreads();
-        if (tid == 1023) { s_carry = excl + v; s_carry2 = excl2 + cnt; }
-        __syncthreads();
+        total += round_chunks;
+        entries += round_entries;
     }
-    const int total = s_carry;
     if (tid == 0) chunk_base[n_cells] = total;
     for (int i = tid; i < 2 * sweep::RADIX; i += 1024) digit_hist[i] = (&s_dh[0][0])[i];
     for (int i = tid; i < n_tiles; i += 1024) tile_total[i] = 0;    // accumulated by chunk_counts_kernel
@@ -682,9 +604,42 @@ __device__ __forceinline__ uint32_t transpose32(uint32_t x, unsigned lane) {
     return x;
 }
 
-// Phase C: one block per chunk (256 consecutive entries of one cell's depth-ordered list): per-tile entry counts.
-// Each warp transposes the masks of its 32 entries: lane t then holds, for tiles t and t+32, the bit set of the warp's
-// entries that reach the tile.
+// Prologue of phases C and E, one block per chunk c (CHUNK consecutive entries of one cell's depth-ordered list): thread i loads
+// entry i of the chunk (with IDS it also stores its Gaussian id to s_id[i]; without, it reads the masks only: half the bytes).
+// Each warp transposes the masks of its 32 entries: lane t then holds in wlo / whi, for tiles t and t+32, the bit set of the
+// warp's entries that reach the tile, and s_cnt[warp][tile] = its popcount.  Returns the chunk's cell.
+template <bool IDS>
+__device__ __forceinline__ int load_chunk(int c, const int2* __restrict__ cell_ranges, const int32_t* __restrict__ chunk_base,
+                                          const int32_t* __restrict__ chunk_cell, const CellEntry* __restrict__ entries,
+                                          uint16_t (*s_cnt)[CELL_TILES], int32_t* s_id, uint32_t& wlo, uint32_t& whi) {
+    const int cell = __ldg(chunk_cell + c);
+    const int2 r = cell_ranges[cell];
+    const int e = r.x + (c - __ldg(chunk_base + cell)) * CHUNK + (int)threadIdx.x;
+    const unsigned lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+    uint32_t lo = 0, hi = 0;
+    if (e < r.y) {
+        if (IDS) {
+            const uint4 v = __ldg(entries + e);
+            lo = v.x; hi = v.y;
+            s_id[threadIdx.x] = (int)v.z;
+        } else {
+            const uint2 m = __ldg(reinterpret_cast<const uint2*>(entries + e));
+            lo = m.x; hi = m.y;
+        }
+    }
+    wlo = transpose32(lo, lane);
+    whi = transpose32(hi, lane);
+    s_cnt[w][lane] = (uint16_t)__popc(wlo);
+    s_cnt[w][lane + 32] = (uint16_t)__popc(whi);
+    return cell;
+}
+
+// tile t of a coarse cell (bit t of its masks) -> tile coordinates
+__device__ __forceinline__ int2 cell_tile(int cell, int t, int cgrid_x) {
+    return make_int2(((cell % cgrid_x) << SUPER_SHIFT) + (t & (SUPER - 1)), ((cell / cgrid_x) << SUPER_SHIFT) + (t >> SUPER_SHIFT));
+}
+
+// Phase C: per-tile entry counts of every chunk.
 __global__ void __launch_bounds__(CHUNK) chunk_counts_kernel(int n_cells, int cgrid_x, int grid_x, int grid_y, const int2* __restrict__ cell_ranges,
                                                              const int32_t* __restrict__ chunk_base, const int32_t* __restrict__ chunk_cell,
                                                              const CellEntry* __restrict__ entries, uint16_t* __restrict__ chunk_cnt,
@@ -692,28 +647,17 @@ __global__ void __launch_bounds__(CHUNK) chunk_counts_kernel(int n_cells, int cg
     __shared__ uint16_t s_cnt[CHUNK / 32][CELL_TILES];
     const int c = blockIdx.x;
     if (c >= __ldg(chunk_base + n_cells)) return;
-    const int cell = __ldg(chunk_cell + c);
-    const int2 r = cell_ranges[cell];
-    const int e = r.x + (c - __ldg(chunk_base + cell)) * CHUNK + (int)threadIdx.x;
-    const unsigned lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
-    uint32_t lo = 0, hi = 0;
-    if (e < r.y) {
-        const uint2 m = __ldg(reinterpret_cast<const uint2*>(entries + e));
-        lo = m.x; hi = m.y;
-    }
-    s_cnt[w][lane] = (uint16_t)__popc(transpose32(lo, lane));
-    s_cnt[w][lane + 32] = (uint16_t)__popc(transpose32(hi, lane));
+    uint32_t wlo, whi;
+    const int cell = load_chunk<false>(c, cell_ranges, chunk_base, chunk_cell, entries, s_cnt, nullptr, wlo, whi);
     __syncthreads();
     if (threadIdx.x < CELL_TILES) {
         int sum = 0;
 #pragma unroll
         for (int k = 0; k < CHUNK / 32; ++k) sum += s_cnt[k][threadIdx.x];
         chunk_cnt[int64_t(c) * CELL_TILES + threadIdx.x] = (uint16_t)sum;
-        const int t = threadIdx.x;
-        const int tx = ((cell % cgrid_x) << SUPER_SHIFT) + (t & (SUPER - 1));
-        const int ty = ((cell / cgrid_x) << SUPER_SHIFT) + (t >> SUPER_SHIFT);
-        if (sum > 0 && tx < grid_x && ty < grid_y)
-            atomicAdd(reinterpret_cast<unsigned long long*>(tile_total + int64_t(ty) * grid_x + tx), (unsigned long long)sum);
+        const int2 tile = cell_tile(cell, threadIdx.x, cgrid_x);
+        if (sum > 0 && tile.x < grid_x && tile.y < grid_y)
+            atomicAdd(reinterpret_cast<unsigned long long*>(tile_total + int64_t(tile.y) * grid_x + tile.x), (unsigned long long)sum);
     }
 }
 
@@ -727,7 +671,7 @@ __global__ void __launch_bounds__(1024) chunk_prefix_kernel(int n_cells, int n_t
                                                             int2* __restrict__ tile_ranges, int64_t* __restrict__ d_counts) {
     __shared__ uint32_t s_part[16][CELL_TILES];
     __shared__ int64_t s_warp[32];
-    __shared__ int64_t s_carry;
+    __shared__ int64_t s_carry;     // pairs of the tiles before this round
     const int tid = threadIdx.x;
     if ((int)blockIdx.x < n_cells) {
         const int cell = blockIdx.x;
@@ -771,8 +715,6 @@ __global__ void __launch_bounds__(1024) chunk_prefix_kernel(int n_cells, int n_t
         return;
     }
     if (tid == 0) s_carry = 0;
-    __syncthreads();
-    const int lane = tid & 31, w = tid >> 5;
     for (int base = 0; base < n_tiles; base += 8192) {
         const int i0 = base + tid * 8;
         int64_t v[8];
@@ -790,26 +732,8 @@ __global__ void __launch_bounds__(1024) chunk_prefix_kernel(int n_cells, int n_t
         int64_t sum = 0;
 #pragma unroll
         for (int k = 0; k < 8; ++k) sum += v[k];
-        int64_t inc = sum;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int64_t t = __shfl_up_sync(0xffffffffu, inc, o);
-            if (lane >= o) inc += t;
-        }
-        if (lane == 31) s_warp[w] = inc;
-        __syncthreads();
-        if (w == 0) {
-            const int64_t ws = s_warp[lane];
-            int64_t winc = ws;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int64_t t = __shfl_up_sync(0xffffffffu, winc, o);
-                if (lane >= o) winc += t;
-            }
-            s_warp[lane] = winc - ws;
-        }
-        __syncthreads();
-        int64_t run = s_carry + s_warp[w] + inc - sum;
+        int64_t run = sweep::block_exclusive<int64_t, 32>(sum, s_warp, nullptr);
+        run += s_carry;     // after the scan's barriers: the carry of the rounds before
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
             if (i0 + k < n_tiles) {
@@ -818,7 +742,7 @@ __global__ void __launch_bounds__(1024) chunk_prefix_kernel(int n_cells, int n_t
             }
             run += v[k];
         }
-        __syncthreads();
+        __syncthreads();    // every thread has read s_carry
         if (tid == 1023) s_carry = run;
         __syncthreads();
     }
@@ -847,37 +771,20 @@ __global__ void __launch_bounds__(CHUNK) scatter_ids_kernel(int n_cells, int cgr
     const int c = blockIdx.x;
     if (c >= __ldg(chunk_base + n_cells)) return;
     const unsigned lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
-    const int cell = __ldg(chunk_cell + c);
-    const int2 r = cell_ranges[cell];
-    const int e = r.x + (c - __ldg(chunk_base + cell)) * CHUNK + (int)threadIdx.x;
-    uint32_t mlo = 0, mhi = 0;
-    if (e < r.y) {
-        const uint4 v = __ldg(entries + e);
-        mlo = v.x; mhi = v.y;
-        s_id[threadIdx.x] = (int)v.z;
-    }
-    uint32_t wlo = transpose32(mlo, lane), whi = transpose32(mhi, lane);   // entries of this warp reaching tile lane / lane + 32
-    s_cnt[w][lane] = (uint16_t)__popc(wlo);
-    s_cnt[w][lane + 32] = (uint16_t)__popc(whi);
+    uint32_t wlo, whi;     // entries of this warp reaching tile lane / lane + 32
+    const int cell = load_chunk<true>(c, cell_ranges, chunk_base, chunk_cell, entries, s_cnt, s_id, wlo, whi);
     __syncthreads();
     if (threadIdx.x < CELL_TILES) {
         const int t = threadIdx.x;
-        const int tx = ((cell % cgrid_x) << SUPER_SHIFT) + (t & (SUPER - 1));
-        const int ty = ((cell / cgrid_x) << SUPER_SHIFT) + (t >> SUPER_SHIFT);
-        s_gbase[t] = (tx < grid_x && ty < grid_y) ? tile_start[int64_t(ty) * grid_x + tx] + chunk_pre[int64_t(c) * CELL_TILES + t] : 0;
+        const int2 tile = cell_tile(cell, t, cgrid_x);
+        s_gbase[t] = (tile.x < grid_x && tile.y < grid_y) ? tile_start[int64_t(tile.y) * grid_x + tile.x] + chunk_pre[int64_t(c) * CELL_TILES + t] : 0;
         int run = 0;
 #pragma unroll
         for (int k = 0; k < WARPS; ++k) {
             s_wbase[k][t] = run;
             run += s_cnt[k][t];
         }
-        int inc = run;   // inclusive scan of the tile totals inside each of the two warps
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int v = __shfl_up_sync(0xffffffffu, inc, o);
-            if ((int)lane >= o) inc += v;
-        }
-        s_off[t + 1] = inc;
+        s_off[t + 1] = sweep::warp_inclusive(run);   // inclusive scan of the tile totals inside each of the two warps
     }
     __syncthreads();
     const int half = s_off[32];       // total of tiles 0..31
@@ -911,52 +818,23 @@ __global__ void __launch_bounds__(CHUNK) scatter_ids_kernel(int n_cells, int cgr
 
 }  // namespace
 
-size_t bin_count_workspace_bytes(int64_t n) { return make_layout_a(n).total; }
-size_t bin_sort_workspace_bytes(int64_t n, int64_t max_coarse, int width, int height) { return make_layout_b(n, max_coarse, width, height).total; }
-
-static BinSrc make_src(int row_stride, const float* xy, const float* depth, const int32_t* radii, const float* conic, const float* opacity,
-                       const int64_t* block_counts, int64_t block_rows) {
-    if (block_rows <= 0) block_counts = nullptr;
-    if (row_stride > 0)
-        return BinSrc{xy, depth, radii, conic, opacity, row_stride, row_stride, row_stride, row_stride, row_stride, block_counts, (int)block_rows};
-    return BinSrc{xy, depth, radii, conic, opacity, 2, 1, 1, 3, 1, block_counts, (int)block_rows};
-}
+size_t bin_count_workspace_bytes(int64_t n) { return carve_a(nullptr, n).bytes; }
+size_t bin_sort_workspace_bytes(int64_t n, int64_t max_coarse, int width, int height) { return carve_b(nullptr, n, max_coarse, width, height).bytes; }
 
 // Counter read-back.  For pinned (mapped) host memory the counters are PUBLISHED by a kernel with system-scope stores
 // instead of a cudaMemcpyAsync: an in-stream D2H copy is serviced by a copy engine, and queues behind whatever bulk
 // transfer the application has in flight on it (e.g. the H2D prefetch of the next training image) — which would stall
 // the whole forward behind a 32-byte copy.  Pageable host memory falls back to the copy.
-__global__ void publish_counts_kernel(const int64_t* __restrict__ d_counts, volatile int64_t* __restrict__ host_counts) {
-    if (threadIdx.x < 4) host_counts[threadIdx.x] = d_counts[threadIdx.x];
-    __threadfence_system();
-}
-
 __global__ void publish_i64_kernel(const int64_t* __restrict__ src, volatile int64_t* __restrict__ dst, int n) {
     for (int i = threadIdx.x; i < n; i += blockDim.x) dst[i] = src[i];
     __threadfence_system();
-}
-
-static int copy_counts(const int64_t* d_counts, int64_t* host_counts, int sync_host, cudaStream_t s) {
-    if (host_counts != nullptr) {
-        cudaPointerAttributes attr{};
-        const cudaError_t e = cudaPointerGetAttributes(&attr, host_counts);
-        if (e == cudaSuccess && attr.type == cudaMemoryTypeHost && attr.devicePointer != nullptr) {
-            publish_counts_kernel<<<1, 32, 0, s>>>(d_counts, (volatile int64_t*)attr.devicePointer);
-            B200GS_LAUNCH_CHECK();
-        } else {
-            (void)cudaGetLastError();
-            B200GS_CUDA(cudaMemcpyAsync(host_counts, d_counts, 4 * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-        }
-        if (sync_host) B200GS_CUDA(cudaStreamSynchronize(s));
-    }
-    return B200GS_OK;
 }
 
 int publish_i64(const int64_t* d_values, int64_t* host_values, int n, cudaStream_t s) {
     cudaPointerAttributes attr{};
     const cudaError_t e = cudaPointerGetAttributes(&attr, host_values);
     if (e == cudaSuccess && attr.type == cudaMemoryTypeHost && attr.devicePointer != nullptr) {
-        publish_i64_kernel<<<1, 64, 0, s>>>(d_values, (volatile int64_t*)attr.devicePointer, n);
+        publish_i64_kernel<<<1, 32, 0, s>>>(d_values, (volatile int64_t*)attr.devicePointer, n);   // one warp: every warp pays for a fence
         B200GS_LAUNCH_CHECK();
     } else {
         (void)cudaGetLastError();
@@ -965,55 +843,52 @@ int publish_i64(const int64_t* d_values, int64_t* host_values, int n, cudaStream
     return B200GS_OK;
 }
 
-int bin_count(int mode, int width, int height, int64_t n, int row_stride, const float* xy, const float* depth, const int32_t* radii,
+// the four binning counters to host_counts (when given), then optionally wait for them
+static int publish_counts(const int64_t* d_counts, int64_t* host_counts, int sync_host, cudaStream_t s) {
+    if (host_counts == nullptr) return B200GS_OK;
+    const int rc = publish_i64(d_counts, host_counts, 4, s);
+    if (rc != B200GS_OK) return rc;
+    if (sync_host) B200GS_CUDA(cudaStreamSynchronize(s));
+    return B200GS_OK;
+}
+
+int bin_count(int mode, int width, int height, int64_t n, bool rows, const float* xy, const float* depth, const int32_t* radii,
               const float* conic, const float* opacity, void* ws, size_t ws_bytes, int64_t* d_counts, int64_t* host_counts,
               int sync_host, cudaStream_t s, const int64_t* block_counts, int64_t block_rows) {
-    const LayoutA L = make_layout_a(n);
-    if (ws_bytes < L.total) {
-        set_error("bin_count: workspace too small (%zu < %zu)", ws_bytes, L.total);
+    const WorkspaceA W = carve_a(ws, n);
+    if (ws_bytes < W.bytes) {
+        set_error("bin_count: workspace too small (%zu < %zu)", ws_bytes, W.bytes);
         return B200GS_ENOSPACE;
     }
     if (n >= (int64_t(1) << 30)) {
         set_error("bin_count: %lld Gaussians exceed the 2^30 limit of the look-back words", (long long)n);
         return B200GS_ENOSPACE;
     }
-    char* w = (char*)ws;
-    uint2* rec_a = (uint2*)(w + L.rec_a);
-    uint2* rec_b = (uint2*)(w + L.rec_b);
-    SplatRec* recs = (SplatRec*)(w + L.recs);
-    uint32_t* hist = (uint32_t*)(w + L.hist);
-    uint32_t* tickets = (uint32_t*)(w + L.tickets);
-    uint32_t* scan_state = (uint32_t*)(w + L.scan_state);
-    uint32_t* lookback = (uint32_t*)(w + L.lookback);
     const int grid_x = div_up(width, TILE), grid_y = div_up(height, TILE);
     B200GS_CUDA(cudaMemsetAsync(d_counts, 0, 4 * sizeof(int64_t), s));
     if (n > 0) {
-        B200GS_CUDA(cudaMemsetAsync(w + L.zero, 0, L.zero_bytes, s));
-        const unsigned blocks = (unsigned)L.blocks;
-        const BinSrc src = make_src(row_stride, xy, depth, radii, conic, opacity, block_counts, block_rows);
-        // all five inputs are columns of one 16-byte aligned [n,12] row buffer -> 128-bit row loads
-        const bool rows16 = row_stride == B200GS_ROW_FLOATS && conic != nullptr && depth == xy + B200GS_ROW_DEPTH && conic == xy + B200GS_ROW_CONIC &&
-                            opacity == xy + B200GS_ROW_OPACITY && reinterpret_cast<const float*>(radii) == xy + B200GS_ROW_RADIUS &&
-                            (reinterpret_cast<uintptr_t>(xy) & 15) == 0;
+        B200GS_CUDA(cudaMemsetAsync(W.hist, 0, W.zero_bytes, s));
+        const BinSrc src{xy, depth, radii, conic, opacity, block_rows > 0 ? block_counts : nullptr, (int)block_rows};
         const int pack = pack_ncells(n, width, height) ? 1 : 0;
-#define B200GS_DK_LAUNCH(G, R) depth_keys_kernel<G, R><<<blocks, 256, 0, s>>>(n, grid_x, grid_y, pack, src, rec_a, recs, tickets, scan_state, hist, (unsigned long long*)d_counts)
-        if (mode == B200GS_MODE_GSPLAT) { if (rows16) B200GS_DK_LAUNCH(true, true); else B200GS_DK_LAUNCH(true, false); }
-        else                            { if (rows16) B200GS_DK_LAUNCH(false, true); else B200GS_DK_LAUNCH(false, false); }
-#undef B200GS_DK_LAUNCH
+        static constexpr decltype(&depth_keys_kernel<false, false>) kernels[2][2] = {
+            {depth_keys_kernel<false, false>, depth_keys_kernel<false, true>}, {depth_keys_kernel<true, false>, depth_keys_kernel<true, true>}};
+        kernels[mode == B200GS_MODE_GSPLAT][rows]<<<(unsigned)W.blocks, 256, 0, s>>>(n, grid_x, grid_y, pack, src, W.rec_a, W.recs, W.tickets,
+                                                                                   W.scan_state, W.hist, (unsigned long long*)d_counts);
         B200GS_LAUNCH_CHECK();
         // stable LSD sort of the V visible {depth key, id} records (V = d_counts[3], known on the device only; byte histograms from above)
         const int64_t* d_visible = d_counts + 3;
-        uint2* src_rec = rec_a;
-        uint2* dst_rec = rec_b;
+        uint2* src_rec = W.rec_a;
+        uint2* dst_rec = W.rec_b;
         for (int pass = 0; pass < 4; ++pass) {
-            sweep::onesweep_pass_kernel<uint2, DEPTH_IPT><<<(unsigned)L.tiles, sweep::PASS_THREADS, 0, s>>>(
-                src_rec, dst_rec, d_visible, n, 8 * pass, hist + pass * sweep::RADIX, lookback + (size_t)pass * L.tiles * sweep::RADIX, tickets + 1 + pass);
+            sweep::onesweep_pass_kernel<uint2, DEPTH_IPT><<<(unsigned)W.tiles, sweep::PASS_THREADS, 0, s>>>(
+                src_rec, dst_rec, d_visible, n, 8 * pass, W.hist + pass * sweep::RADIX, W.lookback + (size_t)pass * W.tiles * sweep::RADIX,
+                W.tickets + 1 + pass);
             B200GS_LAUNCH_CHECK();
             uint2* tmp = src_rec; src_rec = dst_rec; dst_rec = tmp;
         }
         // 4 passes: the sorted records are back in rec_a
     }
-    return copy_counts(d_counts, host_counts, sync_host, s);
+    return publish_counts(d_counts, host_counts, sync_host, s);
 }
 
 int bin_sort(int mode, int width, int height, int64_t n, int cull, int64_t max_coarse, int64_t max_pairs, int64_t* d_counts,
@@ -1032,75 +907,55 @@ int bin_sort(int mode, int width, int height, int64_t n, int cull, int64_t max_c
     }
     if (max_coarse == 0 || n == 0) {   // nothing on screen (or nothing can be stored): empty lists; counts[2] stays 0
         B200GS_CUDA(cudaMemsetAsync(tile_ranges, 0, sizeof(int32_t) * 2 * (size_t)n_tiles, s));
-        return copy_counts(d_counts, host_counts, sync_host, s);
+        return publish_counts(d_counts, host_counts, sync_host, s);
     }
-    const LayoutA LA = make_layout_a(n);
-    const LayoutB L = make_layout_b(n, max_coarse, width, height);
-    if (ws_bytes < L.total) {
-        set_error("bin_sort: workspace too small (%zu < %zu)", ws_bytes, L.total);
+    const WorkspaceA A = carve_a(const_cast<void*>(ws_a), n);
+    const WorkspaceB W = carve_b(ws_b, n, max_coarse, width, height);
+    if (ws_bytes < W.bytes) {
+        set_error("bin_sort: workspace too small (%zu < %zu)", ws_bytes, W.bytes);
         return B200GS_ENOSPACE;
     }
-    const char* wa = (const char*)ws_a;
-    char* w = (char*)ws_b;
-    const uint2* order = (const uint2*)(wa + LA.rec_a);
-    const SplatRec* recs = (const SplatRec*)(wa + LA.recs);
-    CellEntry* entries_in = (CellEntry*)(w + L.entries_in);
-    CellEntry* entries = (CellEntry*)(w + L.entries);
-    uint32_t* offsets = (uint32_t*)(w + L.offsets);
-    uint32_t* cell_hist = (uint32_t*)(w + L.cell_hist);
-    uint32_t* tickets = (uint32_t*)(w + L.tickets);
-    uint32_t* scan_state = (uint32_t*)(w + L.scan_state);
-    uint32_t* lookback = (uint32_t*)(w + L.lookback);
-    uint32_t* digit_hist = (uint32_t*)(w + L.digit_hist);
-    int2* cell_ranges = (int2*)(w + L.cell_ranges);
-    int32_t* chunk_base = (int32_t*)(w + L.chunk_base);
-    int32_t* chunk_cell = (int32_t*)(w + L.chunk_cell);
-    uint16_t* chunk_cnt = (uint16_t*)(w + L.chunk_cnt);
-    uint32_t* chunk_pre = (uint32_t*)(w + L.chunk_pre);
-    int64_t* tile_start = (int64_t*)(w + L.tile_start);
+    const uint2* order = A.rec_a;
+    const SplatRec* recs = A.recs;
     const int64_t* d_visible = d_counts + 3;
     const int64_t* d_coarse = d_counts + 1;
 
     // B: coarse entries with their tile masks in depth order; per-cell counts
-    B200GS_CUDA(cudaMemsetAsync(w + L.zero, 0, L.zero_bytes, s));
-    const bool two_pass = n_cells > sweep::RADIX;
-    CellEntry* emit_dst = two_pass ? entries : entries_in;   // one pass: in -> entries; two passes: entries -> in -> entries
+    B200GS_CUDA(cudaMemsetAsync(W.cell_hist, 0, W.zero_bytes, s));
+    const int passes = n_cells > sweep::RADIX ? 2 : 1;     // partition passes: one per byte of the cell id
+    CellEntry* emit_dst = passes == 2 ? W.entries : W.entries_in;   // the partitioned entries end in W.entries
     const int pack = pack_ncells(n, width, height) ? 1 : 0;
-    rank_offsets_kernel<<<(unsigned)L.scan_blocks, 256, 0, s>>>(d_visible, pack, order, recs, offsets, tickets, scan_state);
+    rank_offsets_kernel<<<(unsigned)W.scan_blocks, 256, 0, s>>>(d_visible, pack, order, recs, W.offsets, W.tickets, W.scan_state);
     B200GS_LAUNCH_CHECK();
-    if (mode == B200GS_MODE_GSPLAT)
-        emit_cells_kernel<true><<<(unsigned)L.blocks, 256, 0, s>>>(d_visible, pack, grid_x, grid_y, cgrid_x, cull, max_coarse, order, recs, offsets, emit_dst,
-                                                                    n_cells, cell_hist);
-    else
-        emit_cells_kernel<false><<<(unsigned)L.blocks, 256, 0, s>>>(d_visible, pack, grid_x, grid_y, cgrid_x, cull, max_coarse, order, recs, offsets, emit_dst,
-                                                                     n_cells, cell_hist);
+    static constexpr decltype(&emit_cells_kernel<false>) emit[2] = {emit_cells_kernel<false>, emit_cells_kernel<true>};
+    emit[mode == B200GS_MODE_GSPLAT]<<<(unsigned)W.blocks, 256, 0, s>>>(d_visible, pack, grid_x, grid_y, cgrid_x, cull, max_coarse, order, recs,
+                                                                         W.offsets, emit_dst, n_cells, W.cell_hist);
     B200GS_LAUNCH_CHECK();
-    cell_table_kernel<<<1, 1024, 0, s>>>(n_cells, cell_hist, cell_ranges, chunk_base, chunk_cell, digit_hist, n_tiles, tile_start);
+    cell_table_kernel<<<1, 1024, 0, s>>>(n_cells, W.cell_hist, W.cell_ranges, W.chunk_base, W.chunk_cell, W.digit_hist, n_tiles, W.tile_start);
     B200GS_LAUNCH_CHECK();
-    // stable partition by cell: one onesweep pass per byte of the cell id (the entry carries its cell in .w)
-    if (two_pass) {
-        sweep::onesweep_pass_kernel<CellEntry, CELL_IPT><<<(unsigned)L.tiles, sweep::PASS_THREADS, 0, s>>>(entries, entries_in, d_coarse, max_coarse, 0, digit_hist,
-                                                                                                      lookback, tickets + 1);
+    // stable partition by cell (the entry carries its cell in .w)
+    CellEntry* src_ent = emit_dst;
+    CellEntry* dst_ent = passes == 2 ? W.entries_in : W.entries;
+    for (int pass = 0; pass < passes; ++pass) {
+        sweep::onesweep_pass_kernel<CellEntry, CELL_IPT><<<(unsigned)W.tiles, sweep::PASS_THREADS, 0, s>>>(
+            src_ent, dst_ent, d_coarse, max_coarse, 8 * pass, W.digit_hist + pass * sweep::RADIX, W.lookback + (size_t)pass * W.tiles * sweep::RADIX,
+            W.tickets + 1 + pass);
         B200GS_LAUNCH_CHECK();
-        sweep::onesweep_pass_kernel<CellEntry, CELL_IPT><<<(unsigned)L.tiles, sweep::PASS_THREADS, 0, s>>>(
-            entries_in, entries, d_coarse, max_coarse, 8, digit_hist + sweep::RADIX, lookback + (size_t)L.tiles * sweep::RADIX, tickets + 2);
-    } else {
-        sweep::onesweep_pass_kernel<CellEntry, CELL_IPT><<<(unsigned)L.tiles, sweep::PASS_THREADS, 0, s>>>(entries_in, entries, d_coarse, max_coarse, 0, digit_hist,
-                                                                                                      lookback, tickets + 1);
+        CellEntry* tmp = src_ent; src_ent = dst_ent; dst_ent = tmp;
     }
-    B200GS_LAUNCH_CHECK();
 
     // C: per-chunk tile counts;  D: chunk prefixes, tile starts / ranges / total;  E: ids in place
-    const unsigned chunks = (unsigned)L.max_chunks;
-    chunk_counts_kernel<<<chunks, CHUNK, 0, s>>>(n_cells, cgrid_x, grid_x, grid_y, cell_ranges, chunk_base, chunk_cell, entries, chunk_cnt, tile_start);
+    const unsigned chunks = (unsigned)W.max_chunks;
+    chunk_counts_kernel<<<chunks, CHUNK, 0, s>>>(n_cells, cgrid_x, grid_x, grid_y, W.cell_ranges, W.chunk_base, W.chunk_cell, W.entries, W.chunk_cnt,
+                                                 W.tile_start);
     B200GS_LAUNCH_CHECK();
-    chunk_prefix_kernel<<<(unsigned)n_cells + 1, 1024, 0, s>>>(n_cells, n_tiles, chunk_base, chunk_cnt, chunk_pre, tile_start, max_pairs,
+    chunk_prefix_kernel<<<(unsigned)n_cells + 1, 1024, 0, s>>>(n_cells, n_tiles, W.chunk_base, W.chunk_cnt, W.chunk_pre, W.tile_start, max_pairs,
                                                                (int2*)tile_ranges, d_counts);
     B200GS_LAUNCH_CHECK();
-    scatter_ids_kernel<<<chunks, CHUNK, 0, s>>>(n_cells, cgrid_x, grid_x, grid_y, max_pairs, cell_ranges, chunk_base, chunk_cell, entries, chunk_pre,
-                                                tile_start, sorted_ids);
+    scatter_ids_kernel<<<chunks, CHUNK, 0, s>>>(n_cells, cgrid_x, grid_x, grid_y, max_pairs, W.cell_ranges, W.chunk_base, W.chunk_cell, W.entries,
+                                                W.chunk_pre, W.tile_start, sorted_ids);
     B200GS_LAUNCH_CHECK();
-    return copy_counts(d_counts, host_counts, sync_host, s);
+    return publish_counts(d_counts, host_counts, sync_host, s);
 }
 
 // ---- row packing for the Gaussian-sharded exchange -------------------------------------------------------------------
@@ -1113,12 +968,7 @@ constexpr int VS_ITEMS = 8;
 
 __global__ void __launch_bounds__(256) visible_scan_kernel(int64_t n, const int32_t* __restrict__ radii, int32_t* __restrict__ scan,
                                                            uint32_t* __restrict__ ticket, uint32_t* __restrict__ state) {
-    __shared__ int s_scan[sweep::WARPS + 1];
-    __shared__ int s_tile;
-    __shared__ uint32_t s_excl;
-    if (threadIdx.x == 0) s_tile = (int)atomicAdd(ticket, 1u);
-    __syncthreads();
-    const int t = s_tile;
+    const int t = sweep::block_ticket(ticket);
     const int64_t i0 = (int64_t(t) * blockDim.x + threadIdx.x) * VS_ITEMS;
     int vis[VS_ITEMS];
     int mine = 0;
@@ -1133,14 +983,7 @@ __global__ void __launch_bounds__(256) visible_scan_kernel(int64_t n, const int3
     }
 #pragma unroll
     for (int k = 0; k < VS_ITEMS; ++k) mine += vis[k];
-    int block_total;
-    const int local = sweep::block_exclusive(mine, s_scan, &block_total);
-    if (threadIdx.x < 32) {
-        const uint32_t excl = sweep::chained_exclusive(state, t, (uint32_t)block_total);
-        if (threadIdx.x == 0) s_excl = excl;
-    }
-    __syncthreads();
-    int run = (int)(s_excl + (uint32_t)local);
+    int run = (int)sweep::chained_block_exclusive<8>(mine, state, t);
     int out[VS_ITEMS];
 #pragma unroll
     for (int k = 0; k < VS_ITEMS; ++k) { out[k] = run; run += vis[k]; }

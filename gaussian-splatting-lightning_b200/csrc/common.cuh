@@ -105,7 +105,10 @@ int launch_sh_bwd(int degree, int stride, int64_t n, const float* dirs, const fl
 
 size_t bin_count_workspace_bytes(int64_t n);
 size_t bin_sort_workspace_bytes(int64_t n, int64_t max_coarse, int width, int height);
-int bin_count(int mode, int width, int height, int64_t n, int row_stride, const float* xy, const float* depth, const int32_t* radii,
+// rows: xy, depth, radii, conic and opacity are columns of one 16-byte aligned [n,12] row buffer (b200gs.h), optionally in
+// blocks of block_rows rows of which the first block_counts[b] are valid; otherwise separate arrays, conic and opacity NULL
+// without culling
+int bin_count(int mode, int width, int height, int64_t n, bool rows, const float* xy, const float* depth, const int32_t* radii,
               const float* conic, const float* opacity, void* ws, size_t ws_bytes, int64_t* d_counts, int64_t* host_counts,
               int sync_host, cudaStream_t s, const int64_t* block_counts = nullptr, int64_t block_rows = 0);
 int publish_i64(const int64_t* d_values, int64_t* host_values, int n, cudaStream_t s);

@@ -117,6 +117,30 @@ __global__ void __launch_bounds__(128) knn_search_kernel(int64_t n, const float4
     out[__float_as_int(p.w)] = cnt ? sum / 3.0f : 0.f;
 }
 
+// histograms of the four key bytes of the uint2 records: the digit counts of all the radix passes at once
+constexpr int HIST_THREADS = 256;
+
+__global__ void __launch_bounds__(HIST_THREADS) hist4_kernel(const uint2* __restrict__ recs, const int64_t* __restrict__ d_n, int64_t cap,
+                                                             uint32_t* __restrict__ hist /*[4][RADIX]*/) {
+    using sweep::RADIX;
+    __shared__ uint32_t s_h[4][RADIX];
+    const int64_t n = d_n ? min(cap, *d_n) : cap;
+    for (int i = threadIdx.x; i < 4 * RADIX; i += HIST_THREADS) (&s_h[0][0])[i] = 0;
+    __syncthreads();
+    for (int64_t i = int64_t(blockIdx.x) * HIST_THREADS + threadIdx.x; i < n; i += int64_t(gridDim.x) * HIST_THREADS) {
+        const uint32_t k = recs[i].x;
+        atomicAdd(&s_h[0][k & 255u], 1u);
+        atomicAdd(&s_h[1][(k >> 8) & 255u], 1u);
+        atomicAdd(&s_h[2][(k >> 16) & 255u], 1u);
+        atomicAdd(&s_h[3][k >> 24], 1u);
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < 4 * RADIX; i += HIST_THREADS) {
+        const uint32_t c = (&s_h[0][0])[i];
+        if (c) atomicAdd(hist + i, c);
+    }
+}
+
 struct KnnLayout {
     size_t bounds, rec_a, rec_b, sorted, zero, zero_bytes, hist, tickets, lookback, cell_lo, cell_hi, total;
     int64_t tiles, max_cells;
@@ -208,7 +232,7 @@ int launch_knn_mean_dist2(int64_t n, const float* points, float* out, void* ws, 
     const unsigned blocks = (unsigned)div_up64(n, 256);
     knn_keys_kernel<<<blocks, 256, 0, s>>>(n, points, g, rec_a);
     B200GS_LAUNCH_CHECK();
-    sweep::hist4_kernel<<<(unsigned)min((int64_t)592, (int64_t)blocks), sweep::THREADS, 0, s>>>(rec_a, nullptr, n, hist);
+    hist4_kernel<<<(unsigned)min((int64_t)592, (int64_t)blocks), HIST_THREADS, 0, s>>>(rec_a, nullptr, n, hist);
     B200GS_LAUNCH_CHECK();
     int bits = 1;
     while ((int64_t(1) << bits) < n_cells) ++bits;

@@ -1,8 +1,8 @@
-// Hand-written device-wide primitives of the tile binning (no cub): a single-pass chained scan (decoupled look-back on
-// one value per block) and a stable LSD radix sort in the onesweep style — one histogram kernel for all digits, then one
-// kernel per 8-bit digit in which every tile ranks its records with warp match/ballot, publishes its digit counts,
-// obtains its global offsets by looking back over the preceding tiles' counts, and scatters through a shared-memory
-// staging area so that the global writes are runs of consecutive addresses.
+// Hand-written device-wide primitives of the tile binning (no cub): warp and block scans, a single-pass chained scan
+// (decoupled look-back on one value per block) and a stable LSD radix sort in the onesweep style — the caller builds the
+// histograms of all digits in one go, then one kernel per 8-bit digit in which every tile ranks its records with warp
+// ballots, publishes its digit counts, obtains its global offsets by looking back over the preceding tiles' counts, and
+// scatters through a shared-memory staging area so that the global writes are runs of consecutive addresses.
 //
 // Records carry their key inside (a uint2 {depth key, Gaussian id} for the depth sort, a uint4 {tile mask lo, hi, id,
 // coarse cell} for the partition by cell), so keys and payload move as one 8- or 16-byte vector.
@@ -14,8 +14,6 @@ namespace b200gs {
 namespace sweep {
 
 constexpr int RADIX = 256;
-constexpr int THREADS = 256;
-constexpr int WARPS = THREADS / 32;
 constexpr uint32_t FLAG_AGG = 1u << 30, FLAG_PREFIX = 2u << 30, VALUE_MASK = (1u << 30) - 1u;
 
 __device__ __forceinline__ uint32_t ld_volatile(const uint32_t* p) {
@@ -29,11 +27,6 @@ __device__ __forceinline__ uint32_t ld_relaxed_if(const uint32_t* p, bool pred, 
     asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\tmov.u32 %0, %3;\n\t@q ld.relaxed.gpu.global.u32 %0, [%1];\n\t}"
                  : "=r"(v) : "l"(p), "r"((uint32_t)pred), "r"(dflt) : "memory");
     return v;
-}
-__device__ __forceinline__ unsigned long long global_ns() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
 }
 __device__ __forceinline__ void st_volatile(uint32_t* p, uint32_t v) { asm volatile("st.volatile.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
 
@@ -51,24 +44,69 @@ __device__ __forceinline__ uint32_t wait_published(const uint32_t* p) {
 __device__ __forceinline__ uint32_t key_of(const uint2& r) { return r.x; }
 __device__ __forceinline__ uint32_t key_of(const uint4& r) { return r.w; }
 
-// ---- chained scan --------------------------------------------------------------------------------------------------
+// ---- scans -----------------------------------------------------------------------------------------------------------
+// inclusive scan over the 32 lanes of a warp (all lanes call it)
+template <typename T>
+__device__ __forceinline__ T warp_inclusive(T v) {
+    const unsigned lane = threadIdx.x & 31u;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const T t = __shfl_up_sync(0xffffffffu, v, o);
+        if ((int)lane >= o) v += t;
+    }
+    return v;
+}
+
+// Block-wide exclusive scan of one value per thread over NW warps: returns the thread's exclusive prefix, *total = block sum
+// (total may be NULL).  s_warp[NW + 1] (NW without total) is free again when it returns.  Up to 16 warps every thread sums the warp totals it needs; 32 warps scan them
+// in warp 0 instead of every thread reading all 32.
+template <typename T, int NW>
+__device__ __forceinline__ T block_exclusive(T v, T* s_warp, T* total) {
+    const unsigned lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+    const T inc = warp_inclusive(v);
+    if (lane == 31) s_warp[w] = inc;
+    __syncthreads();
+    T base = 0, tot = 0;
+    if (NW <= 16) {
+#pragma unroll
+        for (int k = 0; k < NW; ++k) {
+            const T c = s_warp[k];
+            base += (k < (int)w) ? c : T(0);
+            tot += c;
+        }
+    } else {
+        static_assert(NW <= 32, "one warp scans the warp totals");
+        if (w == 0) {
+            const T c = (int)lane < NW ? s_warp[lane] : T(0);
+            const T winc = warp_inclusive(c);
+            s_warp[lane] = winc - c;
+            if (total != nullptr && lane == 31) s_warp[NW] = winc;     // the slot costs chunk_prefix_kernel 2 registers
+        }
+        __syncthreads();
+        base = s_warp[w];
+        if (total != nullptr) tot = s_warp[NW];
+    }
+    const T excl = base + inc - v;
+    __syncthreads();
+    if (total != nullptr) *total = tot;
+    return excl;
+}
+
 // Exclusive prefix of one 30-bit value per tile over the tiles in ticket order.  `state[t]` must be zero before the launch.
 // Called by ALL 32 lanes of ONE warp (same arguments); returns (to every lane) the sum of the values of tiles 0..t-1.
-// The look-back is warp-wide and four words deep: 128 predecessors per step (lane l loads tiles p - l - 32 j, j = 0..3, all four
-// loads in flight together); the walk stops at the nearest tile that has already published its inclusive prefix and resumes at
-// the first word that is not published yet.  When a whole wave of tiles starts at once none has a prefix yet, and tile t needs
-// t / 128 round trips to L2 (with one predecessor per step: t).
-// DEPTH0 / DEPTH: words per lane in the first step / at most.  The default ramps 32 -> 64 -> 128 predecessors per step (long grids: in the
-// steady state the nearest predecessor's prefix is out already and wide steps only waste L2 requests); grids of a few hundred blocks
-// that all start together (depth_keys, rank_offsets: one wave) use <8, 8>: 256 predecessors in the first round trip.
-template <int DEPTH0 = 1, int DEPTH = 4>
+// The look-back is warp-wide: lane l loads tiles p - l - 32 j, j < depth, all loads in flight together; the walk stops at the
+// nearest tile that has already published its inclusive prefix and resumes at the first word that is not published yet.
+// depth ramps 1 -> 2 -> 4 words per lane (32 -> 64 -> 128 predecessors per step) while every word read is published: in the
+// steady state of a long grid the nearest predecessor's prefix is out already and wide steps only waste L2 requests, while a
+// whole wave of tiles that starts at once has no prefix yet and tile t needs about t / 128 round trips to L2.
 __device__ __forceinline__ uint32_t chained_exclusive(uint32_t* state, int t, uint32_t value) {
+    constexpr int DEPTH = 4;
     const unsigned lane = threadIdx.x & 31u;
     if (lane == 0) st_volatile(state + t, (value & VALUE_MASK) | (t == 0 ? FLAG_PREFIX : FLAG_AGG));
     uint32_t acc = 0;                 // per-lane partial sum, reduced once at the end
     bool done = (t == 0);
     unsigned spins = 0;
-    int depth = DEPTH0;               // default: 32 words in the first step, then 64, 128, 128, ..
+    int depth = 1;
     for (int p = t - 1; !done;) {
         uint32_t v[DEPTH];
 #pragma unroll
@@ -102,49 +140,28 @@ __device__ __forceinline__ uint32_t chained_exclusive(uint32_t* state, int t, ui
     return acc;
 }
 
-// block-wide exclusive scan of one int per thread (NW warps); returns the exclusive prefix, *total = block sum
-template <int NW = WARPS>
-__device__ __forceinline__ int block_exclusive(int v, int* s_warp /*[NW + 1]*/, int* total) {
-    const unsigned lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
-    int inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int t = __shfl_up_sync(0xffffffffu, inc, o);
-        if ((int)lane >= o) inc += t;
-    }
-    if (lane == 31) s_warp[w] = inc;
+// The block's ticket: blocks are numbered in the order they start, so every block a chained scan waits for is already running.
+__device__ __forceinline__ int block_ticket(uint32_t* ticket) {
+    __shared__ int s_tile;
+    if (threadIdx.x == 0) s_tile = (int)atomicAdd(ticket, 1u);
     __syncthreads();
-    int base = 0, tot = 0;
-#pragma unroll
-    for (int k = 0; k < NW; ++k) {
-        const int c = s_warp[k];
-        base += (k < (int)w) ? c : 0;
-        tot += c;
-    }
-    __syncthreads();
-    *total = tot;
-    return base + inc - v;
+    return s_tile;
 }
 
-// ---- histogram of the four digits of uint2 records ------------------------------------------------------------------
-static __global__ void __launch_bounds__(THREADS) hist4_kernel(const uint2* __restrict__ recs, const int64_t* __restrict__ d_n, int64_t cap,
-                                                       uint32_t* __restrict__ hist /*[4][RADIX]*/) {
-    __shared__ uint32_t s_h[4][RADIX];
-    const int64_t n = d_n ? min(cap, *d_n) : cap;
-    for (int i = threadIdx.x; i < 4 * RADIX; i += THREADS) (&s_h[0][0])[i] = 0;
-    __syncthreads();
-    for (int64_t i = int64_t(blockIdx.x) * THREADS + threadIdx.x; i < n; i += int64_t(gridDim.x) * THREADS) {
-        const uint32_t k = recs[i].x;
-        atomicAdd(&s_h[0][k & 255u], 1u);
-        atomicAdd(&s_h[1][(k >> 8) & 255u], 1u);
-        atomicAdd(&s_h[2][(k >> 16) & 255u], 1u);
-        atomicAdd(&s_h[3][k >> 24], 1u);
+// Device-wide exclusive scan of one int per thread over the blocks in ticket order t (NW warps per block): block scan, chained
+// scan of the block totals, returns the thread's global exclusive prefix.
+template <int NW>
+__device__ __forceinline__ uint32_t chained_block_exclusive(int v, uint32_t* state, int t) {
+    __shared__ int s_warp[NW + 1];
+    __shared__ uint32_t s_excl;
+    int block_total;
+    const int local = block_exclusive<int, NW>(v, s_warp, &block_total);
+    if (threadIdx.x < 32) {
+        const uint32_t excl = chained_exclusive(state, t, (uint32_t)block_total);
+        if (threadIdx.x == 0) s_excl = excl;
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < 4 * RADIX; i += THREADS) {
-        const uint32_t c = (&s_h[0][0])[i];
-        if (c) atomicAdd(hist + i, c);
-    }
+    return s_excl + (uint32_t)local;
 }
 
 // ---- one digit pass ----------------------------------------------------------------------------------------------------
@@ -156,17 +173,10 @@ static __global__ void __launch_bounds__(THREADS) hist4_kernel(const uint2* __re
 constexpr int PASS_THREADS = 512;
 constexpr int PASS_WARPS = PASS_THREADS / 32;
 
-// LB0 / LBMAX: first and largest look-back batch; LDMODE 0: volatile loads (branch per load), 1: predicated relaxed.gpu loads;
-// TRACE: thread 0 of every tile records %globaltimer at the phase boundaries into trace[tile][8].
-// On a pass over 0.65 M / 2.3 M 8-byte records a fixed batch of 8 with predicated relaxed loads beat both the doubling 4..32 batches
-// and a fixed 32 — the wide batches cost more in L2 requests than they save in round trips.  Default: fixed 8, relaxed.
-template <typename Rec, int IPT, int LB0 = 8, int LBMAX = 8, int LDMODE = 1, bool TRACE = false>
+template <typename Rec, int IPT>
 __global__ void __launch_bounds__(PASS_THREADS, 2) onesweep_pass_kernel(const Rec* __restrict__ in, Rec* __restrict__ out, const int64_t* __restrict__ d_n,
                                                                         int64_t cap, int shift, const uint32_t* __restrict__ hist,
-                                                                        uint32_t* __restrict__ lookback, uint32_t* __restrict__ ticket,
-                                                                        unsigned long long* __restrict__ trace = nullptr) {
-    unsigned long long tr[8];
-    if (TRACE) tr[0] = global_ns();
+                                                                        uint32_t* __restrict__ lookback, uint32_t* __restrict__ ticket) {
     constexpr int TILE_ITEMS = PASS_THREADS * IPT;
     static_assert(TILE_ITEMS < 65536, "per-warp digit counts are 16-bit");
     __shared__ unsigned short s_cnt[PASS_WARPS][RADIX];   // per-warp digit counts -> offsets of the warp inside the tile's digit run
@@ -184,7 +194,6 @@ __global__ void __launch_bounds__(PASS_THREADS, 2) onesweep_pass_kernel(const Re
     const int64_t tile_lo = int64_t(t) * TILE_ITEMS;
     if (tile_lo >= n) return;
     const int tile_n = (int)min((int64_t)TILE_ITEMS, n - tile_lo);
-    if (TRACE) tr[1] = global_ns();
 
     Rec rec[IPT];
     int dig[IPT];      // 0..255, or 256 for the slots past the end
@@ -226,7 +235,6 @@ __global__ void __launch_bounds__(PASS_THREADS, 2) onesweep_pass_kernel(const Re
         rank[i] = before + lt;
     }
     __syncthreads();
-    if (TRACE) tr[2] = global_ns();
     // thread d (< RADIX) owns digit d: offsets of the warps inside the digit's run, the tile's count
     uint32_t run = 0;
     uint32_t* col = lookback + (tid & (RADIX - 1));                        // lookback[p * RADIX + d]
@@ -240,7 +248,7 @@ __global__ void __launch_bounds__(PASS_THREADS, 2) onesweep_pass_kernel(const Re
         st_volatile(col + int64_t(t) * RADIX, (run & VALUE_MASK) | (t == 0 ? FLAG_PREFIX : FLAG_AGG));
     }
     int tot;
-    const int tile_start = block_exclusive<PASS_WARPS>((int)run, s_scan, &tot);                              // first slot of digit d in the staged tile
+    const int tile_start = block_exclusive<int, PASS_WARPS>((int)run, s_scan, &tot);                              // first slot of digit d in the staged tile
     if (tid < RADIX) {
         // slot of a record = tile_start[d] + warp offset + rank; fold tile_start into the warp offsets
 #pragma unroll
@@ -252,30 +260,22 @@ __global__ void __launch_bounds__(PASS_THREADS, 2) onesweep_pass_kernel(const Re
 #pragma unroll
     for (int i = 0; i < IPT; ++i)
         if (dig[i] < 256) s_stage[my_cnt[dig[i]] + rank[i]] = rec[i];
-    // look-back over the preceding tiles' words of digit d, `width` independent loads in flight per step, width = 4, 8, 16, 32, 32, ..
-    // When a whole wave of tiles starts at once no tile has a prefix yet and tile t has to sum the counts of all its predecessors:
-    // with a fixed 8 per step that was 20 dependent round trips to L2, most of a pass over 0.65 M records.  In the steady state of
-    // a long pass the nearest predecessor's prefix is usually out already, and a fixed 32 per step wasted 4x the L2 requests — hence the
-    // doubling.  A word that is not published yet ends the batch; the walk resumes there.
-    constexpr int LB = LBMAX;
+    // look-back over the preceding tiles' words of digit d: LB predicated relaxed loads in flight per step (before tile 0 a word
+    // reads as an empty prefix).  The run of published words up to the nearest prefix is summed; a word that is not published yet
+    // ends the step and the walk resumes there.  On a pass over 0.65 M / 2.3 M 8-byte records a fixed 8 per step beat both batches
+    // doubling from 4 to 32 and a fixed 32: the wide batches cost more in L2 requests than they save in round trips.
+    constexpr int LB = 8;
     uint32_t before_tiles = 0;
-    if (TRACE) tr[3] = global_ns();
     if (tid < RADIX) {
-        int width = LB0;
         for (int p = t - 1; p >= 0;) {
             uint32_t v[LB];
 #pragma unroll
-            for (int k = 0; k < LB; ++k) {
-                if (LDMODE == 1)
-                    v[k] = ld_relaxed_if(col + int64_t(max(p - k, 0)) * RADIX, k < width && p - k >= 0, (k < width) ? FLAG_PREFIX : 0u);
-                else
-                    v[k] = (k >= width) ? 0u : ((p - k >= 0) ? ld_volatile(col + int64_t(p - k) * RADIX) : FLAG_PREFIX);
-            }
+            for (int k = 0; k < LB; ++k) v[k] = ld_relaxed_if(col + int64_t(max(p - k, 0)) * RADIX, p - k >= 0, FLAG_PREFIX);
             int used = 0;
             bool done = false, open = true;
 #pragma unroll
             for (int k = 0; k < LB; ++k) {
-                const bool pub = (v[k] >> 30) != 0u;                       // words past `width` read as unpublished
+                const bool pub = (v[k] >> 30) != 0u;
                 open = open && !done && pub;                               // still inside the run of published words, before any prefix
                 before_tiles += open ? (v[k] & VALUE_MASK) : 0u;
                 used += open ? 1 : 0;
@@ -283,7 +283,6 @@ __global__ void __launch_bounds__(PASS_THREADS, 2) onesweep_pass_kernel(const Re
             }
             if (done) break;
             p -= used;
-            if (used == width) width = min(2 * width, LB);
             if (used == 0 && p >= 0) {     // the nearest word is not out yet: wait for it, then go on from the next one
                 const uint32_t w0 = wait_published(col + int64_t(p) * RADIX);
                 before_tiles += w0 & VALUE_MASK;
@@ -293,19 +292,13 @@ __global__ void __launch_bounds__(PASS_THREADS, 2) onesweep_pass_kernel(const Re
         }
         if (t > 0) st_volatile(col + int64_t(t) * RADIX, ((before_tiles + run) & VALUE_MASK) | FLAG_PREFIX);
     }
-    if (TRACE) tr[4] = global_ns();
-    const int digit_start = block_exclusive<PASS_WARPS>(tid < RADIX ? (int)hist[tid] : 0, s_scan, &tot);   // first global index of digit d
+    const int digit_start = block_exclusive<int, PASS_WARPS>(tid < RADIX ? (int)hist[tid] : 0, s_scan, &tot);   // first global index of digit d
     if (tid < RADIX) s_base[tid] = digit_start + (int)before_tiles - tile_start;
     __syncthreads();
     for (int s = tid; s < tile_n; s += PASS_THREADS) {
         const Rec r = s_stage[s];
         const int d = (int)((key_of(r) >> shift) & 255u);
         out[s_base[d] + s] = r;
-    }
-    if (TRACE) {
-        tr[5] = global_ns();
-        if (tid == 0 && trace != nullptr)
-            for (int k = 0; k < 6; ++k) trace[size_t(t) * 8 + k] = tr[k];
     }
 }
 

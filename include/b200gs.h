@@ -296,7 +296,10 @@ B200GS_API size_t b200gs_pack_rows_workspace_bytes(int64_t n);
 B200GS_API int b200gs_pack_rows(int64_t n, const float* xy, const float* depth, const float* conic, const float* comp, const float* opacity,
                                 const float* rgb, const int32_t* radii, void* workspace, size_t workspace_bytes, int32_t* row_index,
                                 float* rows, int64_t* d_count, void* stream);
-/* block_counts / block_rows (optional; NULL / 0 = every row counts): the rows arrive in blocks of block_rows rows of which only the first
+/* b200gs_bin_count_rows reads every row with three 16-byte loads: rows must be 16-byte aligned (an allocation base is), or the call
+ *     fails with B200GS_EINVAL.  It always packs the conic and opacity columns for phase B, so its cull argument has no effect: the cull
+ *     argument of b200gs_bin_sort decides whether the tiles are culled.
+ * block_counts / block_rows (optional; NULL / 0 = every row counts): the rows arrive in blocks of block_rows rows of which only the first
  *     block_counts[b] are valid (the fixed-capacity exchange of the sharded renderer) — the rest reads as culled, so the receive buffer
  *     needs no padding pass. */
 B200GS_API int b200gs_bin_count_rows(int32_t mode, int32_t width, int32_t height, int64_t n, const float* rows, int32_t cull,

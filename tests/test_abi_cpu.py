@@ -71,6 +71,8 @@ def test_argument_validation_without_gpu(lib):
     for rows, v_rows in ((d8, d16), (d16, d8)):
         assert L.b200gs_blend_bwd_rows(0, 64, 64, d16, d16, rows, d16, d16, d16, d16, 3, 1, d16, 1.0, 1.0, v_rows, None) == -1
         assert b"aligned" in L.b200gs_last_error()
+    assert L.b200gs_bin_count_rows(0, 64, 64, 1, d8, 1, d16, 1 << 20, d16, None, 0, None, None, 0) == -1
+    assert b"aligned" in L.b200gs_last_error()
     # n = 0 is a valid no-op everywhere that takes a count
     v.sh_stride = 16
     assert L.b200gs_project_fwd(ctypes.byref(v), 0, *([None] * 13), None) == 0

@@ -144,8 +144,26 @@ def test_binning_exact(mode, n, W, H, seed, pose, ms):
 
 # Shapes that drive the hierarchical binning off its common path: huge splats (rects of many coarse cells -> long (rank,row)
 # item lists in the emit kernel; 256-entry chunks whose output exceeds the shared-memory staging buffer -> direct-write
-# path of the scatter kernel) and an image with more than 256 coarse cells (two radix passes over the cell keys).
-STRESS = [(1500, 512, 384, 7, 1, 1.0), (2500, 2304, 2304, 9, 4, 0.06)]
+# path of the scatter kernel), an image with more than 256 coarse cells (two radix passes over the cell keys), one with more
+# than 1024 (the emit kernel's cell histogram and the cell table's chunk search in global memory) and one cell with more than
+# 256 chunks of 256 entries (the chunk prefix kernel's loop past its register window).  Every tile after the first listed one
+# must have a pair: the library writes an empty tile's range as (0, 0), the oracle as (k, k) at its place in the list.
+STRESS = [(1500, 512, 384, 7, 1, 1.0), (2500, 2304, 2304, 9, 4, 0.06), (6000, 4200, 4200, 3, 5, 0.03), (200000, 128, 128, 2, 6, 0.004)]
+# (more coarse cells than, more coarse entries in one cell than) each shape must reach, checked on the oracle's tile rects so
+# that a change of sizes cannot quietly lose the branch
+STRESS_REACH = {STRESS[2]: (1024, 0), STRESS[3]: (0, 256 * 256)}
+
+
+def _coarse_cover(ref, W, H):
+    """(coarse cells of the image, most coarse entries of one cell) of the oracle's tile rects; a cell is 8x8 tiles."""
+    cgx, cgy = ((W + 15) // 16 + 7) // 8, ((H + 15) // 16 + 7) // 8
+    vis = ref["tiles"] > 0
+    c0 = ref["rect_min"][vis].long() // 8
+    c1 = (ref["rect_max"][vis].long() - 1) // 8 + 1
+    d = torch.zeros(cgy + 1, cgx + 1, dtype=torch.long)     # 2D difference array of the rects in cell units
+    for ys, xs, sign in ((c0[:, 1], c0[:, 0], 1), (c0[:, 1], c1[:, 0], -1), (c1[:, 1], c0[:, 0], -1), (c1[:, 1], c1[:, 0], 1)):
+        d.index_put_((ys, xs), torch.full_like(ys, sign), accumulate=True)
+    return cgx * cgy, int(d.cumsum(0).cumsum(1).max())
 
 
 @pytest.mark.parametrize("mode", [O.MODE_VANILLA, O.MODE_GSPLAT])
@@ -153,6 +171,10 @@ STRESS = [(1500, 512, 384, 7, 1, 1.0), (2500, 2304, 2304, 9, 4, 0.06)]
 def test_binning_exact_stress(mode, n, W, H, seed, pose, ms):
     from b200gs import ops
     ref, colors, op, sids, ranges = _projected_inputs(mode, n, W, H, seed, pose, ms)
+    if (n, W, H, seed, pose, ms) in STRESS_REACH:
+        min_cells, min_cell_entries = STRESS_REACH[(n, W, H, seed, pose, ms)]
+        cells, cell_entries = _coarse_cover(ref, W, H)
+        assert cells > min_cells and cell_entries > min_cell_entries, (cells, cell_entries)
     dxy, ddep, drad, dcon, dop = (t.detach().to(DEV).contiguous() for t in (ref["xy"], ref["depth"], ref["radii"], ref["conic"], op))
     full = ops.bin_gaussians(mode, W, H, dxy, ddep, drad)
     assert full.total == int(ref["tiles"].sum()) == full.rect_pairs
