@@ -5,7 +5,7 @@ through ``oracle/`` or a torch re-implementation.
 """
 import ctypes
 import os
-from ctypes import POINTER, c_char_p, c_float, c_int32, c_int64, c_size_t, c_void_p
+from ctypes import POINTER, c_char_p, c_float, c_int32, c_int64, c_size_t, c_uint64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200gs.so")
@@ -42,6 +42,8 @@ _SIGNATURES = {
     "b200gs_project_bwd": (c_int32, [POINTER(B200gsView), c_int64] + [_P] * 4 + [_P] * 2 + [_P] * 5 + [_P] * 4 + [_P]),
     "b200gs_selective_adam": (c_int32, [c_int64, c_int32, _P, _P, _P, _P, _P, c_float, c_float, c_float, c_float, _P]),
     "b200gs_densify_stats": (c_int32, [c_int64, _P, _P, _P, c_int32, c_float, c_float, _P, _P, _P, _P]),
+    "b200gs_mcmc_relocation": (c_int32, [c_int64, _P, _P, _P, _P, c_int32, _P, _P, _P]),
+    "b200gs_mcmc_position_noise": (c_int32, [c_int64, _P, _P, _P, _P, c_float, c_uint64, c_uint64, _P]),
     "b200gs_knn_workspace_bytes": (c_size_t, [c_int64]),
     "b200gs_knn_mean_dist2": (c_int32, [c_int64, _P, _P, _P, c_size_t, _P]),
     "b200gs_sh_fwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P]),

@@ -42,3 +42,8 @@ def install(force: bool = False):
         for nm in names:
             setattr(m, nm, getattr(gsplat_v0, nm))
         put(f"gsplat.{sub}", m)
+    # gsplat.relocation.compute_relocation (internal/density_controllers/mcmc_density_controller.py:13)
+    from .. import mcmc
+    reloc = types.ModuleType("gsplat.relocation")
+    reloc.compute_relocation = mcmc.compute_relocation
+    put("gsplat.relocation", reloc)

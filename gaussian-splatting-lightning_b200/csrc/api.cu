@@ -41,7 +41,7 @@ using namespace b200gs;
 extern "C" {
 
 const char* b200gs_last_error(void) { return g_error; }
-int b200gs_version(void) { return 223; }
+int b200gs_version(void) { return 224; }
 int64_t b200gs_launch_count(void) { return (int64_t)g_launches.load(std::memory_order_relaxed); }
 
 int b200gs_project_fwd(const B200gsView* view, int64_t n, const float* means, const float* scales, const float* quats,
@@ -234,6 +234,22 @@ int b200gs_densify_stats(int64_t n, const int32_t* radii, const uint8_t* visible
     B200GS_CHECK_ARG(n >= 0 && grad_stride >= 2, "bad sizes");
     B200GS_CHECK_ARG(n == 0 || (radii && grad && max_radii2d && grad_accum && denom), "NULL pointer");
     return launch_densify_stats(n, radii, visible, grad, grad_stride, scale_x, scale_y, max_radii2d, grad_accum, denom, (cudaStream_t)stream);
+}
+
+int b200gs_mcmc_relocation(int64_t n, const float* opacities, const float* scales, const int32_t* counts, const float* binoms, int32_t n_max,
+                           float* new_opacities, float* new_scales, void* stream) {
+    B200GS_CHECK_ARG(n >= 0, "n < 0");
+    B200GS_CHECK_ARG(n_max >= 1, "n_max < 1");
+    B200GS_CHECK_ARG(n == 0 || (opacities && scales && counts && binoms && new_opacities && new_scales), "NULL pointer");
+    return launch_mcmc_relocation(n, opacities, scales, counts, n_max, new_opacities, new_scales, (cudaStream_t)stream);
+}
+
+int b200gs_mcmc_position_noise(int64_t n, float* means, const float* log_scales, const float* raw_quats, const float* opacity_logits,
+                               float scale, uint64_t seed, uint64_t offset, void* stream) {
+    B200GS_CHECK_ARG(n >= 0, "n < 0");
+    B200GS_CHECK_ARG(n == 0 || (means && log_scales && raw_quats && opacity_logits), "NULL pointer");
+    B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(raw_quats) & 15u) == 0, "raw_quats must be 16-byte aligned");
+    return launch_mcmc_position_noise(n, means, log_scales, raw_quats, opacity_logits, scale, seed, offset, (cudaStream_t)stream);
 }
 
 size_t b200gs_knn_workspace_bytes(int64_t n) { return n < 0 ? 0 : knn_workspace_bytes(n); }

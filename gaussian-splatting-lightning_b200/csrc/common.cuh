@@ -124,6 +124,11 @@ int launch_selective_adam(int64_t rows, int width, float* param, const float* gr
 int launch_densify_stats(int64_t n, const int32_t* radii, const uint8_t* visible, const float* grad, int grad_stride, float sx, float sy,
                          float* max_radii2d, float* grad_accum, float* denom, cudaStream_t s);
 
+int launch_mcmc_relocation(int64_t n, const float* opacities, const float* scales, const int32_t* counts, int n_max, float* new_opacities,
+                           float* new_scales, cudaStream_t s);
+int launch_mcmc_position_noise(int64_t n, float* means, const float* log_scales, const float* raw_quats, const float* opacity_logits,
+                               float scale, uint64_t seed, uint64_t offset, cudaStream_t s);
+
 size_t knn_workspace_bytes(int64_t n);
 int launch_knn_mean_dist2(int64_t n, const float* points, float* out, void* ws, size_t ws_bytes, cudaStream_t s);
 

@@ -113,6 +113,25 @@ B200GS_API int b200gs_selective_adam(int64_t rows, int32_t width, float* param, 
 B200GS_API int b200gs_densify_stats(int64_t n, const int32_t* radii, const uint8_t* visible, const float* grad, int32_t grad_stride,
                                     float scale_x, float scale_y, float* max_radii2d, float* grad_accum, float* denom, void* stream);
 
+/* ---- 3DGS-MCMC (internal/density_controllers/mcmc_density_controller.py) -------------------------------------------------
+ * b200gs_mcmc_relocation: gsplat's compute_relocation (mcmc_density_controller.py:13,121-128), Eq. (9) of 3DGS-MCMC, one sampled
+ *     Gaussian per thread.  With N = clamp(counts[i], 1, n_max):
+ *         new_opacities[i] = o' = 1 - (1 - o)^(1/N)
+ *         new_scales[i]    = scales[i] * o / D,   D = sum_{j=1..N} (-1)^(j-1) C(N,j) o'^j / sqrt(j)
+ *     (the hockey-stick form of the paper's double sum), evaluated in fp64.  binoms is the controller's [n_max, n_max] table
+ *     (mcmc_density_controller.py:53-60): it bounds N, and no entry of it is read (fp32 rounds every C(n,k) > 2^24, which
+ *     moves D by up to 9e-5 relative), so unlike gsplat's kernel a count above n_max never reads outside it.
+ * b200gs_mcmc_position_noise: MCMCDensityControllerImpl._add_xyz_noise (mcmc_density_controller.py:93-120) in one in-place pass
+ *     over the raw parameters: means[i] += scale * w * Sigma z, Sigma = R(q) diag(s)^2 R(q)^T with s = exp(log_scales[i]) and
+ *     q = raw_quats[i] / max(|raw_quats[i]|, 1e-12) (K8's fp32 geometry), o = sigmoid(opacity_logits[i]),
+ *     w = 1 / (1 + exp(-100 ((1 - o) - 0.995))), and z three standard normals of Philox4x32-10 keyed by seed, subsequence
+ *     offset + i.  scale = noise_lr * xyz_lr.  raw_quats must be 16-byte aligned (read as float4).
+ * Algorithmic bytes: relocation 20 B in + 16 B out per sampled Gaussian; position noise 44 B in + 12 B out per Gaussian. */
+B200GS_API int b200gs_mcmc_relocation(int64_t n, const float* opacities, const float* scales, const int32_t* counts, const float* binoms,
+                                      int32_t n_max, float* new_opacities, float* new_scales, void* stream);
+B200GS_API int b200gs_mcmc_position_noise(int64_t n, float* means, const float* log_scales, const float* raw_quats,
+                                          const float* opacity_logits, float scale, uint64_t seed, uint64_t offset, void* stream);
+
 /* b200gs_knn_mean_dist2: simple_knn's distCUDA2 (vanilla_gaussian.py:122-125, the scale initialiser): mean_dist2[i] = mean of the squared
  *     distances from points[i] (float[n,3]) to its 3 nearest neighbours (exact).  Synchronises the stream once (the hash grid is sized
  *     on the host from the bounding box); init-time only. */
