@@ -108,7 +108,8 @@ __global__ void __launch_bounds__(128) knn_search_kernel(int64_t n, const float4
         const float reach = float(r) * g.cs;
         if (b2 <= reach * reach) break;
     }
-    // fewer than 3 other points in the whole set: average what exists (simple-knn leaves such inputs undefined)
+    // fewer than 3 other points in the whole set: the missing distances count as 0, i.e. the sum of those there are over 3, and 0
+    // for a single point (simple-knn leaves such inputs undefined)
     float sum = 0.f;
     int cnt = 0;
     if (b0 < FLT_MAX) { sum += b0; ++cnt; }
