@@ -60,6 +60,8 @@ _SIGNATURES = {
     "b200gs_blend_fwd_hits": (c_int32, [c_int32] * 4 + [_P] * 7 + [_P, c_int64, c_int64, _P, _P, _P, _P, _P]),
     "b200gs_blend_bwd": (c_int32, [c_int32] * 4 + [_P] * 7 + [_P, _P, _P, c_int64, c_int64, _P, c_float, c_float]
                          + [_P] * 5 + [_P]),
+    "b200gs_blend_feat_fwd": (c_int32, [c_int32] * 3 + [_P] * 7 + [_P] * 4 + [_P]),
+    "b200gs_blend_feat_bwd": (c_int32, [c_int32] * 3 + [_P] * 7 + [_P] * 4 + [_P] * 5 + [_P]),
     "b200gs_project_bwd_rows": (c_int32, [POINTER(B200gsView), c_int64] + [_P] * 6 + [c_int32] + [_P] * 4 + [c_int32] + [_P] * 6 + [_P, c_int32] + [_P]),
     "b200gs_project_fwd_raw_multi": (c_int32, [POINTER(B200gsView), c_int32, c_int64] + [_P] * 6 + [c_int32] + [_P] * 7 + [_P]),
     "b200gs_project_bwd_rows_multi": (c_int32, [POINTER(B200gsView), c_int32, c_int64] + [_P] * 6 + [c_int32] + [_P] * 3 + [POINTER(c_void_p)] + [_P] * 6 + [_P]),

@@ -346,6 +346,32 @@ int b200gs_blend_bwd(int32_t mode, int32_t width, int32_t height, int32_t channe
                             v_opacity, v_colors, v_xy_abs, (cudaStream_t)stream);
 }
 
+int b200gs_blend_feat_fwd(int32_t width, int32_t height, int32_t channels, const int32_t* tile_ranges, const int32_t* sorted_ids,
+                          const float* xy, const float* conic, const float* opacity, const float* features, const float* bg, float* image,
+                          float* final_T, int32_t* n_contrib, float* alpha, void* stream) {
+    B200GS_CHECK_ARG(width > 0 && height > 0, "bad size");
+    B200GS_CHECK_ARG(channels >= 1, "channels must be >= 1");
+    B200GS_CHECK_ARG(tile_ranges && sorted_ids && xy && conic && opacity && features, "NULL input pointer");
+    B200GS_CHECK_ARG(image && final_T && n_contrib, "NULL output pointer");
+    return launch_blend_feat_fwd(width, height, channels, tile_ranges, sorted_ids, xy, conic, opacity, features, bg, image, final_T, n_contrib,
+                                 alpha, (cudaStream_t)stream);
+}
+
+int b200gs_blend_feat_bwd(int32_t width, int32_t height, int32_t channels, const int32_t* tile_ranges, const int32_t* sorted_ids,
+                          const float* xy, const float* conic, const float* opacity, const float* features, const float* bg,
+                          const float* final_T, const int32_t* n_contrib, const float* v_image, const float* v_alpha, float* v_features,
+                          float* v_xy, float* v_conic, float* v_opacity, float* v_xy_abs, void* stream) {
+    B200GS_CHECK_ARG(width > 0 && height > 0, "bad size");
+    B200GS_CHECK_ARG(channels >= 1, "channels must be >= 1");
+    B200GS_CHECK_ARG(tile_ranges && sorted_ids && xy && conic && opacity && features, "NULL input pointer");
+    B200GS_CHECK_ARG(final_T && n_contrib && v_image && v_features, "NULL input/output pointer");
+    B200GS_CHECK_ARG((v_xy == nullptr) == (v_conic == nullptr) && (v_xy == nullptr) == (v_opacity == nullptr),
+                     "v_xy, v_conic and v_opacity are all given or all NULL");
+    B200GS_CHECK_ARG(v_xy_abs == nullptr || v_xy != nullptr, "v_xy_abs needs the geometry gradients");
+    return launch_blend_feat_bwd(width, height, channels, tile_ranges, sorted_ids, xy, conic, opacity, features, bg, final_T, n_contrib,
+                                 v_image, v_alpha, v_features, v_xy, v_conic, v_opacity, v_xy_abs, (cudaStream_t)stream);
+}
+
 int b200gs_publish_i64(const int64_t* d_values, int64_t* host_values, int32_t n, void* stream) {
     B200GS_CHECK_ARG(d_values && host_values && n > 0, "bad argument");
     return publish_i64(d_values, host_values, n, (cudaStream_t)stream);

@@ -703,6 +703,429 @@ int bwd_dispatch(bool rows, int width, int height, const int32_t* ranges, const 
     }
 }
 
+// ---- wide feature maps (gsplat mode): D channels in chunks of up to 32 ----------------------------------------------------
+// The feature renderers of the reference (contrastive / SegAnyGS / Feature3DGS) composite 32-channel features through gsplat's
+// rasterize_gaussians.  K6 / K7 at <= 4 channels would re-walk every tile list and recompute every alpha 8 times for 4 FMAs per
+// sample.  These kernels keep K6 / K7's tile, list and staging machinery (tile_pixel, block_mask, build_list, DUMMY padding) and
+// carry CH in {8, 16, 32} channels per launch; the launchers split D into chunks of 32, the tail chunk taking the smallest
+// instantiation that holds it (the channels past D are masked at load and store).
+//
+// Forward: the geometry record is staged as in K6; the batch's feature rows go to their own [257][CH] array (row DUMMY zero),
+// loaded by the whole CTA with coalesced reads.  Per sample the alpha / Tc / stop arithmetic is composite4's, then CH FMAs on
+// warp-uniform LDS.128 broadcasts of the feature row: each channel sees the same operations in the same order as in K6, so a
+// chunk's composite is bit-identical to the <= 4-channel groups of rasterize_binned.  The background term is one FMA here; K6
+// leaves C + T * bg to nvcc, which fuses it for some channels and rounds T * bg first for others, so with a background a
+// channel may differ from K6's by that one rounding.
+template <int CH>
+struct FeatFwdSmem {
+    float4 rec[REC_SLAB];
+    float feat[BLOCK_PIX + 1][CH];
+    int32_t gid[BLOCK_PIX];
+    unsigned short list[NWARP][BLOCK_PIX + 2 * LIST_PAD];
+    unsigned char mask[BLOCK_PIX];
+};
+
+// Features of the `cnt` staged splats, channels [c0, c0 + width) of [n, D] rows, into feat[0..cnt) (channels >= width zero).
+// Consecutive threads read consecutive channels of one row: a 32-channel row is one 128-byte read per warp.
+template <int CH>
+__device__ __forceinline__ void stage_features(float (*feat)[CH], const int32_t* gid, int cnt, const float* __restrict__ features, int D,
+                                               int c0, int width, int tid) {
+    for (int k = tid; k < cnt * CH; k += BLOCK_PIX) {
+        const int i = k / CH, c = k - i * CH;
+        feat[i][c] = (c < width) ? __ldg(features + int64_t(gid[i]) * D + c0 + c) : 0.f;
+    }
+}
+
+template <int CH>
+__global__ void __launch_bounds__(BLOCK_PIX, CH > 16 ? 2 : CH > 8 ? 3 : 4) blend_feat_fwd_kernel(int width, int height, int grid_x, const int2* __restrict__ ranges,
+                                                                               const int32_t* __restrict__ ids, const float* __restrict__ xy,
+                                                                               const float* __restrict__ conic, const float* __restrict__ opacity,
+                                                                               const float* __restrict__ features, int D, int c0, int cw,
+                                                                               const float* __restrict__ bg, float* __restrict__ image,
+                                                                               float* __restrict__ final_T, int32_t* __restrict__ n_contrib,
+                                                                               float* __restrict__ alpha_out) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    FeatFwdSmem<CH>& sm = *reinterpret_cast<FeatFwdSmem<CH>*>(smem_raw);
+    float4* s_rec = sm.rec;
+    const SplatStrides st{2, 3, 1, 0};
+
+    const int tid = threadIdx.x;
+    const int warp = tid >> 5;
+    const unsigned lane = tid & 31u;
+    int last = 0;
+    float C[CH];
+#pragma unroll
+    for (int c = 0; c < CH; ++c) C[c] = 0.f;
+    const TilePixel t = tile_pixel<true>(tid, grid_x, width, height);
+    if (tid < 3) s_rec[DUMMY * 3 + tid] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (tid < CH) sm.feat[DUMMY][tid] = 0.f;
+
+    const int2 range = ranges[t.tile];
+    int todo = range.y - range.x;
+    float T = 1.0f, Tc = t.inside ? 1.0f : 0.0f;     // Tc == 0: this pixel is finished (or outside the image)
+
+    for (int base = 0; todo > 0; base += BLOCK_PIX, todo -= BLOCK_PIX) {
+        if (__syncthreads_and(Tc == 0.0f)) break;
+        const int cnt = min(BLOCK_PIX, todo);
+        if (tid < cnt) {
+            const int g = __ldg(ids + range.x + base + tid);
+            float2 m;
+            float A, B, Cc, o, col[4] = {0.f, 0.f, 0.f, 0.f};
+            gather_splat<0>(g, st, xy, conic, opacity, nullptr, m, A, B, Cc, o, col);
+            stage_record<0, false>(s_rec, sm.mask, tid, m.x, m.y, A, B, Cc, o, col, g, t.ox, t.oy);
+            sm.gid[tid] = g;
+        }
+        __syncthreads();
+        stage_features<CH>(sm.feat, sm.gid, cnt, features, D, c0, cw, tid);
+        __syncthreads();
+        if (__all_sync(FULL, Tc == 0.0f)) continue;  // warp finished: only keeps the block barriers company
+        const unsigned short* my_list = sm.list[warp] + LIST_PAD;
+        const int nl = build_list(sm.mask, sm.list[warp], cnt, warp, lane);
+        for (int i0 = 0; i0 < nl; i0 += 4) {
+            if (__all_sync(FULL, Tc == 0.0f)) break;
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                const int j = my_list[i0 + u];                 // warp-uniform: the feature reads below are broadcasts
+                const float4 r0 = s_rec[j * 3 + 0];
+                const float4 r1 = s_rec[j * 3 + 1];
+                const float dx = r0.x - t.pxf, dy = r0.y - t.pyf;
+                const float p2 = fmaf(r1.x * dy, dy, fmaf(r0.w, dy, r0.z * dx) * dx);
+                float a = fminf(t.amax, r1.y * ex2_approx(p2));
+                a = (!(p2 > 0.0f) && !(a < ALPHA_MIN)) ? a : 0.f;
+                const float nT = fmaf(-a, Tc, Tc);
+                const bool stop = nT <= T_STOP;
+                const float w = stop ? 0.f : a * Tc;
+                const float4* f = reinterpret_cast<const float4*>(sm.feat[j]);
+#pragma unroll
+                for (int q = 0; q < CH / 4; ++q) {
+                    const float4 fq = f[q];
+                    C[4 * q + 0] = fmaf(fq.x, w, C[4 * q + 0]);
+                    C[4 * q + 1] = fmaf(fq.y, w, C[4 * q + 1]);
+                    C[4 * q + 2] = fmaf(fq.z, w, C[4 * q + 2]);
+                    C[4 * q + 3] = fmaf(fq.w, w, C[4 * q + 3]);
+                }
+                last = (w > 0.f) ? base + j + 1 : last;
+                T = stop ? T : nT;
+                Tc = stop ? 0.f : nT;
+            }
+        }
+    }
+    if (t.inside && final_T) {             // chunk 0 only
+        const int64_t pix = int64_t(t.py) * width + t.px;
+        final_T[pix] = T;
+        n_contrib[pix] = last;
+        if (alpha_out) alpha_out[pix] = 1.0f - T;
+    }
+    // The pixel's CH outputs go through the feature array (free now) so that the warp stores them coalesced: a pixel's channels
+    // are D floats apart from the next pixel's, and the 8 pixels of a block row are adjacent in the image.  Row p of the tile is
+    // rotated by p so that the 32 lanes of a warp write different banks.  The background term is one explicit FMA: its rounding
+    // does not depend on nvcc's contraction choices.
+    __syncthreads();                       // every warp has left the blend loop: the feature array may be overwritten
+    float* tile = &sm.feat[0][0];
+#pragma unroll
+    for (int c = 0; c < CH; ++c)
+        tile[tid * CH + ((c + tid) & (CH - 1))] = bg ? __fmaf_rn(T, __ldg(bg + c0 + (c < cw ? c : 0)), C[c]) : C[c];
+    __syncwarp();
+    const int tile_x = t.px - (t.px & (TILE - 1)), tile_y = t.py - (t.py & (TILE - 1));
+    for (int k = lane; k < 32 * cw; k += 32) {
+        const int p = k / cw, c = k - p * cw;
+        int lx, ly;
+        pixel_of_thread(warp * 32 + p, lx, ly);
+        const int px = tile_x + lx, py = tile_y + ly;
+        if (px < width && py < height)
+            image[(int64_t(py) * width + px) * D + c0 + c] = tile[(warp * 32 + p) * CH + ((c + p) & (CH - 1))];
+    }
+}
+
+// Backward: blend_bwd_tr_kernel's reverse walk (up to the warp's deepest contributor), per-warp value tile of GE entries and
+// reduce phase.  The warp's v_image tile [32 pixels][CH] sits in shared memory; the feature gradient is reduced lane = channel:
+// for each entry lane c sums fac[pixel] * v[pixel][c] over the warp's 32 pixels (fac broadcast, v rows conflict-free, no
+// shuffles) and issues one atomic, so a 32-channel entry leaves as one coalesced 128-byte reduction.  At CH < 32 the warp takes
+// 32 / CH entries at a time.
+// GEOM = false (the geometry needs no gradient): per sample only the transmittance walk and fac = alpha T; no <f, v> product, no
+// moments, no geometry atomics, no feature staging.  GEOM = true: S = <f_j, v_pix> over the chunk's CH channels (the pixel's v row
+// in registers, the feature row broadcast from shared memory), then K7's moment reduction and geometry atomics; ABS: absgrad.
+template <int CH, bool GEOM, bool ABS>
+struct FeatBwdSmem {
+    static constexpr int VAL_BYTES = GEOM ? (ABS ? 16 : 8) : 4;   // per (entry, pixel): {fac}, {go, fac} or {go, fac, |gx|, |gy|}
+    static constexpr int FAC_OFF = GEOM ? 4 : 0;
+    static constexpr int VAL_ROW = 32 * VAL_BYTES + 16;           // bytes per entry row of the value tile (+ pad)
+    float4 rec[REC_SLAB];
+    float feat[GEOM ? BLOCK_PIX + 1 : 1][CH];
+    float vimg[NWARP][32 * CH];                                   // v_image of the warp's pixels, pixel-major
+    unsigned char val[NWARP][GE * VAL_ROW];
+    unsigned short list[NWARP][BWD_LIST];
+    int32_t gid[GEOM ? BLOCK_PIX : 1];
+    unsigned char mask[BLOCK_PIX];
+    int wmax[NWARP];
+};
+
+template <int CH, bool GEOM, bool ABS>
+__global__ void __launch_bounds__(BLOCK_PIX, GEOM ? (CH > 16 ? 1 : 2) : 3) blend_feat_bwd_kernel(int width, int height, int grid_x, const int2* __restrict__ ranges,
+                                                                    const int32_t* __restrict__ ids, const float* __restrict__ xy,
+                                                                    const float* __restrict__ conic, const float* __restrict__ opacity,
+                                                                    const float* __restrict__ features, int D, int c0, int cw,
+                                                                    const float* __restrict__ bg, const float* __restrict__ final_T,
+                                                                    const int32_t* __restrict__ n_contrib, const float* __restrict__ v_image,
+                                                                    const float* __restrict__ v_alpha, float* __restrict__ v_features,
+                                                                    float* __restrict__ v_xy, float* __restrict__ v_conic,
+                                                                    float* __restrict__ v_opacity, float* __restrict__ v_xy_abs) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    typedef FeatBwdSmem<CH, GEOM, ABS> Smem;
+    constexpr int VAL_ROW = Smem::VAL_ROW, VAL_BYTES = Smem::VAL_BYTES;
+    constexpr int EPP = 32 / CH;                                  // entries per pass of the channel reduction
+    Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
+    float4* s_rec = sm.rec;
+    const SplatStrides st{2, 3, 1, 0};
+
+    const int tid = threadIdx.x;
+    const int warp = tid >> 5;
+    const unsigned lane = tid & 31u;
+    const TilePixel t = tile_pixel<true>(tid, grid_x, width, height);
+    const int64_t pix = int64_t(t.py) * width + t.px;
+    if (tid < 3) s_rec[DUMMY * 3 + tid] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (GEOM && tid < CH) sm.feat[GEOM ? DUMMY : 0][tid] = 0.f;
+
+    // the warp's 32 v_image rows, coalesced: consecutive lanes read consecutive channels of one pixel
+    float* my_vimg = sm.vimg[warp];
+    for (int k = lane; k < 32 * CH; k += 32) {
+        const int p = k / CH, c = k - p * CH;
+        int lx, ly;
+        pixel_of_thread(warp * 32 + p, lx, ly);
+        const int px = t.px - (t.px & (TILE - 1)) + lx, py = t.py - (t.py & (TILE - 1)) + ly;
+        my_vimg[k] = (c < cw && px < width && py < height) ? __ldg(v_image + (int64_t(py) * width + px) * D + c0 + c) : 0.f;
+    }
+    __syncwarp();
+
+    const int2 range = ranges[t.tile];
+    const float Tf = t.inside ? final_T[pix] : 0.f;
+    const int last = t.inside ? n_contrib[pix] : 0;
+    float vo[GEOM ? CH : 1];
+    float tail = 0.f;
+    if (GEOM) {
+        float bg_dot = 0.f;
+#pragma unroll
+        for (int c = 0; c < CH; ++c) {
+            vo[c] = my_vimg[lane * CH + c];
+            if (bg && c < cw) bg_dot += __ldg(bg + c0 + c) * vo[c];
+        }
+        const float va = (v_alpha && t.inside) ? __ldg(v_alpha + pix) : 0.f;
+        tail = Tf * (va - bg_dot);   // d(out)/d(alpha_i) through everything behind the last contributor
+    }
+
+    const int wmax = __reduce_max_sync(FULL, last);
+    if (lane == 0) sm.wmax[warp] = wmax;
+    __syncthreads();
+    int max_last = 0;
+#pragma unroll
+    for (int w = 0; w < NWARP; ++w) max_last = max(max_last, sm.wmax[w]);
+    if (max_last == 0) return;
+
+    float T = Tf;
+    float Dacc = 0.f;   // <feature accumulated behind the current splat, v_image> for this pixel (GEOM)
+    unsigned char* my_val = sm.val[warp] + lane * VAL_BYTES;      // eval phase: this pixel's value column
+    const int re = lane & (GE - 1), rh = lane >> 4;               // geometry reduce: entry and pixel half of this lane
+    const float4* my_row = reinterpret_cast<const float4*>(sm.val[warp] + re * VAL_ROW + rh * 16 * VAL_BYTES);
+    const int ce = lane / CH, cc = lane - ce * CH;                // channel reduce: entry of the pass and channel of this lane
+    const float bx0 = t.ox + float((warp & 1) << 3), by0 = t.oy + float((warp >> 1) << 2);
+    const float hh = float(2 * rh);
+
+    for (int hi = max_last; hi > 0; hi -= BLOCK_PIX) {
+        const int lo = max(0, hi - BLOCK_PIX);
+        const int cnt = hi - lo;
+        __syncthreads();
+        if (tid < cnt) {
+            const int g = __ldg(ids + range.x + lo + tid);
+            float2 m;
+            float A, B, Cc, o, col[4] = {0.f, 0.f, 0.f, 0.f};
+            gather_splat<0>(g, st, xy, conic, opacity, nullptr, m, A, B, Cc, o, col);
+            stage_record<0, true>(s_rec, sm.mask, tid, m.x, m.y, A, B, Cc, o, col, g, t.ox, t.oy);
+            if (GEOM) sm.gid[GEOM ? tid : 0] = g;
+        }
+        __syncthreads();
+        if (GEOM) {
+            stage_features<CH>(sm.feat, sm.gid, cnt, features, D, c0, cw, tid);
+            __syncthreads();
+        }
+        if (wmax <= lo) continue;  // this warp has no contributor in the batch
+        const unsigned short* my_list = sm.list[warp] + GE;   // my_list[-GE..-1] are DUMMY
+        const int nl = build_list<GE>(sm.mask, sm.list[warp], min(cnt, wmax - lo), warp, lane);
+        const int rel_last = last - lo;
+        for (int ii = nl - 1; ii >= 0; ii -= GE) {
+            unsigned vm = 0;   // bit u: this pixel has a valid sample of list entry ii-u
+#pragma unroll
+            for (int u = 0; u < GE; ++u) {
+                const int j = my_list[ii - u];
+                const float4 r0 = s_rec[j * 3 + 0];
+                const float4 r1 = s_rec[j * 3 + 1];
+                const float dx = r0.x - t.pxf, dy = r0.y - t.pyf;
+                const float p2 = fmaf(r1.x * dy, dy, fmaf(r0.w, dy, r0.z * dx) * dx);
+                const float G = ex2_approx(p2);
+                const float oG = r1.y * G;
+                const float a = fminf(t.amax, oG);
+                const bool valid = (j < rel_last) && !(p2 > 0.0f) && (a >= ALPHA_MIN);
+                float go = 0.f, fac = 0.f, gax = 0.f, gay = 0.f;
+                if (valid) {
+                    const float ra = 1.0f / (1.0f - a);
+                    T *= ra;
+                    fac = a * T;
+                    vm |= 1u << u;
+                    if (GEOM) {
+                        const float4* f = reinterpret_cast<const float4*>(sm.feat[GEOM ? j : 0]);
+                        float S = 0.f;
+#pragma unroll
+                        for (int q = 0; q < CH / 4; ++q) {
+                            const float4 fq = f[q];
+                            S = fmaf(fq.x, vo[4 * q + 0], S);
+                            S = fmaf(fq.y, vo[4 * q + 1], S);
+                            S = fmaf(fq.z, vo[4 * q + 2], S);
+                            S = fmaf(fq.w, vo[4 * q + 3], S);
+                        }
+                        const float v_al = fmaf(T, S, ra * (tail - Dacc));
+                        Dacc = fmaf(fac, S, Dacc);
+                        if (oG <= 0.999f) go = G * v_al;
+                        if (ABS) {
+                            const float vsg = r1.y * go * (2.0f / LOG2E);
+                            gax = fabsf(vsg * fmaf(r0.z, dx, 0.5f * r0.w * dy));
+                            gay = fabsf(vsg * fmaf(0.5f * r0.w, dx, r1.x * dy));
+                        }
+                    }
+                }
+                if (!GEOM) *reinterpret_cast<float*>(my_val + u * VAL_ROW) = fac;
+                else if (ABS) *reinterpret_cast<float4*>(my_val + u * VAL_ROW) = make_float4(go, fac, gax, gay);
+                else *reinterpret_cast<float2*>(my_val + u * VAL_ROW) = make_float2(go, fac);
+            }
+            const unsigned present = __reduce_or_sync(FULL, vm);
+            __syncwarp();   // the tile stores of all lanes are visible to the row loads below
+            if (present == 0u) {
+                __syncwarp();
+                continue;
+            }
+            // ---- feature gradient: lane (ce, cc) sums entry ii - (e0 + ce), channel cc, over the warp's 32 pixels
+#pragma unroll 1
+            for (int e0 = 0; e0 < GE; e0 += EPP) {
+                if (((present >> e0) & ((1u << EPP) - 1u)) == 0u) continue;
+                const int e = e0 + ce;
+                const unsigned char* frow = sm.val[warp] + e * VAL_ROW + Smem::FAC_OFF;
+                float s[4] = {0.f, 0.f, 0.f, 0.f};    // four partial sums: four independent FMA chains
+#pragma unroll
+                for (int p = 0; p < 32; ++p) s[p & 3] = fmaf(*reinterpret_cast<const float*>(frow + p * VAL_BYTES), my_vimg[p * CH + cc], s[p & 3]);
+                if (((present >> e) & 1u) && cc < cw) {
+                    const int g = __float_as_int(s_rec[my_list[ii - e] * 3 + 2].z);
+                    atomicAdd(v_features + int64_t(g) * D + c0 + cc, (s[0] + s[1]) + (s[2] + s[3]));
+                }
+            }
+            if (GEOM) {
+                // ---- geometry: blend_bwd_tr_kernel's moment reduction, lane (re, rh) over pixels 16 rh .. 16 rh + 15
+                float R0 = 0.f, R0x = 0.f, R0xx = 0.f, R1 = 0.f, R1x = 0.f, R1xx = 0.f;
+                float Ax = 0.f, Ay = 0.f;
+#pragma unroll
+                for (int k2 = 0; k2 < 8; ++k2) {
+                    float4 v;                             // {go, fac} of pixels 2 k2, 2 k2 + 1
+                    if (ABS) {
+                        const float4 va = my_row[2 * k2], vb = my_row[2 * k2 + 1];
+                        v = make_float4(va.x, va.y, vb.x, vb.y);
+                        Ax += va.z + vb.z;
+                        Ay += va.w + vb.w;
+                    } else {
+                        v = my_row[k2];
+                    }
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int k = 2 * k2 + e;
+                        const float gk = e ? v.z : v.x;
+                        const float x = float(k & 7);
+                        if (k < 8) { R0 += gk; if (k & 7) { R0x = fmaf(gk, x, R0x); R0xx = fmaf(gk, x * x, R0xx); } }
+                        else       { R1 += gk; if (k & 7) { R1x = fmaf(gk, x, R1x); R1xx = fmaf(gk, x * x, R1xx); } }
+                    }
+                }
+                float S0 = R0 + R1, Sx = R0x + R1x, Sxx = R0xx + R1xx;
+                float Sy = fmaf(hh, S0, R1), Sxy = fmaf(hh, Sx, R1x), Syy = fmaf(hh * hh, S0, fmaf(2.0f * hh, R1, R1));
+                S0 += __shfl_xor_sync(FULL, S0, 16);
+                Sx += __shfl_xor_sync(FULL, Sx, 16);
+                Sy += __shfl_xor_sync(FULL, Sy, 16);
+                Sxx += __shfl_xor_sync(FULL, Sxx, 16);
+                Sxy += __shfl_xor_sync(FULL, Sxy, 16);
+                Syy += __shfl_xor_sync(FULL, Syy, 16);
+                if (ABS) {
+                    Ax += __shfl_xor_sync(FULL, Ax, 16);
+                    Ay += __shfl_xor_sync(FULL, Ay, 16);
+                }
+                if ((present >> re) & 1u) {
+                    const int j = my_list[ii - re];
+                    const int g = __float_as_int(s_rec[j * 3 + 2].z);
+                    if (rh == 0) {
+                        const float4 r0 = s_rec[j * 3 + 0];
+                        const float4 r1 = s_rec[j * 3 + 1];
+                        const float A = r0.z * (-2.0f / LOG2E), B = r0.w * (-1.0f / LOG2E), Cc = r1.x * (-2.0f / LOG2E);
+                        const float ex = r0.x - bx0, ey = r0.y - by0;
+                        const float no = -r1.y;
+                        const float M1 = no * fmaf(ex, S0, -Sx), M2 = no * fmaf(ey, S0, -Sy);
+                        const float M3 = no * fmaf(ex, fmaf(ex, S0, -2.0f * Sx), Sxx);
+                        const float M4 = no * (fmaf(ex, fmaf(ey, S0, -Sy), Sxy) - ey * Sx);
+                        const float M5 = no * fmaf(ey, fmaf(ey, S0, -2.0f * Sy), Syy);
+                        atomicAdd(v_xy + 2 * int64_t(g), A * M1 + B * M2);
+                        atomicAdd(v_xy + 2 * int64_t(g) + 1, B * M1 + Cc * M2);
+                        atomicAdd(v_conic + 3 * int64_t(g), 0.5f * M3);
+                        atomicAdd(v_conic + 3 * int64_t(g) + 1, M4);
+                        atomicAdd(v_conic + 3 * int64_t(g) + 2, 0.5f * M5);
+                    } else {
+                        atomicAdd(v_opacity + g, S0);
+                        if (ABS) {
+                            atomicAdd(v_xy_abs + 2 * int64_t(g), Ax);
+                            atomicAdd(v_xy_abs + 2 * int64_t(g) + 1, Ay);
+                        }
+                    }
+                }
+            }
+            __syncwarp();   // the rows are read: the next group may overwrite the tile
+        }
+    }
+}
+
+// Sets the dynamic shared-memory limit of a kernel once (first launch) and launches it.
+template <typename Kernel, typename... Args>
+int launch_dyn(Kernel kernel, const cudaError_t& attr_rc, size_t smem, dim3 grid, cudaStream_t s, const char* what, Args... args) {
+    if (attr_rc != cudaSuccess) {
+        set_error("%s: cudaFuncSetAttribute failed: %s", what, cudaGetErrorString(attr_rc));
+        return B200GS_ECUDA;
+    }
+    kernel<<<grid, BLOCK_PIX, smem, s>>>(args...);
+    B200GS_LAUNCH_CHECK();
+    return B200GS_OK;
+}
+
+template <typename Kernel>
+cudaError_t set_smem(Kernel kernel, size_t smem) {
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    return e;
+}
+
+template <int CH>
+int feat_fwd_chunk(dim3 grid, int gx, int width, int height, const int32_t* ranges, const int32_t* ids, const float* xy, const float* conic,
+                   const float* opacity, const float* features, int D, int c0, int cw, const float* bg, float* image, float* final_T,
+                   int32_t* n_contrib, float* alpha, cudaStream_t s) {
+    const auto kernel = blend_feat_fwd_kernel<CH>;
+    static const cudaError_t attr_rc = set_smem(kernel, sizeof(FeatFwdSmem<CH>));
+    return launch_dyn(kernel, attr_rc, sizeof(FeatFwdSmem<CH>), grid, s, "blend_feat_fwd", width, height, gx,
+                      reinterpret_cast<const int2*>(ranges), ids, xy, conic, opacity, features, D, c0, cw, bg, image, final_T, n_contrib,
+                      alpha);
+}
+
+template <int CH, bool GEOM, bool ABS>
+int feat_bwd_chunk(dim3 grid, int gx, int width, int height, const int32_t* ranges, const int32_t* ids, const float* xy, const float* conic,
+                   const float* opacity, const float* features, int D, int c0, int cw, const float* bg, const float* final_T,
+                   const int32_t* n_contrib, const float* v_image, const float* v_alpha, float* v_features, float* v_xy, float* v_conic,
+                   float* v_opacity, float* v_xy_abs, cudaStream_t s) {
+    typedef FeatBwdSmem<CH, GEOM, ABS> Smem;
+    const auto kernel = blend_feat_bwd_kernel<CH, GEOM, ABS>;
+    static const cudaError_t attr_rc = set_smem(kernel, sizeof(Smem));
+    return launch_dyn(kernel, attr_rc, sizeof(Smem), grid, s, "blend_feat_bwd", width, height, gx, reinterpret_cast<const int2*>(ranges), ids,
+                      xy, conic, opacity, features, D, c0, cw, bg, final_T, n_contrib, v_image, v_alpha, v_features, v_xy, v_conic,
+                      v_opacity, v_xy_abs);
+}
+
 }  // namespace
 
 int launch_blend_fwd(int mode, int width, int height, int channels, const int32_t* ranges, const int32_t* ids, bool rows, const float* xy,
@@ -735,6 +1158,49 @@ int launch_blend_bwd(int mode, int width, int height, int channels, const int32_
     return by_channels[channels - 1][mode == B200GS_MODE_GSPLAT](rows, width, height, ranges, ids, xy, conic, opacity, colors, bg, final_T,
                                                                   n_contrib, v_image, pix_stride, ch_stride, v_alpha, sx, sy, v_xy, v_conic,
                                                                   v_opacity, v_colors, v_xy_abs, s);
+}
+
+// Chunks of 32 channels over the same binning; a chunk of cw channels runs the smallest instantiation >= cw.  Only chunk 0 writes
+// final_T / n_contrib / alpha (every chunk computes the same ones).
+int launch_blend_feat_fwd(int width, int height, int channels, const int32_t* ranges, const int32_t* ids, const float* xy, const float* conic,
+                          const float* opacity, const float* features, const float* bg, float* image, float* final_T, int32_t* n_contrib,
+                          float* alpha, cudaStream_t s) {
+    const int gx = div_up(width, TILE);
+    const dim3 grid(gx * div_up(height, TILE));
+    for (int c0 = 0; c0 < channels; c0 += 32) {
+        const int cw = min(32, channels - c0);
+        const bool first = c0 == 0;
+        const auto by_width = cw <= 8 ? feat_fwd_chunk<8> : cw <= 16 ? feat_fwd_chunk<16> : feat_fwd_chunk<32>;
+        const int rc = by_width(grid, gx, width, height, ranges, ids, xy, conic, opacity, features, channels, c0, cw, bg, image,
+                                first ? final_T : nullptr, first ? n_contrib : nullptr, first ? alpha : nullptr, s);
+        if (rc) return rc;
+    }
+    return B200GS_OK;
+}
+
+// Only chunk 0 takes the alpha cotangent: the geometry gradients are linear in the per-channel terms, so the chunks' sum is the
+// D-channel gradient.  v_xy == NULL selects the features-only kernels.  absgrad (v_xy_abs) is each chunk's |.| summed over chunks:
+// exact for D <= 32, an upper bound of the all-channel value beyond.
+int launch_blend_feat_bwd(int width, int height, int channels, const int32_t* ranges, const int32_t* ids, const float* xy, const float* conic,
+                          const float* opacity, const float* features, const float* bg, const float* final_T, const int32_t* n_contrib,
+                          const float* v_image, const float* v_alpha, float* v_features, float* v_xy, float* v_conic, float* v_opacity,
+                          float* v_xy_abs, cudaStream_t s) {
+    const int gx = div_up(width, TILE);
+    const dim3 grid(gx * div_up(height, TILE));
+    static constexpr decltype(&feat_bwd_chunk<8, false, false>) by_width[3][3] = {
+        {feat_bwd_chunk<8, false, false>, feat_bwd_chunk<8, true, false>, feat_bwd_chunk<8, true, true>},
+        {feat_bwd_chunk<16, false, false>, feat_bwd_chunk<16, true, false>, feat_bwd_chunk<16, true, true>},
+        {feat_bwd_chunk<32, false, false>, feat_bwd_chunk<32, true, false>, feat_bwd_chunk<32, true, true>}};
+    const int variant = v_xy == nullptr ? 0 : v_xy_abs == nullptr ? 1 : 2;
+    for (int c0 = 0; c0 < channels; c0 += 32) {
+        const int cw = min(32, channels - c0);
+        const int rc = by_width[cw <= 8 ? 0 : cw <= 16 ? 1 : 2][variant](grid, gx, width, height, ranges, ids, xy, conic, opacity, features,
+                                                                          channels, c0, cw, bg, final_T, n_contrib, v_image,
+                                                                          c0 == 0 ? v_alpha : nullptr, v_features, v_xy, v_conic, v_opacity,
+                                                                          v_xy_abs, s);
+        if (rc) return rc;
+    }
+    return B200GS_OK;
 }
 
 }  // namespace b200gs

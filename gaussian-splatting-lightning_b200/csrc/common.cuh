@@ -147,5 +147,13 @@ int launch_blend_bwd(int mode, int width, int height, int channels, const int32_
                      const float* final_T, const int32_t* n_contrib, const float* v_image, int64_t pix_stride,
                      int64_t ch_stride, const float* v_alpha, float sx, float sy, float* v_xy, float* v_conic,
                      float* v_opacity, float* v_colors, float* v_xy_abs, cudaStream_t s);
+// gsplat mode, any channel count >= 1 (chunks of 32); [n, channels] features, [H, W, channels] image; v_xy == NULL: features only
+int launch_blend_feat_fwd(int width, int height, int channels, const int32_t* ranges, const int32_t* ids, const float* xy, const float* conic,
+                          const float* opacity, const float* features, const float* bg, float* image, float* final_T, int32_t* n_contrib,
+                          float* alpha, cudaStream_t s);
+int launch_blend_feat_bwd(int width, int height, int channels, const int32_t* ranges, const int32_t* ids, const float* xy, const float* conic,
+                          const float* opacity, const float* features, const float* bg, const float* final_T, const int32_t* n_contrib,
+                          const float* v_image, const float* v_alpha, float* v_features, float* v_xy, float* v_conic, float* v_opacity,
+                          float* v_xy_abs, cudaStream_t s);
 
 }  // namespace b200gs

@@ -283,23 +283,26 @@ def blend_forward_rows(mode, width, height, binning: Binning, rows, bg, planar=F
     return image, final_T, n_contrib
 
 
-def bin_and_blend_rows(mode, width, height, rows, bg, cull=True, planar=False, block_counts=None, block_rows=0):
-    binning = bin_rows(mode, width, height, rows, cull, lazy=True, block_counts=block_counts, block_rows=block_rows)
-    out = blend_forward_rows(mode, width, height, binning, rows, bg, planar)
+def _bin_then_blend(bin_fn, blend_fn):
+    """The lazy (sync-free) binning protocol: bin_fn(lazy=True) sizes the lists from the previous view's counts, blend_fn(binning)
+    is enqueued, and only then are the counts checked; in the rare case a capacity was exceeded both are redone exactly."""
+    binning = bin_fn(True)
+    out = blend_fn(binning)
     if not binning.resolve():
-        binning = bin_rows(mode, width, height, rows, cull, lazy=False, block_counts=block_counts, block_rows=block_rows)
-        out = blend_forward_rows(mode, width, height, binning, rows, bg, planar)
+        binning = bin_fn(False)
+        out = blend_fn(binning)
     return binning, out
+
+
+def bin_and_blend_rows(mode, width, height, rows, bg, cull=True, planar=False, block_counts=None, block_rows=0):
+    return _bin_then_blend(lambda lazy: bin_rows(mode, width, height, rows, cull, lazy=lazy, block_counts=block_counts, block_rows=block_rows),
+                           lambda binning: blend_forward_rows(mode, width, height, binning, rows, bg, planar))
 
 
 def bin_and_blend(mode, width, height, xy, depth, radii, conic, opacity, colors, bg, planar, want_alpha):
     """Forward binning + blend with the lazy (sync-free) pair count; falls back to an exact re-run on overflow."""
-    binning = bin_gaussians(mode, width, height, xy, depth, radii, conic, opacity, lazy=True)
-    out = blend_forward(mode, width, height, binning, xy, conic, opacity, colors, bg, planar, want_alpha)
-    if not binning.resolve():
-        binning = bin_gaussians(mode, width, height, xy, depth, radii, conic, opacity, lazy=False)
-        out = blend_forward(mode, width, height, binning, xy, conic, opacity, colors, bg, planar, want_alpha)
-    return binning, out
+    return _bin_then_blend(lambda lazy: bin_gaussians(mode, width, height, xy, depth, radii, conic, opacity, lazy=lazy),
+                           lambda binning: blend_forward(mode, width, height, binning, xy, conic, opacity, colors, bg, planar, want_alpha))
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -390,6 +393,47 @@ def blend_backward(mode, width, height, binning: Binning, xy, conic, opacity, co
                                  ptr(v_alpha), float(xy_scale[0]), float(xy_scale[1]), ptr(v_xy), ptr(v_conic), ptr(v_opacity),
                                  ptr(v_colors), ptr(v_abs), _stream()), "b200gs_blend_bwd")
     return v_xy, v_conic, v_opacity, v_colors, v_abs
+
+
+def blend_features_forward(width, height, binning: Binning, xy, conic, opacity, features, bg):
+    """Gsplat-mode blend of [N, D] features, any D >= 1 (b200gs_blend_feat_fwd: chunks of 32 channels over one binning)
+    -> image [H,W,D], final_T, n_contrib, alpha."""
+    L = lib()
+    d = features.shape[1]
+    dev = xy.device
+    image = torch.empty(height, width, d, dtype=torch.float32, device=dev)
+    final_T = torch.empty(height, width, dtype=torch.float32, device=dev)
+    n_contrib = torch.empty(height, width, dtype=torch.int32, device=dev)
+    alpha = torch.empty(height, width, dtype=torch.float32, device=dev)
+    with _stage("blend_feat_fwd"):
+        check(L.b200gs_blend_feat_fwd(width, height, d, ptr(binning.tile_ranges), ptr(binning.sorted_ids), ptr(xy), ptr(conic), ptr(opacity),
+                                      ptr(features), ptr(bg), ptr(image), ptr(final_T), ptr(n_contrib), ptr(alpha), _stream()),
+              "b200gs_blend_feat_fwd")
+    return image, final_T, n_contrib, alpha
+
+
+def blend_features_backward(width, height, binning: Binning, xy, conic, opacity, features, bg, final_T, n_contrib, v_image, v_alpha,
+                            geometry: bool = True, want_abs: bool = False):
+    """Backward of blend_features_forward -> (v_xy, v_conic, v_opacity, v_features, v_abs).  geometry=False runs the features-only
+    kernels: v_xy / v_conic / v_opacity / v_abs are None and no geometry gradient is computed."""
+    L = lib()
+    n, d = features.shape
+    dev = xy.device
+    cols = d + ((2 + 3 + 1 + (2 if want_abs else 0)) if geometry else 0)
+    slab = torch.zeros(n * cols, dtype=torch.float32, device=dev)     # one zero-filled slab for all atomically accumulated outputs
+    v_feat = slab[:n * d].view(n, d)
+    v_xy = v_conic = v_opacity = v_abs = None
+    if geometry:
+        o = n * d
+        v_xy = slab[o:o + 2 * n].view(n, 2); o += 2 * n
+        v_conic = slab[o:o + 3 * n].view(n, 3); o += 3 * n
+        v_opacity = slab[o:o + n]; o += n
+        v_abs = slab[o:o + 2 * n].view(n, 2) if want_abs else None
+    with _stage("blend_feat_bwd"):
+        check(L.b200gs_blend_feat_bwd(width, height, d, ptr(binning.tile_ranges), ptr(binning.sorted_ids), ptr(xy), ptr(conic), ptr(opacity),
+                                      ptr(features), ptr(bg), ptr(final_T), ptr(n_contrib), ptr(v_image), ptr(v_alpha), ptr(v_feat), ptr(v_xy),
+                                      ptr(v_conic), ptr(v_opacity), ptr(v_abs), _stream()), "b200gs_blend_feat_bwd")
+    return v_xy, v_conic, v_opacity, v_feat, v_abs
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -651,17 +695,61 @@ class _RasterizeGaussians(torch.autograd.Function):
         return v_xy, None, None, v_conic, v_colors, v_opacity.reshape(ctx.opac_shape), None, None, None, None, None
 
 
+class _RasterizeFeatures(torch.autograd.Function):
+    """rasterize_gaussians for D > 4 channels (the reference's feature renderers: 32-channel features, often with the geometry
+    frozen).  One binning, the D-channel blend kernels; the backward runs the features-only kernels when none of xys, conics and
+    opacity needs a gradient."""
+
+    @staticmethod
+    def forward(ctx, xys, depths, radii, conics, colors, opacity, img_height, img_width, background, absgrad):
+        xys = _f32c(xys, "xys")
+        depths = _f32c(depths, "depths")
+        conics = _f32c(conics, "conics")
+        colors = _f32c(colors, "colors")
+        opac = _f32c(opacity, "opacity").reshape(-1)
+        radii = radii.contiguous()
+        bg = _f32c(background, "background") if background is not None else None
+        H, W = int(img_height), int(img_width)
+        binning, (image, final_T, n_contrib, alpha) = _bin_then_blend(
+            lambda lazy: bin_gaussians(MODE_GSPLAT, W, H, xys, depths, radii, conics, opac, lazy=lazy),
+            lambda binning: blend_features_forward(W, H, binning, xys, conics, opac, colors, bg))
+        ctx.binning, ctx.hw, ctx.absgrad, ctx.opac_shape = binning, (H, W), bool(absgrad), tuple(opacity.shape)
+        ctx.save_for_backward(xys, conics, colors, opac, bg, final_T, n_contrib)
+        ctx.xys_ref = xys
+        return image, alpha
+
+    @staticmethod
+    def backward(ctx, v_image, v_alpha):
+        xys, conics, colors, opac, bg, final_T, n_contrib = ctx.saved_tensors
+        H, W = ctx.hw
+        need = ctx.needs_input_grad
+        geometry = need[0] or need[3] or need[5]
+        v_image = _f32c(v_image, "grad_image")
+        v_alpha = _f32c(v_alpha, "grad_alpha") if v_alpha is not None else None
+        v_xy, v_conic, v_opacity, v_colors, v_abs = blend_features_backward(W, H, ctx.binning, xys, conics, opac, colors, bg, final_T,
+                                                                            n_contrib, v_image, v_alpha, geometry, geometry and ctx.absgrad)
+        if v_abs is not None:
+            ctx.xys_ref.absgrad = v_abs
+        return (v_xy, None, None, v_conic, v_colors if need[4] else None, v_opacity.reshape(ctx.opac_shape) if geometry else None,
+                None, None, None, None)
+
+
 def rasterize_gaussians(xys, depths, radii, conics, num_tiles_hit, colors, opacity, img_height, img_width, block_width=16,
                         background=None, return_alpha=False, absgrad=False):
-    """gsplat v0 ``rasterize_gaussians`` -> [H,W,D] (and alpha [H,W] when return_alpha)."""
+    """gsplat v0 ``rasterize_gaussians`` -> [H,W,D] (and alpha [H,W] when return_alpha), any D >= 1.  D <= 4 runs K6 / K7; wider
+    feature maps run the D-channel kernels in chunks of 32 channels over one binning.  `xys.absgrad` is exact for D <= 32; beyond,
+    it is the sum of each 32-channel chunk's value (an upper bound of gsplat's all-channel value)."""
     if block_width != TILE:
         raise ValueError(f"b200gs supports block_width {TILE} only")
-    if colors.dim() != 2 or not (1 <= colors.shape[1] <= 4):
-        raise ValueError("colors must be [N, D] with 1 <= D <= 4")
+    if colors.dim() != 2 or colors.shape[1] < 1:
+        raise ValueError("colors must be [N, D] with D >= 1")
     if background is not None and background.shape[0] != colors.shape[1]:
         raise ValueError("background must have one entry per colour channel")
-    image, alpha = _RasterizeGaussians.apply(xys, depths, radii, conics, colors, opacity, img_height, img_width, background,
-                                             return_alpha, absgrad)
+    if colors.shape[1] <= 4:
+        image, alpha = _RasterizeGaussians.apply(xys, depths, radii, conics, colors, opacity, img_height, img_width, background,
+                                                 return_alpha, absgrad)
+    else:
+        image, alpha = _RasterizeFeatures.apply(xys, depths, radii, conics, colors, opacity, img_height, img_width, background, absgrad)
     return (image, alpha) if return_alpha else image
 
 

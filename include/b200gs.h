@@ -222,6 +222,26 @@ B200GS_API int b200gs_blend_bwd(int32_t mode, int32_t width, int32_t height, int
                      float xy_scale_x, float xy_scale_y, float* v_xy, float* v_conic, float* v_opacity,
                      float* v_colors, float* v_xy_abs, void* stream);
 
+/* ---- wide feature maps: K6 / K7 for any channel count (gsplat mode) ------------------------------------------------------
+ * gsplat rasterize_gaussians with colors [n, D], D >= 1 — the reference's feature renderers composite 32-channel features
+ * (internal/segany_splatting.py, seganygs_renderer.py, feature_3dgs_renderer.py).  Processed in chunks of 32 channels over the same
+ * tile lists; per channel the arithmetic is K6's, so the composite of every channel is bit-identical to K6 on the same lists.
+ * The background is added as one FMA, fmaf(final_T, bg[c], composite); K6 rounds final_T * bg[c] separately for some channels,
+ * so with a background a channel may differ from K6's by that one rounding.
+ * in : xy[n,2] conic[n,3] opacity[n] features[n,channels] (contiguous); bg[channels] or NULL.
+ * fwd out: image[H,W,channels], final_T[H*W], n_contrib[H*W], alpha[H*W] = 1 - final_T (nullable).
+ * bwd in : final_T, n_contrib, v_image[H,W,channels], v_alpha[H*W] (nullable).
+ * bwd out (ACCUMULATED with atomics — caller zero-fills): v_features[n,channels]; v_xy[n,2] (pixel units), v_conic[n,3],
+ *      v_opacity[n] — all three given, or all NULL for the features-only kernel (no geometry work at all); v_xy_abs[n,2]
+ *      (nullable, needs v_xy): gsplat absgrad, exact for channels <= 32, the sum of each 32-channel chunk's value beyond. */
+B200GS_API int b200gs_blend_feat_fwd(int32_t width, int32_t height, int32_t channels, const int32_t* tile_ranges, const int32_t* sorted_ids,
+                                     const float* xy, const float* conic, const float* opacity, const float* features, const float* bg,
+                                     float* image, float* final_T, int32_t* n_contrib, float* alpha, void* stream);
+B200GS_API int b200gs_blend_feat_bwd(int32_t width, int32_t height, int32_t channels, const int32_t* tile_ranges, const int32_t* sorted_ids,
+                                     const float* xy, const float* conic, const float* opacity, const float* features, const float* bg,
+                                     const float* final_T, const int32_t* n_contrib, const float* v_image, const float* v_alpha,
+                                     float* v_features, float* v_xy, float* v_conic, float* v_opacity, float* v_xy_abs, void* stream);
+
 /* ---- fused L1 + SSIM training loss on the rendered image (validated by tests/test_gpu_loss.py) ----------------------------------
  * replaces  loss = (1-lambda) * l1_loss(image, gt) + lambda * (1 - ssim(image, gt))   (internal/metrics/vanilla_metrics.py:57-74,
  * internal/utils/ssim.py:17-63: 11-tap Gaussian window sigma 1.5, zero padding, C1 = 0.01^2, C2 = 0.03^2).  image/target [C,H,W].
