@@ -48,6 +48,10 @@ _SIGNATURES = {
     "b200gs_knn_mean_dist2": (c_int32, [c_int64, _P, _P, _P, c_size_t, _P]),
     "b200gs_sh_fwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P]),
     "b200gs_sh_bwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P, _P, _P]),
+    "b200gs_sh_split_fwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P, _P, _P]),
+    "b200gs_sh_split_bwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "b200gs_isect_keys": (c_int32, [c_int32, _P, _P, c_int64, _P, _P, _P]),
+    "b200gs_isect_offsets": (c_int32, [c_int64, _P, c_int32, _P, _P]),
     "b200gs_bin_count_workspace_bytes": (c_size_t, [c_int64]),
     "b200gs_bin_sort_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int32, c_int32]),
     "b200gs_bin_count": (c_int32, [c_int32, c_int32, c_int32, c_int64, _P, _P, _P, _P, _P, _P, c_size_t, _P, _P, c_int32, _P]),

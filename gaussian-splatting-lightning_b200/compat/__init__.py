@@ -1,7 +1,8 @@
 """Drop-in modules carrying the names the reference imports from its CUDA pip dependencies.
 
 ``install()`` aliases them in ``sys.modules`` so that the UNMODIFIED reference renderers
-(``internal/renderers/vanilla_renderer.py:14``, ``gsplat_renderer.py:2-4``) run on the b200gs kernels:
+(``internal/renderers/vanilla_renderer.py:14``, ``gsplat_renderer.py:2-4``, ``gsplat_v1_renderer.py:8-20``) run on the b200gs
+kernels:
 
     import b200gs.compat; b200gs.compat.install()
     from internal.renderers.vanilla_renderer import VanillaRenderer   # now backed by libb200gs.so
@@ -12,7 +13,7 @@ import types
 
 def install(force: bool = False):
     from . import diff_gaussian_rasterization as dgr
-    from . import gsplat_v0
+    from . import gsplat_v0, gsplat_v1
 
     def put(name, module):
         if force or name not in sys.modules:
@@ -41,7 +42,22 @@ def install(force: bool = False):
         m = types.ModuleType(f"gsplat.{sub}")
         for nm in names:
             setattr(m, nm, getattr(gsplat_v0, nm))
+        if sub == "v0_interfaces":     # gsplat_v1_renderer.py:20
+            m.rasterize_to_pixels = gsplat_v1.rasterize_to_pixels
         put(f"gsplat.{sub}", m)
+    # gsplat v1 (gsplat_v1_renderer.py:8-20)
+    cuda = types.ModuleType("gsplat.cuda")
+    cuda.__path__ = []
+    pkg.cuda = cuda
+    for sub, names in (("cuda._wrapper", ("fully_fused_projection", "isect_tiles", "isect_offset_encode", "spherical_harmonics")),
+                       ("cuda.isect_tiles_tile_based_culling", ("isect_tiles_tile_based_culling", "isect_offset_encode_tile_based_culling")),
+                       ("sh_decomposed", ("spherical_harmonics_decomposed",))):
+        m = types.ModuleType(f"gsplat.{sub}")
+        for nm in names:
+            setattr(m, nm, getattr(gsplat_v1, nm))
+        setattr(cuda if sub.startswith("cuda.") else pkg, sub.split(".")[-1], m)
+        put(f"gsplat.{sub}", m)
+    put("gsplat.cuda", cuda)
     # gsplat.relocation.compute_relocation (internal/density_controllers/mcmc_density_controller.py:13)
     from .. import mcmc
     reloc = types.ModuleType("gsplat.relocation")

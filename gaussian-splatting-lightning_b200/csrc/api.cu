@@ -41,7 +41,7 @@ using namespace b200gs;
 extern "C" {
 
 const char* b200gs_last_error(void) { return g_error; }
-int b200gs_version(void) { return 224; }
+int b200gs_version(void) { return 225; }
 int64_t b200gs_launch_count(void) { return (int64_t)g_launches.load(std::memory_order_relaxed); }
 
 int b200gs_project_fwd(const B200gsView* view, int64_t n, const float* means, const float* scales, const float* quats,
@@ -275,6 +275,40 @@ int b200gs_sh_bwd(int32_t degree, int32_t sh_stride, int64_t n, const float* dir
     B200GS_CHECK_ARG(n >= 0, "n < 0");
     B200GS_CHECK_ARG(n == 0 || (dirs && coeffs && v_rgb && v_coeffs), "NULL pointer");
     return launch_sh_bwd(degree, sh_stride, n, dirs, coeffs, v_rgb, v_coeffs, v_dirs, (cudaStream_t)stream);
+}
+
+int b200gs_sh_split_fwd(int32_t degree, int32_t k_rest, int64_t n, const float* dirs, const float* dc, const float* rest, const uint8_t* mask,
+                        float* rgb, void* stream) {
+    B200GS_CHECK_ARG(degree >= 0 && degree <= 4, "degree must be 0..4");
+    B200GS_CHECK_ARG(k_rest >= 0 && k_rest + 1 >= (degree + 1) * (degree + 1), "1 + k_rest < (degree+1)^2");
+    B200GS_CHECK_ARG(n >= 0, "n < 0");
+    B200GS_CHECK_ARG(n == 0 || (dirs && dc && rgb && (k_rest == 0 || rest)), "NULL pointer");
+    return launch_sh_fwd(degree, k_rest + 1, n, dirs, dc, rgb, (cudaStream_t)stream, true, rest, mask);
+}
+
+int b200gs_sh_split_bwd(int32_t degree, int32_t k_rest, int64_t n, const float* dirs, const float* dc, const float* rest, const uint8_t* mask,
+                        const float* v_rgb, float* v_dc, float* v_rest, float* v_dirs, void* stream) {
+    B200GS_CHECK_ARG(degree >= 0 && degree <= 4, "degree must be 0..4");
+    B200GS_CHECK_ARG(k_rest >= 0 && k_rest + 1 >= (degree + 1) * (degree + 1), "1 + k_rest < (degree+1)^2");
+    B200GS_CHECK_ARG(n >= 0, "n < 0");
+    B200GS_CHECK_ARG(n == 0 || (dirs && dc && v_rgb && v_dc && (k_rest == 0 || (rest && v_rest))), "NULL pointer");
+    return launch_sh_bwd(degree, k_rest + 1, n, dirs, dc, v_rgb, v_dc, v_dirs, (cudaStream_t)stream, true, rest, mask, v_rest);
+}
+
+int b200gs_isect_keys(int32_t n_tiles, const int32_t* tile_ranges, const int32_t* sorted_ids, int64_t n_pairs, const float* depth,
+                      int64_t* keys, void* stream) {
+    B200GS_CHECK_ARG(n_tiles >= 0 && n_pairs >= 0 && n_pairs < (int64_t(1) << 31), "bad size");
+    B200GS_CHECK_ARG(n_tiles == 0 || tile_ranges, "tile_ranges must not be NULL");
+    B200GS_CHECK_ARG(n_pairs == 0 || (sorted_ids && depth && keys), "NULL pointer");
+    B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(tile_ranges) & 7u) == 0, "tile_ranges must be 8-byte aligned");
+    return launch_isect_keys(n_tiles, tile_ranges, sorted_ids, n_pairs, depth, keys, (cudaStream_t)stream);
+}
+
+int b200gs_isect_offsets(int64_t n_pairs, const int64_t* keys, int32_t n_tiles, int32_t* offsets, void* stream) {
+    B200GS_CHECK_ARG(n_tiles >= 0 && n_pairs >= 0 && n_pairs < (int64_t(1) << 31), "bad size");
+    B200GS_CHECK_ARG(n_tiles == 0 || offsets, "offsets must not be NULL");
+    B200GS_CHECK_ARG(n_pairs == 0 || keys, "keys must not be NULL");
+    return launch_isect_offsets(n_pairs, keys, n_tiles, offsets, (cudaStream_t)stream);
 }
 
 size_t b200gs_bin_count_workspace_bytes(int64_t n) { return n < 0 ? 0 : bin_count_workspace_bytes(n); }

@@ -99,9 +99,16 @@ int launch_project_bwd_multi(const B200gsView* views, int n_views, int64_t n, co
                              const float* opac_logits, const float* shs_rest, int anti_aliased, const int32_t* radii, const uint8_t* clamped,
                              const int32_t* row_index, const float* const* v_rows, float* v_means, float* v_scales, float* v_quats,
                              float* v_opac_logit, float* v_shs_dc, float* v_shs_rest, cudaStream_t s);
-int launch_sh_fwd(int degree, int stride, int64_t n, const float* dirs, const float* coeffs, float* rgb, cudaStream_t s);
+// split = true: coeffs / v_coeffs are dc [n,1,3], rest / v_rest [n,stride-1,3] read and written in place, mask[n] (nullable) zeroes rows
+int launch_sh_fwd(int degree, int stride, int64_t n, const float* dirs, const float* coeffs, float* rgb, cudaStream_t s, bool split = false,
+                  const float* rest = nullptr, const uint8_t* mask = nullptr);
 int launch_sh_bwd(int degree, int stride, int64_t n, const float* dirs, const float* coeffs, const float* v_rgb,
-                  float* v_coeffs, float* v_dirs, cudaStream_t s);
+                  float* v_coeffs, float* v_dirs, cudaStream_t s, bool split = false, const float* rest = nullptr,
+                  const uint8_t* mask = nullptr, float* v_rest = nullptr);
+// gsplat isect_ids / isect_offset_encode for one camera (isect.cu)
+int launch_isect_keys(int n_tiles, const int32_t* tile_ranges, const int32_t* sorted_ids, int64_t n_pairs, const float* depth, int64_t* keys,
+                      cudaStream_t s);
+int launch_isect_offsets(int64_t n_pairs, const int64_t* keys, int n_tiles, int32_t* offsets, cudaStream_t s);
 
 size_t bin_count_workspace_bytes(int64_t n);
 size_t bin_sort_workspace_bytes(int64_t n, int64_t max_coarse, int width, int height);

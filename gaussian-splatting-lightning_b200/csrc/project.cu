@@ -1012,17 +1012,30 @@ __global__ void __launch_bounds__(BWD_THREADS) project_bwd_multi_kernel(const __
 // ------------------------------------------------------------------------------------------------------------------
 // standalone SH (gsplat.sh.spherical_harmonics)
 // ------------------------------------------------------------------------------------------------------------------
-template <int MC>
+// SPLIT = false: coeffs [n, stride, 3].  SPLIT = true (gsplat's spherical_harmonics_decomposed): coeffs = dc [n, 1, 3] and
+// rest [n, stride - 1, 3] read in place through K1's RAW loader; a row with mask[i] == 0 (mask nullable) reads no coefficient and
+// gets rgb = 0 and zero gradients.  The evaluation is the same code in both, so unmasked rows are bit-identical.
+template <bool SPLIT>
+__device__ __forceinline__ bool sh_row_masked(const uint8_t* __restrict__ mask, int64_t i) {
+    return SPLIT && mask != nullptr && __ldg(mask + i) == 0;
+}
+
+template <bool SPLIT, int MC>
 __global__ void __launch_bounds__(256) sh_fwd_kernel(int deg, int stride, int64_t n, const float* __restrict__ dirs,
-                                                     const float* __restrict__ coeffs, float* __restrict__ rgb) {
+                                                     const float* __restrict__ coeffs, const float* __restrict__ rest,
+                                                     const uint8_t* __restrict__ mask, float* __restrict__ rgb) {
     const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    if (sh_row_masked<SPLIT>(mask, i)) {
+        rgb[3 * i] = 0.f; rgb[3 * i + 1] = 0.f; rgb[3 * i + 2] = 0.f;
+        return;
+    }
     const int ncoef = (deg + 1) * (deg + 1);
     float dx = __ldg(dirs + 3 * i), dy = __ldg(dirs + 3 * i + 1), dz = __ldg(dirs + 3 * i + 2);
     const float inv_len = 1.0f / fmaxf(sqrtf(dx * dx + dy * dy + dz * dz), 1e-12f);
     dx *= inv_len; dy *= inv_len; dz *= inv_len;
     float sh[MC * 3];
-    load_sh<MC>(coeffs + i * int64_t(stride) * 3, ncoef, ((stride * 3) & 3) == 0, sh);
+    load_sh_any<SPLIT, MC>(coeffs, rest, i, stride, ncoef, sh);
     float bs[MC];
     sh_basis<MC>(deg, dx, dy, dz, bs);
     float r = 0.f, g = 0.f, b = 0.f;
@@ -1032,31 +1045,43 @@ __global__ void __launch_bounds__(256) sh_fwd_kernel(int deg, int stride, int64_
     rgb[3 * i] = r; rgb[3 * i + 1] = g; rgb[3 * i + 2] = b;
 }
 
-template <int MC>
+// SPLIT: v_coeffs = v_dc [n, 1, 3], v_rest [n, stride - 1, 3]; both fully written (zeros on masked rows)
+template <bool SPLIT, int MC>
 __global__ void __launch_bounds__(256) sh_bwd_kernel(int deg, int stride, int64_t n, const float* __restrict__ dirs,
-                                                     const float* __restrict__ coeffs, const float* __restrict__ v_rgb,
-                                                     float* __restrict__ v_coeffs, float* __restrict__ v_dirs) {
+                                                     const float* __restrict__ coeffs, const float* __restrict__ rest,
+                                                     const uint8_t* __restrict__ mask, const float* __restrict__ v_rgb,
+                                                     float* __restrict__ v_coeffs, float* __restrict__ v_rest, float* __restrict__ v_dirs) {
     const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const int ncoef = (deg + 1) * (deg + 1);
     const int stride3 = stride * 3;
-    const bool vec4 = (stride3 & 3) == 0;
+    // gradient row of coefficient k: [n, stride, 3], or dc (k = 0) | rest (k >= 1)
+    const auto v_row = [&](int k) { return SPLIT ? (k == 0 ? v_coeffs + 3 * i : v_rest + (i * int64_t(stride - 1) + (k - 1)) * 3)
+                                                 : v_coeffs + i * int64_t(stride3) + 3 * k; };
+    if (sh_row_masked<SPLIT>(mask, i)) {
+        for (int k = 0; k < stride; ++k) {
+            float* o = v_row(k);
+            o[0] = 0.f; o[1] = 0.f; o[2] = 0.f;
+        }
+        if (v_dirs != nullptr) { v_dirs[3 * i] = 0.f; v_dirs[3 * i + 1] = 0.f; v_dirs[3 * i + 2] = 0.f; }
+        return;
+    }
+    const int ncoef = (deg + 1) * (deg + 1);
     float dx = __ldg(dirs + 3 * i), dy = __ldg(dirs + 3 * i + 1), dz = __ldg(dirs + 3 * i + 2);
     const float inv_len = 1.0f / fmaxf(sqrtf(dx * dx + dy * dy + dz * dz), 1e-12f);
     dx *= inv_len; dy *= inv_len; dz *= inv_len;
     const float gr = __ldg(v_rgb + 3 * i), gg = __ldg(v_rgb + 3 * i + 1), gb = __ldg(v_rgb + 3 * i + 2);
     float bs[MC];
     sh_basis<MC>(deg, dx, dy, dz, bs);
-    float* o = v_coeffs + i * int64_t(stride3);
     for (int k = 0; k < stride; ++k) {
         const float bk = (k < ncoef) ? bs[k] : 0.f;
-        o[3 * k] = bk * gr; o[3 * k + 1] = bk * gg; o[3 * k + 2] = bk * gb;
+        float* o = v_row(k);
+        o[0] = bk * gr; o[1] = bk * gg; o[2] = bk * gb;
     }
     if (v_dirs != nullptr) {
         float ddx = 0.f, ddy = 0.f, ddz = 0.f;
         if (deg > 0) {
             float sh[MC * 3];
-            load_sh<MC>(coeffs + i * int64_t(stride3), ncoef, vec4, sh);
+            load_sh_any<SPLIT, MC>(coeffs, rest, i, stride, ncoef, sh);
             float w[MC];
 #pragma unroll
             for (int k = 1; k < MC; ++k) w[k] = (k < ncoef) ? sh[3 * k] * gr + sh[3 * k + 1] * gg + sh[3 * k + 2] * gb : 0.f;
@@ -1229,19 +1254,24 @@ int launch_project_bwd_multi(const B200gsView* views, int n_views, int64_t n, co
     return B200GS_OK;
 }
 
-int launch_sh_fwd(int degree, int stride, int64_t n, const float* dirs, const float* coeffs, float* rgb, cudaStream_t s) {
+// split: coeffs = dc, rest / v_rest as in sh_fwd_kernel; otherwise rest, mask and v_rest are ignored
+int launch_sh_fwd(int degree, int stride, int64_t n, const float* dirs, const float* coeffs, float* rgb, cudaStream_t s, bool split,
+                  const float* rest, const uint8_t* mask) {
+    static constexpr decltype(&sh_fwd_kernel<false, 16>) kernels[2][2] = {
+        {sh_fwd_kernel<false, 16>, sh_fwd_kernel<false, 25>}, {sh_fwd_kernel<true, 16>, sh_fwd_kernel<true, 25>}};
     if (n == 0) return B200GS_OK;
-    const auto kernel = degree > 3 ? sh_fwd_kernel<25> : sh_fwd_kernel<16>;
-    kernel<<<(unsigned)div_up64(n, 256), 256, 0, s>>>(degree, stride, n, dirs, coeffs, rgb);
+    kernels[split][degree > 3]<<<(unsigned)div_up64(n, 256), 256, 0, s>>>(degree, stride, n, dirs, coeffs, rest, mask, rgb);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
 int launch_sh_bwd(int degree, int stride, int64_t n, const float* dirs, const float* coeffs, const float* v_rgb,
-                  float* v_coeffs, float* v_dirs, cudaStream_t s) {
+                  float* v_coeffs, float* v_dirs, cudaStream_t s, bool split, const float* rest, const uint8_t* mask, float* v_rest) {
+    static constexpr decltype(&sh_bwd_kernel<false, 16>) kernels[2][2] = {
+        {sh_bwd_kernel<false, 16>, sh_bwd_kernel<false, 25>}, {sh_bwd_kernel<true, 16>, sh_bwd_kernel<true, 25>}};
     if (n == 0) return B200GS_OK;
-    const auto kernel = degree > 3 ? sh_bwd_kernel<25> : sh_bwd_kernel<16>;
-    kernel<<<(unsigned)div_up64(n, 256), 256, 0, s>>>(degree, stride, n, dirs, coeffs, v_rgb, v_coeffs, v_dirs);
+    kernels[split][degree > 3]<<<(unsigned)div_up64(n, 256), 256, 0, s>>>(degree, stride, n, dirs, coeffs, rest, mask, v_rgb, v_coeffs,
+                                                                          v_rest, v_dirs);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }

@@ -9,6 +9,8 @@ Functions
   project_gaussians(...)      gsplat v0 ``project_gaussians``          (gsplat_renderer.py:64-79)
   spherical_harmonics(...)    gsplat ``spherical_harmonics``           (gsplat_renderer.py:105)
   rasterize_gaussians(...)    gsplat v0 ``rasterize_gaussians``        (gsplat_renderer.py:86-99)
+  spherical_harmonics_decomposed(...)  gsplat ``sh_decomposed``   (gsplat_v1_renderer.py:124)
+  isect_keys / isect_offsets  gsplat v1 ``isect_tiles`` keys / ``isect_offset_encode``   (gsplat_v1_renderer.py:446,458)
 """
 import ctypes
 import os
@@ -661,6 +663,46 @@ def spherical_harmonics(degrees_to_use: int, dirs: torch.Tensor, coeffs: torch.T
     return _SphericalHarmonics.apply(degrees_to_use, dirs, coeffs)
 
 
+class _SphericalHarmonicsSplit(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, degree: int, dirs, dc, rest, mask):
+        dirs, dc, rest = _f32c(dirs, "dirs"), _f32c(dc, "dc"), _f32c(rest, "coeffs")
+        n, k_rest = dc.shape[0], rest.shape[1]
+        rgb = torch.empty(n, 3, dtype=torch.float32, device=dc.device)
+        check(lib().b200gs_sh_split_fwd(int(degree), k_rest, n, ptr(dirs), ptr(dc), ptr(rest), ptr(mask), ptr(rgb), _stream()),
+              "b200gs_sh_split_fwd")
+        ctx.degree = int(degree)
+        ctx.save_for_backward(dirs, dc, rest, mask)
+        return rgb
+
+    @staticmethod
+    def backward(ctx, v_rgb):
+        dirs, dc, rest, mask = ctx.saved_tensors
+        n, k_rest = dc.shape[0], rest.shape[1]
+        v_rgb = _f32c(v_rgb, "grad")
+        v_dc, v_rest = torch.empty_like(dc), torch.empty_like(rest)
+        v_dirs = torch.empty_like(dirs) if ctx.needs_input_grad[1] else None
+        check(lib().b200gs_sh_split_bwd(ctx.degree, k_rest, n, ptr(dirs), ptr(dc), ptr(rest), ptr(mask), ptr(v_rgb), ptr(v_dc), ptr(v_rest),
+                                        ptr(v_dirs), _stream()), "b200gs_sh_split_bwd")
+        return None, v_dirs, v_dc, v_rest, None
+
+
+def spherical_harmonics_decomposed(degrees_to_use: int, dirs: torch.Tensor, dc: torch.Tensor, coeffs: torch.Tensor,
+                                   masks: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``spherical_harmonics_decomposed(deg, dirs[N,3], dc[N,1,3], coeffs[N,K-1,3], masks[N]=None) -> [N,3]`` of yzslab's gsplat fork:
+    SH on dc | rest read in place (no concatenation).  Rows with masks[i] false read no coefficient and get rgb = 0 and zero
+    gradients; the other rows are bit-identical to spherical_harmonics on torch.cat((dc, coeffs), 1)."""
+    n = dc.shape[0]
+    if dc.shape != (n, 1, 3) or coeffs.dim() != 3 or coeffs.shape[0] != n or coeffs.shape[2] != 3 or dirs.shape != (n, 3):
+        raise ValueError("expected dirs [N,3], dc [N,1,3] and coeffs [N,K-1,3]")
+    mask = None
+    if masks is not None:
+        if masks.shape != (n,) or masks.device != dc.device:
+            raise ValueError("masks must be [N] on the device of the coefficients")
+        mask = (masks if masks.dtype == torch.bool else masks != 0).contiguous().view(torch.uint8)
+    return _SphericalHarmonicsSplit.apply(degrees_to_use, dirs, dc, coeffs, mask)
+
+
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xys, depths, radii, conics, colors, opacity, img_height, img_width, background, return_alpha, absgrad):
@@ -806,6 +848,31 @@ def rasterize_binned(means2d, conics, colors, opacities, binning: Binning, img_h
             alpha = out[1]
             hits = out[2] if want_hits else None
     return (images[0] if len(images) == 1 else torch.cat(images, dim=-1)), alpha, hits
+
+
+def isect_keys(binning: Binning, depths: torch.Tensor) -> torch.Tensor:
+    """gsplat's sorted ``isect_ids`` of a binning (b200gs_isect_keys): int64 [binning.total], (tile << 32) | float_bits(depth)
+    in list order, for every tile of binning.tile_ranges.  Reads binning.total, i.e. waits for the counts of a lazy binning."""
+    depths = _f32c(depths, "depths")
+    n_tiles = binning.tile_ranges.shape[0]
+    total = int(binning.total)
+    keys = torch.empty(total, dtype=torch.int64, device=depths.device)
+    with _stage("isect_keys"):
+        check(lib().b200gs_isect_keys(int(n_tiles), ptr(binning.tile_ranges), ptr(binning.sorted_ids), total, ptr(depths), ptr(keys), _stream()),
+              "b200gs_isect_keys")
+    return keys
+
+
+def isect_offsets(keys: torch.Tensor, n_tiles: int) -> torch.Tensor:
+    """gsplat's ``isect_offset_encode`` for one camera (b200gs_isect_offsets): int32 [n_tiles], offsets[t] = index of the first
+    of the sorted keys whose tile is >= t."""
+    if keys.dtype != torch.int64 or keys.dim() != 1 or not keys.is_cuda:
+        raise ValueError("isect_ids must be a 1-D int64 CUDA tensor")
+    keys = keys.contiguous()
+    offsets = torch.empty(int(n_tiles), dtype=torch.int32, device=keys.device)
+    with _stage("isect_offsets"):
+        check(lib().b200gs_isect_offsets(keys.shape[0], ptr(keys), int(n_tiles), ptr(offsets), _stream()), "b200gs_isect_offsets")
+    return offsets
 
 
 def knn_mean_dist2(points: torch.Tensor) -> torch.Tensor:

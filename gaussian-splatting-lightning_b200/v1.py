@@ -35,6 +35,25 @@ def build_rotation(q: torch.Tensor) -> torch.Tensor:
     return R.reshape(-1, 3, 3)
 
 
+def camera_views(viewmats: torch.Tensor, Ks: torch.Tensor, width: int, height: int):
+    """Host-side gsplat-mode views of C cameras: viewmats [C,4,4] world-to-camera, Ks [C,3,3].  Both are read back in one copy
+    (25 floats per camera)."""
+    c = viewmats.shape[0]
+    host = torch.cat((viewmats.detach().reshape(c, 16).float(), Ks.detach().reshape(c, 9).float()), dim=1).cpu()
+    return [ops.make_view(MODE_GSPLAT, width, height, fx=float(h[16]), fy=float(h[20]), cx=float(h[18]), cy=float(h[21]),
+                          viewmatrix=h[:16].reshape(4, 4).T.contiguous()) for h in host]
+
+
+def tiles_per_gauss(means2d: torch.Tensor, radii: torch.Tensor, tile_width: int, tile_height: int, tile_size: int = TILE) -> torch.Tensor:
+    """gsplat's tiles_per_gauss [1,N] int32: the tiles of each Gaussian's bounding rect (gaussian_projection.py:118-125)."""
+    radii, means2d = radii.reshape(-1), means2d.reshape(-1, 2).detach()
+    r = radii.to(means2d.dtype).unsqueeze(-1)
+    grid = torch.tensor([tile_width, tile_height], device=means2d.device, dtype=torch.int32)
+    rmin = torch.minimum(((means2d - r) / tile_size).to(torch.int32).clamp_min(0), grid)
+    rmax = torch.minimum((((means2d + r) / tile_size).to(torch.int32) + 1).clamp_min(0), grid)
+    return torch.where(radii > 0, (rmax - rmin).prod(dim=-1), torch.zeros_like(radii)).unsqueeze(0)
+
+
 class B200GSplatV1:
     @classmethod
     def preprocess_camera(cls, viewpoint_camera):
@@ -62,9 +81,7 @@ class B200GSplatV1:
         view = getattr(preprocessed_camera, "view", None)
         if view is None:   # a plain (viewmats, Ks, (w, h)) tuple built by the caller
             viewmats, Ks, (w, h) = preprocessed_camera
-            K = Ks[0].detach().cpu()
-            view = ops.make_view(MODE_GSPLAT, w, h, fx=float(K[0, 0]), fy=float(K[1, 1]), cx=float(K[0, 2]), cy=float(K[1, 2]),
-                                 viewmatrix=viewmats[0].T.contiguous())
+            view = camera_views(viewmats[:1], Ks[:1], w, h)[0]
         return ops._copy_view(view, eps2d=float(eps2d), scale_modifier=float(scale_modifier))
 
     @classmethod
@@ -93,13 +110,7 @@ class B200GSplatV1:
                                         conics.reshape(-1, 3).detach().contiguous(), opacities.reshape(-1).detach().contiguous())
         else:   # no cull arrays: the reference's pair list (every tile of the 3-sigma rect)
             binning = ops.bin_gaussians(MODE_GSPLAT, img_width, img_height, means2d.contiguous(), depths.contiguous(), radii.contiguous())
-        # tiles of the bounding rect per Gaussian (gaussian_projection.py:118-125)
-        r = radii.to(means2d.dtype).unsqueeze(-1)
-        grid = torch.tensor([tw, th], device=means2d.device, dtype=torch.int32)
-        rmin = torch.minimum(((means2d - r) / tile_size).to(torch.int32).clamp_min(0), grid)
-        rmax = torch.minimum((((means2d + r) / tile_size).to(torch.int32) + 1).clamp_min(0), grid)
-        tiles_per_gauss = torch.where(radii > 0, (rmax - rmin).prod(dim=-1), torch.zeros_like(radii)).unsqueeze(0)
-        out = Isects((tiles_per_gauss, None, binning.sorted_ids, binning.tile_ranges[:, 0].reshape(1, th, tw)))
+        out = Isects((tiles_per_gauss(means2d, radii, tw, th, tile_size), None, binning.sorted_ids, binning.tile_ranges[:, 0].reshape(1, th, tw)))
         out.binning = binning
         return out
 
@@ -241,10 +252,10 @@ class B200GSplatV1RendererModule(Renderer):
     def get_rgbs(self, camera, gaussian_model, projections: Tuple, visibility_filter, status: Any, **kwargs) -> torch.Tensor:
         viewdirs = gaussian_model.get_xyz.detach() - camera.camera_center  # (N, 3)
         if getattr(gaussian_model, "is_pre_activated", False) or not self.config.separate_sh:
-            feats = gaussian_model.get_features
-        else:   # dc | rest kept apart by the model (Taming-3DGS style): the SH kernel takes the concatenation
-            feats = torch.cat((gaussian_model.get_shs_dc(), gaussian_model.get_shs_rest()), dim=1)
-        rgbs = ops.spherical_harmonics(gaussian_model.active_sh_degree, viewdirs, feats, visibility_filter)
+            rgbs = ops.spherical_harmonics(gaussian_model.active_sh_degree, viewdirs, gaussian_model.get_features, visibility_filter)
+        else:   # dc | rest kept apart by the model (Taming-3DGS style): read in place; invisible rows are in no tile list
+            rgbs = ops.spherical_harmonics_decomposed(gaussian_model.active_sh_degree, viewdirs, gaussian_model.get_shs_dc(),
+                                                      gaussian_model.get_shs_rest(), visibility_filter)
         return torch.clamp(rgbs + 0.5, min=0.0)
 
     def forward(self, viewpoint_camera, pc, bg_color: torch.Tensor, scaling_modifier=1.0, render_types: list = None, **kwargs):

@@ -10,6 +10,8 @@
  *   gsplat.v0_interfaces.project_gaussians(...) -> 7-tuple     internal/renderers/gsplat_renderer.py:64-79
  *   gsplat.sh.spherical_harmonics(deg, dirs, coeffs)           internal/renderers/gsplat_renderer.py:105
  *   gsplat.rasterize.rasterize_gaussians(...) -> [H,W,D](,alpha)  internal/renderers/gsplat_renderer.py:86-99
+ *   gsplat.cuda._wrapper / gsplat.sh_decomposed / gsplat.cuda.isect_tiles_tile_based_culling / rasterize_to_pixels
+ *                                                              internal/renderers/gsplat_v1_renderer.py:8-20
  *
  * Conventions
  *   - every pointer is a DEVICE pointer unless named host_*; all floating point is fp32, contiguous.
@@ -145,6 +147,19 @@ B200GS_API int b200gs_sh_fwd(int32_t degree, int32_t sh_stride, int64_t n, const
 B200GS_API int b200gs_sh_bwd(int32_t degree, int32_t sh_stride, int64_t n, const float* dirs, const float* coeffs, const float* v_rgb,
                   float* v_coeffs, float* v_dirs, void* stream);
 
+/* ---- split, masked SH (spherical_harmonics_decomposed of yzslab's gsplat fork) ------------------------------------------
+ * Call sites: gsplat_v1_renderer.py:124 (separate_sh), gsplat_appearance_embedding_renderer.py:193,208, glossy_renderer.py:21,
+ * gsplat_distributed_renderer.py:419.  The coefficients are dc[n,1,3] | rest[n,k_rest,3] read in place (no concatenation);
+ * sh_stride = 1 + k_rest >= (degree+1)^2, rest may be NULL when k_rest = 0.  mask[n] (uint8, nullable): a row with mask[i] == 0
+ * reads no coefficient and gets rgb = 0 and zero v_dc / v_rest / v_dirs.  The same kernels as b200gs_sh_fwd / _bwd with another
+ * coefficient loader: unmasked rows are bit-identical to those on the concatenated tensor.
+ * bwd: v_dc[n,1,3] and v_rest[n,k_rest,3] fully written; v_dirs[n,3] nullable.
+ * Algorithmic bytes per unmasked row at degree 3: fwd 12 + 192 in, 12 out; bwd 24 + 192 in (v_dirs), 192 out (+12). */
+B200GS_API int b200gs_sh_split_fwd(int32_t degree, int32_t k_rest, int64_t n, const float* dirs, const float* dc, const float* rest,
+                                   const uint8_t* mask, float* rgb, void* stream);
+B200GS_API int b200gs_sh_split_bwd(int32_t degree, int32_t k_rest, int64_t n, const float* dirs, const float* dc, const float* rest,
+                                   const uint8_t* mask, const float* v_rgb, float* v_dc, float* v_rest, float* v_dirs, void* stream);
+
 /* ---- K2-K5: tile binning ------------------------------------------------------------------------------------------
  * replaces dgr InclusiveSum + duplicateWithKeys + SortPairs + identifyTileRanges / gsplat isect_tiles + isect_offset_encode.
  * Result order is exactly that of a stable sort of (tile_id << 32 | float_bits(depth)) keys emitted Gaussian-major:
@@ -187,6 +202,22 @@ B200GS_API int b200gs_bin_count(int32_t mode, int32_t width, int32_t height, int
 B200GS_API int b200gs_bin_sort(int32_t mode, int32_t width, int32_t height, int64_t n, int32_t cull, int64_t max_coarse, int64_t max_pairs,
                     int64_t* d_counts, const void* workspace_a, void* workspace_b, size_t workspace_b_bytes, int32_t* sorted_ids,
                     int32_t* tile_ranges, int64_t* host_counts, int32_t sync_host, void* stream);
+
+/* ---- gsplat intersection keys and tile offsets of one camera (C = 1) ---------------------------------------------------
+ * The gsplat-v1 contract isect_tiles -> isect_offset_encode -> rasterize_to_pixels (gsplat_v1_renderer.py:446,458,500-520,588).
+ * b200gs_isect_keys: gsplat's isect_ids of a binning, one per listed pair and in list order:
+ *     keys[i] = (int64(tile) << 32) | float_bits(depth[sorted_ids[i]])      (camera bits 0)
+ *     tile_ranges[n_tiles,2] / sorted_ids are b200gs_bin_sort's outputs with n_pairs = counts[2]; no range may end past n_pairs.
+ *     The binning order is a stable sort of these keys, so they are non-decreasing and, without culling, equal to gsplat's
+ *     sorted keys element for element.  A separate pass: the binning never builds them.
+ *     Algorithmic bytes: 4 B id + 4 B depth gather (L2) in, 8 B key out per pair; 8 B range per tile.
+ * b200gs_isect_offsets: gsplat's isect_offset_encode for C = 1: offsets[t] = index of the first of the n_pairs sorted keys whose
+ *     tile (key >> 32) is >= t, for t < n_tiles (an empty tile gets the next non-empty start, tiles past the last key n_pairs;
+ *     all 0 when n_pairs = 0).  Computed from the keys alone, by a binary search per tile: O(n_tiles log n_pairs) reads.
+ *     n_pairs < 2^31. */
+B200GS_API int b200gs_isect_keys(int32_t n_tiles, const int32_t* tile_ranges, const int32_t* sorted_ids, int64_t n_pairs, const float* depth,
+                                 int64_t* keys, void* stream);
+B200GS_API int b200gs_isect_offsets(int64_t n_pairs, const int64_t* keys, int32_t n_tiles, int32_t* offsets, void* stream);
 
 /* b200gs_publish_i64: deliver n device int64 counters to host memory in stream order, the way the binning phases do
  *     (kernel with system-scope stores for pinned/mapped memory, cudaMemcpyAsync for pageable): for callers that run their
