@@ -44,6 +44,11 @@ _SIGNATURES = {
     "b200gs_densify_stats": (c_int32, [c_int64, _P, _P, _P, c_int32, c_float, c_float, _P, _P, _P, _P]),
     "b200gs_mcmc_relocation": (c_int32, [c_int64, _P, _P, _P, _P, c_int32, _P, _P, _P]),
     "b200gs_mcmc_position_noise": (c_int32, [c_int64, _P, _P, _P, _P, c_float, c_uint64, c_uint64, _P]),
+    "b200gs_bilagrid_slice_fwd": (c_int32, [c_int32] * 4 + [_P] + [c_int32] * 3 + [_P, _P] + [c_int64] * 4 + [_P, c_int32, _P, _P]),
+    "b200gs_bilagrid_slice_bwd": (c_int32, [c_int32] * 4 + [_P] + [c_int32] * 3 + [_P, _P] + [c_int64] * 4 + [_P, c_int32] + [_P] * 3 + [_P]),
+    "b200gs_bilagrid_tv_blocks": (c_int64, [c_int32] * 5),
+    "b200gs_bilagrid_tv_fwd": (c_int32, [c_int32] * 5 + [_P, _P, _P]),
+    "b200gs_bilagrid_tv_bwd": (c_int32, [c_int32] * 5 + [_P, _P, _P, _P]),
     "b200gs_knn_workspace_bytes": (c_size_t, [c_int64]),
     "b200gs_knn_mean_dist2": (c_int32, [c_int64, _P, _P, _P, c_size_t, _P]),
     "b200gs_sh_fwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P]),

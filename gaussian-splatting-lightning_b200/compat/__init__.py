@@ -63,3 +63,9 @@ def install(force: bool = False):
     reloc = types.ModuleType("gsplat.relocation")
     reloc.compute_relocation = mcmc.compute_relocation
     put("gsplat.relocation", reloc)
+    # fused_bilagrid (internal/output_processors/bilagrid.py:40, BilagridProcessor with fused: true, the default)
+    from .. import bilagrid
+    fb = types.ModuleType("fused_bilagrid")
+    for nm in ("BilateralGrid", "slice", "total_variation_loss"):
+        setattr(fb, nm, getattr(bilagrid, nm))
+    put("fused_bilagrid", fb)

@@ -41,7 +41,7 @@ using namespace b200gs;
 extern "C" {
 
 const char* b200gs_last_error(void) { return g_error; }
-int b200gs_version(void) { return 225; }
+int b200gs_version(void) { return 226; }
 int64_t b200gs_launch_count(void) { return (int64_t)g_launches.load(std::memory_order_relaxed); }
 
 int b200gs_project_fwd(const B200gsView* view, int64_t n, const float* means, const float* scales, const float* quats,
@@ -250,6 +250,69 @@ int b200gs_mcmc_position_noise(int64_t n, float* means, const float* log_scales,
     B200GS_CHECK_ARG(n == 0 || (means && log_scales && raw_quats && opacity_logits), "NULL pointer");
     B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(raw_quats) & 15u) == 0, "raw_quats must be 16-byte aligned");
     return launch_mcmc_position_noise(n, means, log_scales, raw_quats, opacity_logits, scale, seed, offset, (cudaStream_t)stream);
+}
+
+// shared by the slice entry points; returns the error code, or 0 when the arguments are valid
+static int check_bilagrid_slice(const char* fn, int32_t n_grids, int32_t grid_l, int32_t grid_h, int32_t grid_w, const float* grids,
+                                int32_t batch, int32_t height, int32_t width, const float* xy, const float* rgb, int64_t sb, int64_t sy,
+                                int64_t sx, int64_t sc, const int64_t* grid_idx, int32_t n_idx, const void* out) {
+    auto fail = [&](const char* msg) { set_error("%s: %s", fn, msg); return B200GS_EINVAL; };
+    if (n_grids < 1 || grid_l < 1 || grid_h < 1 || grid_w < 1) return fail("grid sizes must be >= 1");
+    if (int64_t(12) * grid_l * grid_h * grid_w > INT32_MAX) return fail("grid too large");
+    if (batch < 0 || height < 0 || width < 0) return fail("negative image size");
+    if (sb < 0 || sy < 0 || sx < 0 || sc < 0) return fail("negative stride");
+    if (n_idx != 1 && n_idx != batch) return fail("n_idx must be 1 or batch");
+    if (int64_t(batch) * height * width > 0 && !(grids && xy && rgb && grid_idx && out)) return fail("NULL pointer");
+    return 0;
+}
+
+int b200gs_bilagrid_slice_fwd(int32_t n_grids, int32_t grid_l, int32_t grid_h, int32_t grid_w, const float* grids, int32_t batch,
+                              int32_t height, int32_t width, const float* xy, const float* rgb, int64_t sb, int64_t sy, int64_t sx,
+                              int64_t sc, const int64_t* grid_idx, int32_t n_idx, float* out, void* stream) {
+    if (int rc = check_bilagrid_slice(__func__, n_grids, grid_l, grid_h, grid_w, grids, batch, height, width, xy, rgb, sb, sy, sx, sc,
+                                      grid_idx, n_idx, out))
+        return rc;
+    return launch_bilagrid_slice_fwd(n_grids, grid_l, grid_h, grid_w, grids, batch, height, width, xy, rgb, sb, sy, sx, sc, grid_idx,
+                                     n_idx, out, (cudaStream_t)stream);
+}
+
+int b200gs_bilagrid_slice_bwd(int32_t n_grids, int32_t grid_l, int32_t grid_h, int32_t grid_w, const float* grids, int32_t batch,
+                              int32_t height, int32_t width, const float* xy, const float* rgb, int64_t sb, int64_t sy, int64_t sx,
+                              int64_t sc, const int64_t* grid_idx, int32_t n_idx, const float* v_out, float* v_rgb, float* v_grids,
+                              void* stream) {
+    if (int rc = check_bilagrid_slice(__func__, n_grids, grid_l, grid_h, grid_w, grids, batch, height, width, xy, rgb, sb, sy, sx, sc,
+                                      grid_idx, n_idx, v_out))
+        return rc;
+    return launch_bilagrid_slice_bwd(n_grids, grid_l, grid_h, grid_w, grids, batch, height, width, xy, rgb, sb, sy, sx, sc, grid_idx,
+                                     n_idx, v_out, v_rgb, v_grids, (cudaStream_t)stream);
+}
+
+int64_t b200gs_bilagrid_tv_blocks(int32_t n, int32_t channels, int32_t grid_l, int32_t grid_h, int32_t grid_w) {
+    if (n < 0 || channels < 0 || grid_l < 0 || grid_h < 0 || grid_w < 0) return 0;
+    return bilagrid_tv_blocks(n, channels, grid_l, grid_h, grid_w);
+}
+
+static int check_bilagrid_tv(const char* fn, int32_t n, int32_t channels, int32_t grid_l, int32_t grid_h, int32_t grid_w,
+                             const float* grids, const void* out) {
+    auto fail = [&](const char* msg) { set_error("%s: %s", fn, msg); return B200GS_EINVAL; };
+    if (n < 0 || channels < 0 || grid_l < 0 || grid_h < 0 || grid_w < 0) return fail("negative size");
+    const int64_t total = int64_t(n) * channels * grid_l * grid_h * grid_w;
+    if (total / 256 >= INT32_MAX) return fail("grids too large");
+    if (total > 0 && !(grids && out)) return fail("NULL pointer");
+    return 0;
+}
+
+int b200gs_bilagrid_tv_fwd(int32_t n, int32_t channels, int32_t grid_l, int32_t grid_h, int32_t grid_w, const float* grids,
+                           float* partials, void* stream) {
+    if (int rc = check_bilagrid_tv(__func__, n, channels, grid_l, grid_h, grid_w, grids, partials)) return rc;
+    return launch_bilagrid_tv_fwd(n, channels, grid_l, grid_h, grid_w, grids, partials, (cudaStream_t)stream);
+}
+
+int b200gs_bilagrid_tv_bwd(int32_t n, int32_t channels, int32_t grid_l, int32_t grid_h, int32_t grid_w, const float* grids,
+                           const float* v_tv, float* v_grids, void* stream) {
+    if (int rc = check_bilagrid_tv(__func__, n, channels, grid_l, grid_h, grid_w, grids, v_grids)) return rc;
+    B200GS_CHECK_ARG(int64_t(n) * channels * grid_l * grid_h * grid_w == 0 || v_tv, "NULL pointer");
+    return launch_bilagrid_tv_bwd(n, channels, grid_l, grid_h, grid_w, grids, v_tv, v_grids, (cudaStream_t)stream);
 }
 
 size_t b200gs_knn_workspace_bytes(int64_t n) { return n < 0 ? 0 : knn_workspace_bytes(n); }

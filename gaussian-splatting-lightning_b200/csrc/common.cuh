@@ -136,6 +136,19 @@ int launch_mcmc_relocation(int64_t n, const float* opacities, const float* scale
 int launch_mcmc_position_noise(int64_t n, float* means, const float* log_scales, const float* raw_quats, const float* opacity_logits,
                                float scale, uint64_t seed, uint64_t offset, cudaStream_t s);
 
+// bilateral grid (bilagrid.cu): grids [n_grids,12,L,gh,gw]; xy [batch,height,width,2]; rgb / out / v_out / v_rgb share the element
+// strides (sb, sy, sx, sc); grid_idx int64 [n_idx], n_idx == 1 (broadcast) or batch
+int launch_bilagrid_slice_fwd(int n_grids, int L, int gh, int gw, const float* grids, int batch, int height, int width, const float* xy,
+                              const float* rgb, int64_t sb, int64_t sy, int64_t sx, int64_t sc, const int64_t* grid_idx, int n_idx,
+                              float* out, cudaStream_t s);
+int launch_bilagrid_slice_bwd(int n_grids, int L, int gh, int gw, const float* grids, int batch, int height, int width, const float* xy,
+                              const float* rgb, int64_t sb, int64_t sy, int64_t sx, int64_t sc, const int64_t* grid_idx, int n_idx,
+                              const float* v_out, float* v_rgb, float* v_grids, cudaStream_t s);
+int64_t bilagrid_tv_blocks(int n, int channels, int L, int gh, int gw);
+int launch_bilagrid_tv_fwd(int n, int channels, int L, int gh, int gw, const float* grids, float* partials, cudaStream_t s);
+int launch_bilagrid_tv_bwd(int n, int channels, int L, int gh, int gw, const float* grids, const float* v_tv, float* v_grids,
+                           cudaStream_t s);
+
 size_t knn_workspace_bytes(int64_t n);
 int launch_knn_mean_dist2(int64_t n, const float* points, float* out, void* ws, size_t ws_bytes, cudaStream_t s);
 

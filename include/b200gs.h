@@ -134,6 +134,39 @@ B200GS_API int b200gs_mcmc_relocation(int64_t n, const float* opacities, const f
 B200GS_API int b200gs_mcmc_position_noise(int64_t n, float* means, const float* log_scales, const float* raw_quats,
                                           const float* opacity_logits, float scale, uint64_t seed, uint64_t offset, void* stream);
 
+/* ---- Bilateral-grid colour correction (internal/output_processors/bilagrid.py, internal/utils/lib_bilagrid.py) ------------------
+ * b200gs_bilagrid_slice_fwd: lib_bilagrid's slice(...)["rgb"] as BilagridProcessorModule.forward calls it (bilagrid.py:115-124).
+ *     grids float[n_grids,12,L,gh,gw] contiguous, xy float[batch,height,width,2] contiguous, grid_idx int64[n_idx] with n_idx == 1
+ *     (one grid for every row) or n_idx == batch.  rgb and out are addressed as base[b sb + y sy + x sx + c sc] (element strides,
+ *     so the processor's permuted CHW render needs no copy).  Per pixel, with G = grids[grid_idx[b]]:
+ *         gray = 0.299 r + 0.587 g + 0.114 b,  ix = ((2 (x - 0.5) + 1) / 2) (gw - 1),  iy likewise with gh,
+ *         iz = ((2 gray - 1 + 1) / 2) (L - 1),  each clipped to [0, size - 1];
+ *         A[c] = trilinear interpolation of G[c] at (iz, iy, ix) (corners outside the grid contribute nothing),
+ *         out_i = sum_j A[4i + j] rgb_j + A[4i + 3].
+ *     A grid index outside [0, n_grids) reads no grid and sets that row's output to NaN.
+ * b200gs_bilagrid_slice_bwd: v_out (same strides) -> v_rgb (same strides, NULL: not computed) and v_grids (accumulated into, NULL:
+ *     not computed).  v_rgb includes the path through the guidance gray; a clipped coordinate passes no gradient, a coordinate
+ *     exactly on 0 or size - 1 included (grid_sample's border rule).  xy gets no gradient.
+ * b200gs_bilagrid_tv_fwd: lib_bilagrid's total_variation_loss (bilagrid.py:100-104) on grids float[n,channels,L,gh,gw]:
+ *         tv = (1/n) sum_{axis in L,gh,gw} sum (x[.., i+1, ..] - x[.., i, ..])^2 / max(numel per grid of the difference, 1)
+ *     as b200gs_bilagrid_tv_blocks(...) per-CTA partial sums, which the caller adds in a fixed order.
+ * b200gs_bilagrid_tv_bwd: v_grids = v_tv[0] * d tv / d grids (v_tv a device scalar), written densely.
+ * Algorithmic bytes: slice forward 8 (xy) + 12 (rgb) + 12 (out) per pixel + the grid; backward 8 + 12 + 12 (v_out) + 12 (v_rgb) per
+ *     pixel + the grid and its gradient; tv forward 4 per grid element, backward 8. */
+B200GS_API int b200gs_bilagrid_slice_fwd(int32_t n_grids, int32_t grid_l, int32_t grid_h, int32_t grid_w, const float* grids,
+                                         int32_t batch, int32_t height, int32_t width, const float* xy, const float* rgb, int64_t sb,
+                                         int64_t sy, int64_t sx, int64_t sc, const int64_t* grid_idx, int32_t n_idx, float* out,
+                                         void* stream);
+B200GS_API int b200gs_bilagrid_slice_bwd(int32_t n_grids, int32_t grid_l, int32_t grid_h, int32_t grid_w, const float* grids,
+                                         int32_t batch, int32_t height, int32_t width, const float* xy, const float* rgb, int64_t sb,
+                                         int64_t sy, int64_t sx, int64_t sc, const int64_t* grid_idx, int32_t n_idx,
+                                         const float* v_out, float* v_rgb, float* v_grids, void* stream);
+B200GS_API int64_t b200gs_bilagrid_tv_blocks(int32_t n, int32_t channels, int32_t grid_l, int32_t grid_h, int32_t grid_w);
+B200GS_API int b200gs_bilagrid_tv_fwd(int32_t n, int32_t channels, int32_t grid_l, int32_t grid_h, int32_t grid_w, const float* grids,
+                                      float* partials, void* stream);
+B200GS_API int b200gs_bilagrid_tv_bwd(int32_t n, int32_t channels, int32_t grid_l, int32_t grid_h, int32_t grid_w, const float* grids,
+                                      const float* v_tv, float* v_grids, void* stream);
+
 /* b200gs_knn_mean_dist2: simple_knn's distCUDA2 (vanilla_gaussian.py:122-125, the scale initialiser): mean_dist2[i] = mean of the squared
  *     distances from points[i] (float[n,3]) to its 3 nearest neighbours (exact).  Synchronises the stream once (the hash grid is sized
  *     on the host from the bounding box); init-time only. */
