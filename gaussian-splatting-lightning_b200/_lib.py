@@ -26,6 +26,14 @@ class B200gsView(ctypes.Structure):
     ]
 
 
+class B200gsAppearanceMlp(ctypes.Structure):
+    _fields_ = [
+        ("feat_dim", c_int32), ("n_freq", c_int32), ("n_neurons", c_int32), ("n_layers", c_int32), ("n_out", c_int32),
+        ("normalize", c_int32), ("normalize_dirs", c_int32), ("epilogue", c_int32), ("w0_stride", c_int32), ("w0_pe_col", c_int32),
+        ("weights", c_void_p * 4), ("biases", c_void_p * 4),
+    ]
+
+
 class B200gsError(RuntimeError):
     pass
 
@@ -49,6 +57,9 @@ _SIGNATURES = {
     "b200gs_bilagrid_tv_blocks": (c_int64, [c_int32] * 5),
     "b200gs_bilagrid_tv_fwd": (c_int32, [c_int32] * 5 + [_P, _P, _P]),
     "b200gs_bilagrid_tv_bwd": (c_int32, [c_int32] * 5 + [_P, _P, _P, _P]),
+    "b200gs_appearance_mlp_workspace_bytes": (c_size_t, [c_int32] * 5),
+    "b200gs_appearance_mlp_fwd": (c_int32, [POINTER(B200gsAppearanceMlp), c_int64] + [_P] * 9 + [_P]),
+    "b200gs_appearance_mlp_bwd": (c_int32, [POINTER(B200gsAppearanceMlp), c_int64] + [_P] * 12 + [_P, c_size_t, _P] + [_P]),
     "b200gs_knn_workspace_bytes": (c_size_t, [c_int64]),
     "b200gs_knn_mean_dist2": (c_int32, [c_int64, _P, _P, _P, c_size_t, _P]),
     "b200gs_sh_fwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P]),

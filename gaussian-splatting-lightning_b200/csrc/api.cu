@@ -41,7 +41,7 @@ using namespace b200gs;
 extern "C" {
 
 const char* b200gs_last_error(void) { return g_error; }
-int b200gs_version(void) { return 226; }
+int b200gs_version(void) { return 227; }
 int64_t b200gs_launch_count(void) { return (int64_t)g_launches.load(std::memory_order_relaxed); }
 
 int b200gs_project_fwd(const B200gsView* view, int64_t n, const float* means, const float* scales, const float* quats,
@@ -313,6 +313,68 @@ int b200gs_bilagrid_tv_bwd(int32_t n, int32_t channels, int32_t grid_l, int32_t 
     if (int rc = check_bilagrid_tv(__func__, n, channels, grid_l, grid_h, grid_w, grids, v_grids)) return rc;
     B200GS_CHECK_ARG(int64_t(n) * channels * grid_l * grid_h * grid_w == 0 || v_tv, "NULL pointer");
     return launch_bilagrid_tv_bwd(n, channels, grid_l, grid_h, grid_w, grids, v_tv, v_grids, (cudaStream_t)stream);
+}
+
+static bool appearance_shape_ok(int32_t feat_dim, int32_t n_freq, int32_t n_neurons, int32_t n_layers, int32_t n_out) {
+    return feat_dim >= 8 && feat_dim % 8 == 0 && feat_dim <= 1024 && n_freq <= 16 && (n_neurons == 64 || n_neurons == 128) && n_layers >= 2 &&
+           n_layers <= B200GS_APPEARANCE_MAX_LAYERS && (n_out == 3 || n_out == 4) &&
+           appearance_mlp_fits(feat_dim, n_freq, n_neurons, n_layers, n_out);
+}
+
+size_t b200gs_appearance_mlp_workspace_bytes(int32_t feat_dim, int32_t n_freq, int32_t n_neurons, int32_t n_layers, int32_t n_out) {
+    if (!appearance_shape_ok(feat_dim, n_freq, n_neurons, n_layers, n_out)) return 0;
+    return appearance_mlp_workspace_bytes(feat_dim, n_freq, n_neurons, n_layers, n_out);
+}
+
+static int check_appearance(const char* fn, const B200gsAppearanceMlp* m, int64_t n, const float* features, const float* base_rgb,
+                            const float* dirs, const float* raw_opacity) {
+    auto fail = [&](const char* msg) { set_error("%s: %s", fn, msg); return B200GS_EINVAL; };
+    if (m == nullptr) return fail("mlp is NULL");
+    if (m->feat_dim < 8 || m->feat_dim % 8 != 0) return fail("feat_dim must be a positive multiple of 8");
+    if (m->n_neurons != 64 && m->n_neurons != 128) return fail("n_neurons must be 64 or 128");
+    if (m->n_layers < 2 || m->n_layers > B200GS_APPEARANCE_MAX_LAYERS) return fail("n_layers must be 2..4");
+    if (m->n_out != 3 && m->n_out != 4) return fail("n_out must be 3 or 4");
+    if (!appearance_shape_ok(m->feat_dim, m->n_freq, m->n_neurons, m->n_layers, m->n_out)) return fail("network does not fit shared memory");
+    const int pe = m->n_freq < 0 ? 0 : 3 * (2 * m->n_freq + 1);
+    if (m->w0_stride < m->feat_dim + pe || m->w0_pe_col < m->feat_dim || m->w0_pe_col + pe > m->w0_stride) return fail("bad w0_stride / w0_pe_col");
+    if (n < 0 || n > INT32_MAX) return fail("n out of range");
+    for (int l = 0; l < m->n_layers; ++l)
+        if (!m->weights[l] || !m->biases[l]) return fail("NULL weight or bias pointer");
+    if (n > 0) {
+        if (!features) return fail("NULL features");
+        if (m->n_freq >= 0 && !dirs) return fail("NULL dirs with a view direction");
+        if (m->epilogue && !base_rgb) return fail("NULL base_rgb");
+        if (m->epilogue && m->n_out == 4 && !raw_opacity) return fail("NULL raw_opacity");
+    }
+    return B200GS_OK;
+}
+
+int b200gs_appearance_mlp_fwd(const B200gsAppearanceMlp* mlp, int64_t n, const float* features, const uint8_t* mask, const float* base_rgb,
+                              const float* dirs, const float* cam, const float* raw_opacity, float* out, float* opacity_offsets,
+                              float* opacities, void* stream) {
+    if (int rc = check_appearance(__func__, mlp, n, features, base_rgb, dirs, raw_opacity)) return rc;
+    B200GS_CHECK_ARG(n == 0 || out, "NULL out");
+    B200GS_CHECK_ARG(n == 0 || !(mlp->epilogue && mlp->n_out == 4) || (opacity_offsets && opacities), "NULL opacity output");
+    return launch_appearance_mlp_fwd(*mlp, n, features, mask, base_rgb, dirs, cam, raw_opacity, out, opacity_offsets, opacities,
+                                     (cudaStream_t)stream);
+}
+
+int b200gs_appearance_mlp_bwd(const B200gsAppearanceMlp* mlp, int64_t n, const float* features, const uint8_t* mask, const float* base_rgb,
+                              const float* dirs, const float* cam, const float* raw_opacity, const float* v_out, const float* v_opacities,
+                              const float* v_opacity_offsets, float* v_base_rgb, float* v_features, float* v_raw_opacity, void* workspace,
+                              size_t workspace_bytes, float* v_params, void* stream) {
+    if (int rc = check_appearance(__func__, mlp, n, features, base_rgb, dirs, raw_opacity)) return rc;
+    B200GS_CHECK_ARG(v_params, "NULL v_params");
+    B200GS_CHECK_ARG(n == 0 || (v_out && workspace), "NULL v_out or workspace");
+    B200GS_CHECK_ARG(n == 0 || !mlp->epilogue || v_base_rgb, "NULL v_base_rgb");
+    B200GS_CHECK_ARG(n == 0 || !(mlp->epilogue && mlp->n_out == 4) || v_raw_opacity, "NULL v_raw_opacity");
+    B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(v_features) & 15u) == 0, "v_features must be 16-byte aligned");
+    if (n > 0 && workspace_bytes < appearance_mlp_workspace_bytes(mlp->feat_dim, mlp->n_freq, mlp->n_neurons, mlp->n_layers, mlp->n_out)) {
+        set_error("%s: workspace too small", __func__);
+        return B200GS_ENOSPACE;
+    }
+    return launch_appearance_mlp_bwd(*mlp, n, features, mask, base_rgb, dirs, cam, raw_opacity, v_out, v_opacities, v_opacity_offsets,
+                                     v_base_rgb, v_features, v_raw_opacity, static_cast<float*>(workspace), v_params, (cudaStream_t)stream);
 }
 
 size_t b200gs_knn_workspace_bytes(int64_t n) { return n < 0 ? 0 : knn_workspace_bytes(n); }

@@ -149,6 +149,17 @@ int launch_bilagrid_tv_fwd(int n, int channels, int L, int gh, int gw, const flo
 int launch_bilagrid_tv_bwd(int n, int channels, int L, int gh, int gw, const float* grids, const float* v_tv, float* v_grids,
                            cudaStream_t s);
 
+// appearance MLP (appearance.cu); the shape arguments are those of B200gsAppearanceMlp, validated by the caller
+bool appearance_mlp_fits(int feat_dim, int n_freq, int n_neurons, int n_layers, int n_out);
+size_t appearance_mlp_workspace_bytes(int feat_dim, int n_freq, int n_neurons, int n_layers, int n_out);
+int launch_appearance_mlp_fwd(const B200gsAppearanceMlp& m, int64_t n, const float* features, const uint8_t* mask, const float* base_rgb,
+                              const float* dirs, const float* cam, const float* raw_opacity, float* out, float* opacity_offsets,
+                              float* opacities, cudaStream_t s);
+int launch_appearance_mlp_bwd(const B200gsAppearanceMlp& m, int64_t n, const float* features, const uint8_t* mask, const float* base_rgb,
+                              const float* dirs, const float* cam, const float* raw_opacity, const float* v_out, const float* v_opacities,
+                              const float* v_opacity_offsets, float* v_base_rgb, float* v_features, float* v_raw_opacity, float* workspace,
+                              float* v_params, cudaStream_t s);
+
 size_t knn_workspace_bytes(int64_t n);
 int launch_knn_mean_dist2(int64_t n, const float* points, float* out, void* ws, size_t ws_bytes, cudaStream_t s);
 

@@ -929,3 +929,114 @@ def l1_ssim_loss(image: torch.Tensor, target: torch.Tensor, lambda_dssim: float 
     """(1 - lambda) * L1 + lambda * (1 - SSIM) of `VanillaMetricsImpl._get_basic_metrics` (vanilla_metrics.py:57-74) in two
     kernels; returns (loss, stats) with stats = [mean |image - target|, mean SSIM].  image/target: [C,H,W] fp32 CUDA."""
     return _L1SSIMLoss.apply(image, target, float(lambda_dssim))
+
+
+# ---- appearance-embedding colour pass (csrc/appearance.cu) ---------------------------------------------------------------------
+APPEARANCE_FWD_LAUNCHES = 1     # library launches of one appearance_mlp / appearance_colors forward
+APPEARANCE_BWD_LAUNCHES = 2     # and of its backward: the MLP backward and the reduction of the per-CTA weight-gradient blocks
+
+
+def appearance_supported(feat_dim: int, n_freq: int, n_neurons: int, n_layers: int, n_out: int) -> bool:
+    """Whether the appearance kernels take this network (no device needed)."""
+    return int(lib().b200gs_appearance_mlp_workspace_bytes(feat_dim, n_freq, n_neurons, n_layers, n_out)) > 0
+
+
+def _appearance_offsets(feat_dim, n_freq, n_neurons, n_layers, n_out):
+    """[(offset, rows, cols)] of each layer's weight, then [(offset, rows)] of each bias, in b200gs_appearance_mlp_bwd's v_params."""
+    pe = 0 if n_freq < 0 else 3 * (2 * n_freq + 1)
+    k0p = (feat_dim + pe + 7) // 8 * 8
+    shapes = [(n_out if l == n_layers - 1 else n_neurons, k0p if l == 0 else n_neurons) for l in range(n_layers)]
+    o, ws, bs = 0, [], []
+    for r, c in shapes:
+        ws.append((o, r, c))
+        o += r * c
+    for r, _ in shapes:
+        bs.append((o, r))
+        o += r
+    return ws, bs, o
+
+
+class _AppearanceMlp(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, cfg, features, mask, base_rgb, dirs, cam, raw_opacity, embed_cols, *params):
+        n_freq, normalize, normalize_dirs, epilogue = cfg
+        n, feat_dim = features.shape
+        weights, biases = params[0::2], params[1::2]
+        n_layers, n_neurons, n_out = len(weights), weights[0].shape[0], weights[-1].shape[0]
+        m = _lib.B200gsAppearanceMlp(feat_dim, n_freq, n_neurons, n_layers, n_out, int(normalize), int(normalize_dirs), int(epilogue),
+                                     weights[0].shape[1], feat_dim + embed_cols)
+        for l in range(n_layers):
+            m.weights[l], m.biases[l] = weights[l].data_ptr(), biases[l].data_ptr()
+        dev = features.device
+        with_opacity = epilogue and n_out == 4
+        out = torch.empty(n, 3 if epilogue else n_out, dtype=torch.float32, device=dev)
+        offsets = torch.empty(n, dtype=torch.float32, device=dev) if with_opacity else None
+        opacities = torch.empty(n, dtype=torch.float32, device=dev) if with_opacity else None
+        check(lib().b200gs_appearance_mlp_fwd(ctypes.byref(m), n, ptr(features), ptr(mask), ptr(base_rgb), ptr(dirs), ptr(cam),
+                                              ptr(raw_opacity), ptr(out), ptr(offsets), ptr(opacities), _stream()), "b200gs_appearance_mlp_fwd")
+        ctx.m, ctx.cfg, ctx.embed_cols = m, cfg, embed_cols
+        ctx.save_for_backward(features, mask, base_rgb, dirs, cam, raw_opacity, *params)
+        if not epilogue:
+            return out
+        return (out, opacities, offsets) if with_opacity else out
+
+    @staticmethod
+    def backward(ctx, v_out, v_opacities=None, v_offsets=None):
+        features, mask, base_rgb, dirs, cam, raw_opacity, *params = ctx.saved_tensors
+        m, (n_freq, _, _, epilogue) = ctx.m, ctx.cfg
+        n, feat_dim = features.shape
+        with_opacity = epilogue and m.n_out == 4
+        dev, L_ = features.device, lib()
+        ws, bs, total = _appearance_offsets(feat_dim, n_freq, m.n_neurons, m.n_layers, m.n_out)
+        v_out = _f32c(v_out, "grad")
+        v_opacities = _f32c(v_opacities, "grad") if v_opacities is not None else None
+        v_offsets = _f32c(v_offsets, "grad") if v_offsets is not None else None
+        v_base = torch.empty_like(base_rgb) if epilogue else None
+        v_features = torch.empty_like(features) if ctx.needs_input_grad[1] else None
+        v_raw = torch.empty_like(raw_opacity) if with_opacity else None
+        ws_bytes = int(L_.b200gs_appearance_mlp_workspace_bytes(feat_dim, n_freq, m.n_neurons, m.n_layers, m.n_out))
+        workspace = torch.empty(ws_bytes // 4, dtype=torch.float32, device=dev)
+        v_params = torch.empty(total, dtype=torch.float32, device=dev)
+        check(L_.b200gs_appearance_mlp_bwd(ctypes.byref(m), n, ptr(features), ptr(mask), ptr(base_rgb), ptr(dirs), ptr(cam), ptr(raw_opacity),
+                                           ptr(v_out), ptr(v_opacities), ptr(v_offsets), ptr(v_base), ptr(v_features), ptr(v_raw),
+                                           ptr(workspace), ws_bytes, ptr(v_params), _stream()), "b200gs_appearance_mlp_bwd")
+        grads = []
+        for l, ((wo, r, c), (bo, _)) in enumerate(zip(ws, bs)):
+            v_w = v_params[wo:wo + r * c].view(r, c)
+            if l == 0:      # the kernel's columns are features | view direction; the embedding's columns get theirs through biases[0]
+                pe = 0 if n_freq < 0 else 3 * (2 * n_freq + 1)
+                full = torch.zeros_like(params[0])
+                full[:, :feat_dim] = v_w[:, :feat_dim]
+                if pe:
+                    full[:, feat_dim + ctx.embed_cols:] = v_w[:, feat_dim:feat_dim + pe]
+                v_w = full
+            grads += [v_w, v_params[bo:bo + r]]
+        return (None, v_features, None, v_base, None, None, v_raw, None, *grads)
+
+
+def appearance_mlp(features, embedding, weights, biases, *, dirs=None, cam=None, n_freq=-1, normalize=False, normalize_dirs=False,
+                   mask=None, base_rgb=None, raw_opacity=None):
+    """The appearance network of the reference's GSplatAppearanceEmbeddingRenderer on one kernel each way.
+
+    ``features`` [N, F]; ``embedding`` [E], the image's (already normalised, when the model normalises) embedding row; ``weights`` /
+    ``biases`` the Linear layers, ``weights[0]`` [H, F + E (+ PE)].  The embedding is the same for every row, so it is folded into the
+    first bias here (``b0 + W0[:, F:F+E] @ embedding``, torch, differentiable) and the kernel never sees it.  ``dirs`` [N, 3] minus
+    ``cam`` [3] (optional) is the view direction when ``n_freq >= 0``.  ``mask`` bool [N] (None: every row) selects the rows.
+
+    Without ``base_rgb``: returns the sigmoid outputs [N, 3 | 4] (zeros in unmasked rows).  With ``base_rgb`` [N, 3] (SH colours before
+    the + 0.5): returns ``rgbs`` [N, 3] = clamp(base + 0.5 + 2 s - 1, 0, 1), zeros in unmasked rows, and, for a 4-output network,
+    ``(rgbs, opacities, opacity_offsets)`` with ``opacities = min(raw_opacity + offset, 1)``.  Gradients reach features, base_rgb,
+    raw_opacity, the embedding and every weight and bias; none reaches dirs or cam."""
+    feat_dim, e = features.shape[1], embedding.shape[0]
+    w0 = weights[0]
+    b0 = torch.addmv(biases[0], w0[:, feat_dim:feat_dim + e], embedding)
+    params = []
+    for l, (w, b) in enumerate(zip(weights, biases)):
+        params += [_f32c(w, "weight"), _f32c(b0 if l == 0 else b, "bias")]
+    if mask is not None:
+        mask = (mask if mask.dtype == torch.bool else mask != 0).contiguous().view(torch.uint8)
+    epilogue = base_rgb is not None
+    cfg = (int(n_freq), bool(normalize), bool(normalize_dirs), epilogue)
+    return _AppearanceMlp.apply(cfg, _f32c(features, "features"), mask, _f32c(base_rgb, "base_rgb") if epilogue else None,
+                                _f32c(dirs, "dirs") if n_freq >= 0 else None, _f32c(cam.reshape(-1), "cam") if cam is not None and n_freq >= 0 else None,
+                                _f32c(raw_opacity, "raw_opacity") if raw_opacity is not None else None, e, *params)

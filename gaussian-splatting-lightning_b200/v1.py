@@ -249,14 +249,17 @@ class B200GSplatV1RendererModule(Renderer):
     def get_opacities(self, camera, gaussian_model, projections: Tuple, visibility_filter, status: Any, **kwargs) -> Tuple[torch.Tensor, Any]:
         return gaussian_model.get_opacities().squeeze(-1), status
 
-    def get_rgbs(self, camera, gaussian_model, projections: Tuple, visibility_filter, status: Any, **kwargs) -> torch.Tensor:
+    def sh_colors(self, camera, gaussian_model, visibility_filter) -> torch.Tensor:
+        """SH of the detached view directions, before the + 0.5."""
         viewdirs = gaussian_model.get_xyz.detach() - camera.camera_center  # (N, 3)
         if getattr(gaussian_model, "is_pre_activated", False) or not self.config.separate_sh:
-            rgbs = ops.spherical_harmonics(gaussian_model.active_sh_degree, viewdirs, gaussian_model.get_features, visibility_filter)
-        else:   # dc | rest kept apart by the model (Taming-3DGS style): read in place; invisible rows are in no tile list
-            rgbs = ops.spherical_harmonics_decomposed(gaussian_model.active_sh_degree, viewdirs, gaussian_model.get_shs_dc(),
-                                                      gaussian_model.get_shs_rest(), visibility_filter)
-        return torch.clamp(rgbs + 0.5, min=0.0)
+            return ops.spherical_harmonics(gaussian_model.active_sh_degree, viewdirs, gaussian_model.get_features, visibility_filter)
+        # dc | rest kept apart by the model (Taming-3DGS style): read in place; invisible rows are in no tile list
+        return ops.spherical_harmonics_decomposed(gaussian_model.active_sh_degree, viewdirs, gaussian_model.get_shs_dc(),
+                                                  gaussian_model.get_shs_rest(), visibility_filter)
+
+    def get_rgbs(self, camera, gaussian_model, projections: Tuple, visibility_filter, status: Any, **kwargs) -> torch.Tensor:
+        return torch.clamp(self.sh_colors(camera, gaussian_model, visibility_filter) + 0.5, min=0.0)
 
     def forward(self, viewpoint_camera, pc, bg_color: torch.Tensor, scaling_modifier=1.0, render_types: list = None, **kwargs):
         render_type_bits = self.parse_render_types(render_types)

@@ -167,6 +167,55 @@ B200GS_API int b200gs_bilagrid_tv_fwd(int32_t n, int32_t channels, int32_t grid_
 B200GS_API int b200gs_bilagrid_tv_bwd(int32_t n, int32_t channels, int32_t grid_l, int32_t grid_h, int32_t grid_w, const float* grids,
                                       const float* v_tv, float* v_grids, void* stream);
 
+/* ---- Appearance-embedding colour pass (internal/renderers/gsplat_appearance_embedding_renderer.py) ---------------------------------
+ * The MLP of Model.forward (:77-93) and the colour / opacity epilogue of _get_rgbs_and_opacities (:239-295), on the tensor cores
+ * (mma.sync TF32, each product as three TF32 products of split operands: FP32-level accuracy, FP32 accumulation).
+ * B200gsAppearanceMlp (a HOST struct of sizes, flags and DEVICE pointers) describes the network:
+ *     feat_dim F (a multiple of 8); n_freq: frequencies of PositionalEncoding(3, n_freq) of the view direction, < 0: no view direction;
+ *     n_neurons 64 | 128; n_layers 2..4 linear layers, the output layer included; n_out 3 | 4.
+ *     weights[l] / biases[l], l < n_layers: torch Linear layout [out, in].  weights[0] has w0_stride floats per row; the kernels read
+ *     its columns [0, F) (features) and [w0_pe_col, w0_pe_col + 3 (2 n_freq + 1)) (view direction).  The per-image embedding is the
+ *     same for every row, so the caller folds its columns into biases[0] = b_0 + W_0[:, F:F+E] e.
+ *     normalize: rows of `features` are divided by max(|row|, 1e-12) first.  normalize_dirs: so is the view direction.
+ *     epilogue: 0 = out[n, n_out] holds the sigmoid outputs; 1 = the renderer's colours, see below.
+ * Rows: mask uint8[n] (NULL: every row); a row with mask[i] == 0 is not evaluated.  The view direction of row i is
+ *     dirs[i] - cam (cam float[3] on the device, NULL: zero), both NULL when n_freq < 0.
+ * b200gs_appearance_mlp_fwd, epilogue == 1, with s = the sigmoid outputs of a masked row:
+ *         out[i] = clamp((base_rgb[i] + 0.5) + (2 s[0..2] - 1), 0, 1)                                    out float[n,3]
+ *         n_out == 4: opacity_offsets[i] = s[3], opacities[i] = min(s[3] + raw_opacity[i], 1)
+ *     and out[i] = 0, opacity_offsets[i] = 0, opacities[i] = min(raw_opacity[i], 1) for the other rows: every output is fully written.
+ * b200gs_appearance_mlp_bwd: recomputes the activations.  v_out as out; v_opacities / v_opacity_offsets float[n], nullable.
+ *     Writes v_base_rgb[n,3] and v_raw_opacity[n] (epilogue == 1; the latter when n_out == 4), v_features[n,F] (NULL: not computed;
+ *     through the normalisation when on), each fully written with zeros in the unmasked rows, and v_params, one dense vector
+ *         W_0 [n_neurons, K0p] | W_1 | .. | W_last [n_out, n_neurons] | b_0 | .. | b_last,   K0p = F + 3 (2 n_freq + 1) rounded up to 8,
+ *     W_0's columns being the features, then the view direction, then zeros.  Every persistent CTA sums its rows into its own block
+ *     of `workspace` (b200gs_appearance_mlp_workspace_bytes, 16-byte aligned) and a second kernel adds the blocks in a fixed order: two
+ *     calls on the same inputs give bit-identical v_params.  No gradient reaches dirs or cam (the reference detaches them).
+ * b200gs_appearance_mlp_workspace_bytes: 0 when the shape is not supported (sizes outside the sets above, or a first layer so wide
+ *     that the weights and one 16-row tile of activations exceed 227 KB of shared memory).  A CTA runs 8 warps of 16 rows when
+ *     they fit beside the weights (every 64-neuron network), else 4, 2 or 1.
+ * Launches: forward 1, backward 2 (0 and 1 when n == 0), whatever the mask holds.
+ * Algorithmic bytes per masked row, F = 64: forward 256 (features) + 12 + 12 (+ 12 dirs, + 4 + 8 opacity); backward 256 + 12 + 12
+ *     in, 256 + 12 out.  FLOPs per masked row: 2 MACs x (K0p n_neurons + (n_layers - 2) n_neurons^2 + 8 n_neurons) forward; the
+ *     backward recomputes that and adds twice as much again (gradients to the inputs and to the weights). */
+#define B200GS_APPEARANCE_MAX_LAYERS 4
+typedef struct B200gsAppearanceMlp {
+    int32_t feat_dim, n_freq, n_neurons, n_layers, n_out;
+    int32_t normalize, normalize_dirs, epilogue;
+    int32_t w0_stride, w0_pe_col;
+    const float* weights[B200GS_APPEARANCE_MAX_LAYERS];
+    const float* biases[B200GS_APPEARANCE_MAX_LAYERS];
+} B200gsAppearanceMlp;
+B200GS_API size_t b200gs_appearance_mlp_workspace_bytes(int32_t feat_dim, int32_t n_freq, int32_t n_neurons, int32_t n_layers, int32_t n_out);
+B200GS_API int b200gs_appearance_mlp_fwd(const B200gsAppearanceMlp* mlp, int64_t n, const float* features, const uint8_t* mask,
+                                         const float* base_rgb, const float* dirs, const float* cam, const float* raw_opacity, float* out,
+                                         float* opacity_offsets, float* opacities, void* stream);
+B200GS_API int b200gs_appearance_mlp_bwd(const B200gsAppearanceMlp* mlp, int64_t n, const float* features, const uint8_t* mask,
+                                         const float* base_rgb, const float* dirs, const float* cam, const float* raw_opacity,
+                                         const float* v_out, const float* v_opacities, const float* v_opacity_offsets, float* v_base_rgb,
+                                         float* v_features, float* v_raw_opacity, void* workspace, size_t workspace_bytes, float* v_params,
+                                         void* stream);
+
 /* b200gs_knn_mean_dist2: simple_knn's distCUDA2 (vanilla_gaussian.py:122-125, the scale initialiser): mean_dist2[i] = mean of the squared
  *     distances from points[i] (float[n,3]) to its 3 nearest neighbours (exact).  Synchronises the stream once (the hash grid is sized
  *     on the host from the bounding box); init-time only. */
