@@ -60,6 +60,11 @@ _SIGNATURES = {
     "b200gs_appearance_mlp_workspace_bytes": (c_size_t, [c_int32] * 5),
     "b200gs_appearance_mlp_fwd": (c_int32, [POINTER(B200gsAppearanceMlp), c_int64] + [_P] * 9 + [_P]),
     "b200gs_appearance_mlp_bwd": (c_int32, [POINTER(B200gsAppearanceMlp), c_int64] + [_P] * 12 + [_P, c_size_t, _P] + [_P]),
+    "b200gs_exposure_workspace_bytes": (c_size_t, [c_int32] * 4),
+    "b200gs_exposure_fwd": (c_int32, [c_int32] * 3 + [_P] + [c_int64] * 3 + [c_int32] * 2 + [_P, _P, c_int64, c_int32, _P, c_float, c_float]
+                            + [_P, c_size_t, _P, _P]),
+    "b200gs_exposure_bwd": (c_int32, [c_int32] * 3 + [_P] + [c_int64] * 3 + [c_int32] * 2 + [_P, _P, c_int64, c_int32, _P, c_float, c_float]
+                            + [_P, c_size_t] + [_P] * 4 + [_P]),
     "b200gs_knn_workspace_bytes": (c_size_t, [c_int64]),
     "b200gs_knn_mean_dist2": (c_int32, [c_int64, _P, _P, _P, c_size_t, _P]),
     "b200gs_sh_fwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P]),

@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libb200gs.so")
-SOURCES = ["api.cu", "project.cu", "binning.cu", "blend.cu", "loss.cu", "optim.cu", "knn.cu", "mcmc.cu", "isect.cu", "bilagrid.cu", "appearance.cu"]
+SOURCES = ["api.cu", "project.cu", "binning.cu", "blend.cu", "loss.cu", "optim.cu", "knn.cu", "mcmc.cu", "isect.cu", "bilagrid.cu", "appearance.cu", "exposure.cu"]
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "geometry.cuh"), os.path.join(CSRC, "onesweep.cuh"), os.path.join(os.path.dirname(HERE), "include", "b200gs.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]

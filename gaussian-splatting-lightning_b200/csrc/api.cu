@@ -41,7 +41,7 @@ using namespace b200gs;
 extern "C" {
 
 const char* b200gs_last_error(void) { return g_error; }
-int b200gs_version(void) { return 227; }
+int b200gs_version(void) { return 228; }
 int64_t b200gs_launch_count(void) { return (int64_t)g_launches.load(std::memory_order_relaxed); }
 
 int b200gs_project_fwd(const B200gsView* view, int64_t n, const float* means, const float* scales, const float* quats,
@@ -375,6 +375,62 @@ int b200gs_appearance_mlp_bwd(const B200gsAppearanceMlp* mlp, int64_t n, const f
     }
     return launch_appearance_mlp_bwd(*mlp, n, features, mask, base_rgb, dirs, cam, raw_opacity, v_out, v_opacities, v_opacity_offsets,
                                      v_base_rgb, v_features, v_raw_opacity, static_cast<float*>(workspace), v_params, (cudaStream_t)stream);
+}
+
+static bool exposure_size_ok(int32_t height, int32_t width, int32_t shade_size) {
+    return height >= 1 && width >= 1 && height <= 65535 * 8 && int64_t(height) * width <= INT32_MAX && shade_size >= 0 &&
+           shade_size <= 4096;
+}
+
+size_t b200gs_exposure_workspace_bytes(int32_t height, int32_t width, int32_t shade_size, int32_t backward) {
+    if (!exposure_size_ok(height, width, shade_size)) return 0;
+    return exposure_workspace_bytes(height, width, shade_size, backward != 0);
+}
+
+// shared by the forward and the backward; returns the error code, or 0 when the arguments are valid
+static int check_exposure(const char* fn, int32_t channels, int32_t height, int32_t width, const float* render, int64_t sc, int64_t sy,
+                          int64_t sx, int32_t n_appearances, int32_t n_params, const float* exposure_params, int32_t shade_size,
+                          const float* shade, const void* workspace, size_t workspace_bytes, bool backward, const void* out) {
+    auto fail = [&](const char* msg) { set_error("%s: %s", fn, msg); return B200GS_EINVAL; };
+    if (channels != 3) return fail("channels must be 3");
+    if (height < 1 || width < 1) return fail("image size must be >= 1");
+    if (shade_size < 0) return fail("negative shade_size");
+    if (!exposure_size_ok(height, width, shade_size)) return fail("image or shade map too large");
+    if (sc < 0 || sy < 0 || sx < 0) return fail("negative stride");
+    if (n_appearances < 1) return fail("n_appearances must be >= 1");
+    if (n_params != 4 && n_params != 7) return fail("n_params must be 4 (no bias) or 7 (with bias)");
+    if (!(render && exposure_params && workspace && out) || (shade_size > 0 && !shade)) return fail("NULL pointer");
+    if (workspace_bytes < exposure_workspace_bytes(height, width, shade_size, backward)) {
+        set_error("%s: workspace too small", fn);
+        return B200GS_ENOSPACE;
+    }
+    return 0;
+}
+
+int b200gs_exposure_fwd(int32_t channels, int32_t height, int32_t width, const float* render, int64_t sc, int64_t sy, int64_t sx,
+                        int32_t n_appearances, int32_t n_params, const float* exposure_params, const int64_t* appearance_id,
+                        int64_t host_appearance_id, int32_t shade_size, const float* shade, float max_gray_scale, float max_gamma,
+                        void* workspace, size_t workspace_bytes, float* out, void* stream) {
+    if (int rc = check_exposure(__func__, channels, height, width, render, sc, sy, sx, n_appearances, n_params, exposure_params, shade_size,
+                                shade, workspace, workspace_bytes, false, out))
+        return rc;
+    return launch_exposure_fwd(height, width, render, sc, sy, sx, n_appearances, n_params, exposure_params, appearance_id,
+                               host_appearance_id, shade_size, shade, max_gray_scale, max_gamma, static_cast<float*>(workspace), out,
+                               (cudaStream_t)stream);
+}
+
+int b200gs_exposure_bwd(int32_t channels, int32_t height, int32_t width, const float* render, int64_t sc, int64_t sy, int64_t sx,
+                        int32_t n_appearances, int32_t n_params, const float* exposure_params, const int64_t* appearance_id,
+                        int64_t host_appearance_id, int32_t shade_size, const float* shade, float max_gray_scale, float max_gamma,
+                        void* workspace, size_t workspace_bytes, const float* v_out, float* v_render, float* v_params, float* v_shade,
+                        void* stream) {
+    if (int rc = check_exposure(__func__, channels, height, width, render, sc, sy, sx, n_appearances, n_params, exposure_params, shade_size,
+                                shade, workspace, workspace_bytes, true, v_out))
+        return rc;
+    B200GS_CHECK_ARG(v_render && v_params && (shade_size == 0 || v_shade), "NULL pointer");
+    return launch_exposure_bwd(height, width, render, sc, sy, sx, n_appearances, n_params, exposure_params, appearance_id,
+                               host_appearance_id, shade_size, shade, max_gray_scale, max_gamma, static_cast<float*>(workspace), v_out,
+                               v_render, v_params, v_shade, (cudaStream_t)stream);
 }
 
 size_t b200gs_knn_workspace_bytes(int64_t n) { return n < 0 ? 0 : knn_workspace_bytes(n); }

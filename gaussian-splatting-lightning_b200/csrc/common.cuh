@@ -149,6 +149,17 @@ int launch_bilagrid_tv_fwd(int n, int channels, int L, int gh, int gw, const flo
 int launch_bilagrid_tv_bwd(int n, int channels, int L, int gh, int gw, const float* grids, const float* v_tv, float* v_grids,
                            cudaStream_t s);
 
+// exposure correction (exposure.cu): render / out / v_out / v_render [3,H,W] through the element strides (sc, sy, sx); params
+// [n_app, n_params] (n_params 4 or 7: with bias); the id read from id_dev when not NULL, else id_host; shade [s, s] (s = 0: none)
+size_t exposure_workspace_bytes(int height, int width, int shade_size, bool backward);
+int launch_exposure_fwd(int height, int width, const float* render, int64_t sc, int64_t sy, int64_t sx, int n_app, int n_params,
+                        const float* params, const int64_t* id_dev, int64_t id_host, int s, const float* shade, float max_gray,
+                        float max_gamma, float* ws, float* out, cudaStream_t st);
+int launch_exposure_bwd(int height, int width, const float* render, int64_t sc, int64_t sy, int64_t sx, int n_app, int n_params,
+                        const float* params, const int64_t* id_dev, int64_t id_host, int s, const float* shade, float max_gray,
+                        float max_gamma, float* ws, const float* v_out, float* v_render, float* v_params, float* v_shade,
+                        cudaStream_t st);
+
 // appearance MLP (appearance.cu); the shape arguments are those of B200gsAppearanceMlp, validated by the caller
 bool appearance_mlp_fits(int feat_dim, int n_freq, int n_neurons, int n_layers, int n_out);
 size_t appearance_mlp_workspace_bytes(int feat_dim, int n_freq, int n_neurons, int n_layers, int n_out);

@@ -216,6 +216,38 @@ B200GS_API int b200gs_appearance_mlp_bwd(const B200gsAppearanceMlp* mlp, int64_t
                                          float* v_features, float* v_raw_opacity, void* workspace, size_t workspace_bytes, float* v_params,
                                          void* stream);
 
+/* ---- Learned exposure correction (internal/output_processors/exposure.py, ExposureProcessorModule.forward :112-143) ------------
+ * b200gs_exposure_fwd: one view's colour transform.  render and out are float[3,H,W] addressed as base[c sc + y sy + x sx] (element
+ *     strides, so the permuted [H,W,3] render of the v1 and appearance renderers needs no copy); channels must be 3.
+ *     exposure_params float[n_appearances, n_params] contiguous, n_params 4 (no bias) or 7 (with_bias); the row is the int64 read
+ *     from appearance_id on the device, or host_appearance_id when appearance_id is NULL.  shade float[shade_size, shade_size]
+ *     contiguous (the reference's shade_correction[0]), NULL with shade_size 0 when shade correction is off.  With
+ *     a = sigmoid(exposure_params[id]):
+ *         M = sigmoid(shade) / max(max(sigmoid(shade)), 1e-4),
+ *         m(y, x) = F.interpolate(M, (H, W), mode="bilinear", align_corners=True)   (1 without shade correction),
+ *         x_c = (a_c max_gray_scale) (render_c m) [+ 2 a_{3+c} - 1],   out_c = (clamp(x_c, 0, 1) + 1e-5) ^ (a_last max_gamma).
+ *     An id outside [0, n_appearances) reads no parameter row and makes out NaN.
+ * b200gs_exposure_bwd: v_out (same strides) -> v_render (same strides; the clamp passes the gradient as identity, as the reference's
+ *     straight-through clamp), v_params float[n_appearances, n_params] (written whole: rows other than id are zero) and, with shade
+ *     correction, v_shade float[shade_size, shade_size] (written whole; no gradient through the detached max).  Parameter sums are
+ *     per-CTA partials added in a fixed order and v_shade is gathered per cell in a fixed order: two calls on the same inputs give
+ *     bit-identical gradients.  An out-of-range id makes v_render NaN and v_params, v_shade zero.
+ * b200gs_exposure_workspace_bytes: device scratch of the forward (backward == 0) or the backward (backward != 0) at this image and
+ *     shade size; 0 for sizes the kernels do not take (H or W < 1, H > 524280, H W > 2^31 - 1, shade_size outside 0..4096).
+ * Launches: forward 2 (prologue, pixels), backward 3 (prologue, pixels, reduction).  No host synchronisation.
+ * Algorithmic bytes: forward 12 in + 12 out per pixel; backward 24 in + 12 out per pixel, plus, with shade correction, v_m 4 out and
+ *     4 in per pixel. */
+B200GS_API size_t b200gs_exposure_workspace_bytes(int32_t height, int32_t width, int32_t shade_size, int32_t backward);
+B200GS_API int b200gs_exposure_fwd(int32_t channels, int32_t height, int32_t width, const float* render, int64_t sc, int64_t sy, int64_t sx,
+                                   int32_t n_appearances, int32_t n_params, const float* exposure_params, const int64_t* appearance_id,
+                                   int64_t host_appearance_id, int32_t shade_size, const float* shade, float max_gray_scale,
+                                   float max_gamma, void* workspace, size_t workspace_bytes, float* out, void* stream);
+B200GS_API int b200gs_exposure_bwd(int32_t channels, int32_t height, int32_t width, const float* render, int64_t sc, int64_t sy, int64_t sx,
+                                   int32_t n_appearances, int32_t n_params, const float* exposure_params, const int64_t* appearance_id,
+                                   int64_t host_appearance_id, int32_t shade_size, const float* shade, float max_gray_scale,
+                                   float max_gamma, void* workspace, size_t workspace_bytes, const float* v_out, float* v_render,
+                                   float* v_params, float* v_shade, void* stream);
+
 /* b200gs_knn_mean_dist2: simple_knn's distCUDA2 (vanilla_gaussian.py:122-125, the scale initialiser): mean_dist2[i] = mean of the squared
  *     distances from points[i] (float[n,3]) to its 3 nearest neighbours (exact).  Synchronises the stream once (the hash grid is sized
  *     on the host from the bounding box); init-time only. */
