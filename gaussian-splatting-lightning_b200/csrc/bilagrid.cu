@@ -237,28 +237,20 @@ struct TvWeights { float z, y, x; };    // 1 / (n * max(numel per grid of the di
 
 __global__ void __launch_bounds__(TV_THREADS) tv_fwd_kernel(int64_t total, int L, int gh, int gw, TvWeights w,
                                                             const float* __restrict__ grids, float* __restrict__ partials) {
-    __shared__ float s_red[TV_THREADS / 32];
+    __shared__ float s_red[TV_THREADS / 32][1];
     const int64_t e = int64_t(blockIdx.x) * TV_THREADS + threadIdx.x;
-    float acc = 0.f;
+    float acc[1] = {0.f};
     if (e < total) {
         const int ix = int(e % gw);
         const int64_t t = e / gw;
         const int iy = int(t % gh), iz = int((t / gh) % L);
         const float v = __ldg(grids + e);
         float d;
-        if (ix + 1 < gw) { d = __ldg(grids + e + 1) - v; acc = fmaf(w.x * d, d, acc); }
-        if (iy + 1 < gh) { d = __ldg(grids + e + gw) - v; acc = fmaf(w.y * d, d, acc); }
-        if (iz + 1 < L) { d = __ldg(grids + e + int64_t(gh) * gw) - v; acc = fmaf(w.z * d, d, acc); }
+        if (ix + 1 < gw) { d = __ldg(grids + e + 1) - v; acc[0] = fmaf(w.x * d, d, acc[0]); }
+        if (iy + 1 < gh) { d = __ldg(grids + e + gw) - v; acc[0] = fmaf(w.y * d, d, acc[0]); }
+        if (iz + 1 < L) { d = __ldg(grids + e + int64_t(gh) * gw) - v; acc[0] = fmaf(w.z * d, d, acc[0]); }
     }
-    acc = warp_sum(acc);
-    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        float t = 0.f;
-#pragma unroll
-        for (int i = 0; i < TV_THREADS / 32; ++i) t += s_red[i];
-        partials[blockIdx.x] = t;
-    }
+    cta_sum_row(acc, s_red, threadIdx.x, [&] { return partials + blockIdx.x; });
 }
 
 // v = up * d tv / d x: each squared difference (b - a)^2 w gives 2 w (a - b) to a and 2 w (b - a) to b

@@ -62,13 +62,40 @@ __device__ __forceinline__ void tile_rect(float x, float y, float r, int grid_x,
     }
 }
 
-__device__ __forceinline__ float warp_sum(float v) {
-    v += __shfl_xor_sync(0xffffffffu, v, 16);
-    v += __shfl_xor_sync(0xffffffffu, v, 8);
-    v += __shfl_xor_sync(0xffffffffu, v, 4);
-    v += __shfl_xor_sync(0xffffffffu, v, 2);
-    v += __shfl_xor_sync(0xffffffffu, v, 1);
+struct Sum { template <class T> __device__ __forceinline__ T operator()(T a, T b) const { return a + b; } };
+struct Min { template <class T> __device__ __forceinline__ T operator()(T a, T b) const { return fmin(a, b); } };
+struct Max { template <class T> __device__ __forceinline__ T operator()(T a, T b) const { return fmax(a, b); } };
+
+// Reduction over the 32 lanes of a full warp by the xor butterfly 16, 8, 4, 2, 1: every lane gets the result, combined in the
+// same order on every call.
+template <class Op, class T>
+__device__ __forceinline__ T warp_reduce(T v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = Op()(v, __shfl_xor_sync(0xffffffffu, v, o));
     return v;
+}
+
+__device__ __forceinline__ float warp_sum(float v) { return warp_reduce<Sum>(v); }
+
+// One row of K per-CTA partial sums from K values per thread (tid = the thread's index in the CTA of W full warps, of the caller's
+// integer type): each value is summed over its warp, the warp sums go to s_red[warp][k], and thread k < K adds column k over
+// warps 0, 1, ..., W - 1 in that order and stores it at row()[k], row() giving the CTA's output row.  Every thread of the CTA must
+// call it (it synchronises the CTA); v is overwritten.
+template <int W, int K, class Index, class Row>
+__device__ __forceinline__ void cta_sum_row(float (&v)[K], float (&s_red)[W][K], Index tid, Row row) {
+#pragma unroll
+    for (int k = 0; k < K; ++k) v[k] = warp_sum(v[k]);
+    if ((tid & 31) == 0) {
+#pragma unroll
+        for (int k = 0; k < K; ++k) s_red[tid >> 5][k] = v[k];
+    }
+    __syncthreads();
+    if (tid < K) {
+        float t = 0.f;
+#pragma unroll
+        for (int w = 0; w < W; ++w) t += s_red[w][tid];
+        row()[tid] = t;
+    }
 }
 
 // launchers (one per translation unit)

@@ -15,20 +15,17 @@
 //     workspace head.  Normalisations are positive and monotone in float32, so b's extrema are those of pred, normalised.
 //   * K29 fwd: 16x16 tiles; per-CTA partials of |a-b| or (a-b)^2 and, with SSIM, of the SSIM map, its derivatives with C1 and
 //     C2, and the number of pixels tied at b's max and min; with SSIM also the three derivative maps of the map with b's blurred
-//     moments (mu_b, E[b^2], E[ab]), zero outside the full-window positions.
+//     moments (mu_b, E[b^2], E[ab]), zero outside the full-window positions.  K29 and K31 run the SSIM tile engine of ssim.cuh
+//     with torchmetrics' window, differentiated in b.
 //   * K30 loss (one CTA): adds the partials in block order, writes the loss, the statistics and the backward's coefficients.
 //   * K31 bwd: v_pred = up * chain * (L1/L2 term + blur of the maps + the dr term at the extremum pixels).
 // No float atomics: every sum has a fixed order, so two backwards are bit-identical.
-#include "common.cuh"
+#include "ssim.cuh"
 
 namespace b200gs {
 
 namespace {
 
-constexpr int LT = 16;                  // tile edge
-constexpr int HALO = 5;
-constexpr int LE = LT + 2 * HALO;
-constexpr int TAPS = 11;
 constexpr int STAT_THREADS = 256;
 constexpr int STAT_PIXELS = 2048;       // pixels per stats CTA before the grid saturates
 constexpr int STAT_MAX_BLOCKS = 1024;
@@ -67,24 +64,6 @@ __device__ __forceinline__ bool kept(const uint8_t* __restrict__ mask, const DAr
     return mask == nullptr || __ldg(mask + g.msy * y + g.msx * x) != 0;
 }
 
-__device__ __forceinline__ float warp_min(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = fminf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
-
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
-
-__device__ __forceinline__ double warp_sum_d(double v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 __global__ void __launch_bounds__(STAT_THREADS) depth_stats_kernel(int64_t n, const float* __restrict__ pred, const float* __restrict__ gt,
                                                                    float* __restrict__ partials) {
     __shared__ float s[STAT_THREADS / 32][5];
@@ -95,7 +74,8 @@ __global__ void __launch_bounds__(STAT_THREADS) depth_stats_kernel(int64_t n, co
         v[2] = fminf(v[2], q); v[3] = fmaxf(v[3], q);
         v[4] += q;
     }
-    v[0] = warp_min(v[0]); v[1] = warp_max(v[1]); v[2] = warp_min(v[2]); v[3] = warp_max(v[3]); v[4] = warp_sum(v[4]);
+    v[0] = warp_reduce<Min>(v[0]); v[1] = warp_reduce<Max>(v[1]); v[2] = warp_reduce<Min>(v[2]); v[3] = warp_reduce<Max>(v[3]);
+    v[4] = warp_sum(v[4]);
     const int warp = threadIdx.x >> 5;
     if ((threadIdx.x & 31) == 0) {
 #pragma unroll
@@ -125,8 +105,8 @@ __global__ void __launch_bounds__(RED_THREADS) depth_prep_kernel(DArgs g, int n_
         v[0] = fminf(v[0], p[0]); v[1] = fmaxf(v[1], p[1]); v[2] = fminf(v[2], p[2]); v[3] = fmaxf(v[3], p[3]);
         sum += double(p[4]);
     }
-    v[0] = warp_min(v[0]); v[1] = warp_max(v[1]); v[2] = warp_min(v[2]); v[3] = warp_max(v[3]);
-    sum = warp_sum_d(sum);
+    v[0] = warp_reduce<Min>(v[0]); v[1] = warp_reduce<Max>(v[1]); v[2] = warp_reduce<Min>(v[2]); v[3] = warp_reduce<Max>(v[3]);
+    sum = warp_reduce<Sum>(sum);
     if ((t & 31) == 0) {
 #pragma unroll
         for (int k = 0; k < 4; ++k) s_f[warp][k] = v[k];
@@ -153,23 +133,6 @@ __global__ void __launch_bounds__(RED_THREADS) depth_prep_kernel(DArgs g, int n_
     head[H_SHARE] = rb > ra ? 1.f : (rb == ra ? 0.5f : 0.f);
 }
 
-// the (LE x LE) halo tile of a' and b' (normalised, masked), zero outside the image
-__device__ __forceinline__ void load_ab(const DArgs& g, const float* __restrict__ pred, const float* __restrict__ gt, int x0, int y0,
-                                        float sub, float div, float (*sa)[LE], float (*sb)[LE]) {
-    for (int i = threadIdx.x; i < LE * LE; i += LT * LT) {
-        const int ly = i / LE, lx = i - ly * LE;
-        const int x = x0 + lx - HALO, y = y0 + ly - HALO;
-        float a = 0.f, b = 0.f;
-        if (x >= 0 && x < g.width && y >= 0 && y < g.height) {
-            const int64_t p = int64_t(y) * g.width + x;
-            a = norm_gt(__ldg(gt + p), g.norm, div);
-            b = norm_pred(__ldg(pred + p), g.norm, sub, div);
-        }
-        sa[ly][lx] = a;
-        sb[ly][lx] = b;
-    }
-}
-
 template <bool SSIM>
 __global__ void __launch_bounds__(LT * LT) depth_fwd_kernel(DArgs g, const float* __restrict__ pred, const float* __restrict__ gt,
                                                             const uint8_t* __restrict__ mask, const float* __restrict__ head,
@@ -184,22 +147,12 @@ __global__ void __launch_bounds__(LT * LT) depth_fwd_kernel(DArgs g, const float
     const float sub = __ldg(head + H_SUB), div = __ldg(head + H_DIV);
     float acc[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     if constexpr (SSIM) {
-        load_ab(g, pred, gt, x0, y0, sub, div, s_a, s_b);
+        // the halo tiles of a' and b', normalised
+        load_halo(g.width, g.height, x0, y0, {s_a, s_b}, [&](int m, int64_t p) {
+            return m == 0 ? norm_gt(__ldg(gt + p), g.norm, div) : norm_pred(__ldg(pred + p), g.norm, sub, div);
+        });
         __syncthreads();
-        for (int i = threadIdx.x; i < LE * LT; i += LT * LT) {
-            const int ry = i / LT, rx = i - ry * LT;
-            float m0 = 0.f, m1 = 0.f, m2 = 0.f, m3 = 0.f, m4 = 0.f;
-#pragma unroll
-            for (int k = 0; k < TAPS; ++k) {
-                const float w = c_win[k], a = s_a[ry][rx + k], b = s_b[ry][rx + k];
-                m0 = fmaf(w, a, m0);
-                m1 = fmaf(w, b, m1);
-                m2 = fmaf(w, a * a, m2);
-                m3 = fmaf(w, b * b, m3);
-                m4 = fmaf(w, a * b, m4);
-            }
-            s_h[0][ry][rx] = m0; s_h[1][ry][rx] = m1; s_h[2][ry][rx] = m2; s_h[3][ry][rx] = m3; s_h[4][ry][rx] = m4;
-        }
+        blur_moments_h(c_win, s_a, s_b, s_h);
         __syncthreads();
         if (inside) {
             const float a = s_a[ly + HALO][lx + HALO], b = s_b[ly + HALO][lx + HALO];
@@ -208,29 +161,16 @@ __global__ void __launch_bounds__(LT * LT) depth_fwd_kernel(DArgs g, const float
             acc[5] = b == __ldg(head + H_BMIN) ? 1.f : 0.f;
             float d_mu = 0.f, d_bb = 0.f, d_ab = 0.f;
             if (y >= HALO && y < g.height - HALO && x >= HALO && x < g.width - HALO) {
-                float mu1 = 0.f, mu2 = 0.f, e11 = 0.f, e22 = 0.f, e12 = 0.f;
-#pragma unroll
-                for (int k = 0; k < TAPS; ++k) {
-                    const float w = c_win[k];
-                    mu1 = fmaf(w, s_h[0][ly + k][lx], mu1);
-                    mu2 = fmaf(w, s_h[1][ly + k][lx], mu2);
-                    e11 = fmaf(w, s_h[2][ly + k][lx], e11);
-                    e22 = fmaf(w, s_h[3][ly + k][lx], e22);
-                    e12 = fmaf(w, s_h[4][ly + k][lx], e12);
-                }
-                const float C1 = __ldg(head + H_C1), C2 = __ldg(head + H_C2);
-                const float s1 = e11 - mu1 * mu1, s2 = e22 - mu2 * mu2, s12 = e12 - mu1 * mu2;
-                const float A1 = 2.f * mu1 * mu2 + C1, A2 = 2.f * s12 + C2;
-                const float B1 = mu1 * mu1 + mu2 * mu2 + C1, B2 = s1 + s2 + C2;
-                const float iB1 = 1.f / B1, iB2 = 1.f / B2;
-                const float ss = A1 * A2 * iB1 * iB2;
-                acc[1] = ss;
-                acc[2] = A2 * iB1 * iB2 - ss * iB1;     // d ssim / d C1
-                acc[3] = A1 * iB1 * iB2 - ss * iB2;     // d ssim / d C2
-                // with b's blurred moments (mu_b, E[b^2], E[ab]) as the variables; s2 and s12 depend on mu_b
-                d_mu = (2.f * mu1 * A2 - 2.f * mu1 * A1) * iB1 * iB2 - ss * (2.f * mu2 * iB1 - 2.f * mu2 * iB2);
-                d_bb = -ss * iB2;
-                d_ab = 2.f * A1 * iB1 * iB2;
+                float m[5];
+                blur_moments_v(c_win, s_h, ly, lx, m);
+                // derivatives with b's blurred moments (mu_b, E[b^2], E[ab])
+                const SsimTerms t = ssim_terms<1>(m, __ldg(head + H_C1), __ldg(head + H_C2));
+                acc[1] = t.ssim;
+                acc[2] = t.d_c1;
+                acc[3] = t.d_c2;
+                d_mu = t.d_mu;
+                d_bb = t.d_xx;
+                d_ab = t.d_ab;
             }
             const int64_t p = int64_t(y) * g.width + x, plane = int64_t(g.height) * g.width;
             maps[p] = d_mu;
@@ -242,20 +182,7 @@ __global__ void __launch_bounds__(LT * LT) depth_fwd_kernel(DArgs g, const float
         const float d = kept(mask, g, y, x) ? norm_pred(__ldg(pred + p), g.norm, sub, div) - norm_gt(__ldg(gt + p), g.norm, div) : 0.f;
         acc[0] = g.l2 ? d * d : fabsf(d);
     }
-    const int warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < 6; ++k) acc[k] = warp_sum(acc[k]);
-    if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-        for (int k = 0; k < 6; ++k) s_red[warp][k] = acc[k];
-    }
-    __syncthreads();
-    if (threadIdx.x < 6) {
-        float t = 0.f;
-#pragma unroll
-        for (int w = 0; w < LT * LT / 32; ++w) t += s_red[w][threadIdx.x];
-        partials[(int64_t(blockIdx.y) * gridDim.x + blockIdx.x) * PART + threadIdx.x] = t;
-    }
+    cta_sum_row(acc, s_red, threadIdx.x, [&] { return partials + (int64_t(blockIdx.y) * gridDim.x + blockIdx.x) * PART; });
 }
 
 __global__ void __launch_bounds__(RED_THREADS) depth_loss_kernel(DArgs g, int ssim, int64_t n_blocks, const float* __restrict__ partials,
@@ -267,7 +194,7 @@ __global__ void __launch_bounds__(RED_THREADS) depth_loss_kernel(DArgs g, int ss
     for (int64_t b = t; b < n_blocks; b += RED_THREADS)
         for (int k = 0; k < nv; ++k) v[k] += double(partials[b * PART + k]);
 #pragma unroll
-    for (int k = 0; k < 6; ++k) v[k] = warp_sum_d(v[k]);
+    for (int k = 0; k < 6; ++k) v[k] = warp_reduce<Sum>(v[k]);
     if ((t & 31) == 0) {
 #pragma unroll
         for (int k = 0; k < 6; ++k) s[warp][k] = v[k];
@@ -309,38 +236,14 @@ __global__ void __launch_bounds__(LT * LT) depth_bwd_kernel(DArgs g, const float
     const int x0 = blockIdx.x * LT, y0 = blockIdx.y * LT;
     const int lx = threadIdx.x % LT, ly = threadIdx.x / LT;
     const int x = x0 + lx, y = y0 + ly;
-    float g0 = 0.f, g1 = 0.f, g2 = 0.f;
+    float gm[3] = {0.f, 0.f, 0.f};
     if constexpr (SSIM) {
         const int64_t plane = int64_t(g.height) * g.width;
-        for (int i = threadIdx.x; i < LE * LE; i += LT * LT) {
-            const int ry = i / LE, rx = i - ry * LE;
-            const int xx = x0 + rx - HALO, yy = y0 + ry - HALO;
-            const bool in = xx >= 0 && xx < g.width && yy >= 0 && yy < g.height;
-            const int64_t p = int64_t(yy) * g.width + xx;
-#pragma unroll
-            for (int m = 0; m < 3; ++m) s_m[m][ry][rx] = in ? __ldg(maps + m * plane + p) : 0.f;
-        }
+        load_halo(g.width, g.height, x0, y0, {s_m[0], s_m[1], s_m[2]}, [=](int m, int64_t p) { return __ldg(maps + m * plane + p); });
         __syncthreads();
-        for (int i = threadIdx.x; i < LE * LT; i += LT * LT) {
-            const int ry = i / LT, rx = i - ry * LT;
-            float h0 = 0.f, h1 = 0.f, h2 = 0.f;
-#pragma unroll
-            for (int k = 0; k < TAPS; ++k) {
-                const float w = c_win[k];
-                h0 = fmaf(w, s_m[0][ry][rx + k], h0);
-                h1 = fmaf(w, s_m[1][ry][rx + k], h1);
-                h2 = fmaf(w, s_m[2][ry][rx + k], h2);
-            }
-            s_h[0][ry][rx] = h0; s_h[1][ry][rx] = h1; s_h[2][ry][rx] = h2;
-        }
+        blur_maps_h(c_win, s_m, s_h);
         __syncthreads();
-#pragma unroll
-        for (int k = 0; k < TAPS; ++k) {
-            const float w = c_win[k];
-            g0 = fmaf(w, s_h[0][ly + k][lx], g0);
-            g1 = fmaf(w, s_h[1][ly + k][lx], g1);
-            g2 = fmaf(w, s_h[2][ly + k][lx], g2);
-        }
+        blur_maps_v(c_win, s_h, ly, lx, gm);
     }
     if (x >= g.width || y >= g.height) return;
     const int64_t p = int64_t(y) * g.width + x;
@@ -355,7 +258,7 @@ __global__ void __launch_bounds__(LT * LT) depth_bwd_kernel(DArgs g, const float
     const float sgn = d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f);          // torch.abs' subgradient at 0 is 0
     float v = __ldg(head + H_VL) * (g.l2 ? d : sgn);
     if (SSIM) {
-        v += __ldg(head + H_VS) * (g0 + 2.f * b * g1 + a * g2);
+        v += __ldg(head + H_VS) * ssim_grad(gm, b, a);
         if (b == __ldg(head + H_BMAX)) v += __ldg(head + H_GMAX);
         if (b == __ldg(head + H_BMIN)) v += __ldg(head + H_GMIN);
     }

@@ -70,8 +70,7 @@ __global__ void __launch_bounds__(PREP_THREADS) exposure_prep_kernel(int n_app, 
     const int n = s * s;
     float mx = 0.f;                     // sigmoid > 0
     for (int i = t; i < n; i += PREP_THREADS) mx = fmaxf(mx, sigmoidf(__ldg(S + i)));
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    mx = warp_reduce<Max>(mx);
     if ((t & 31) == 0) s_max[t >> 5] = mx;
     __syncthreads();
     mx = 0.f;
@@ -138,19 +137,7 @@ __global__ void __launch_bounds__(BX * BY) exposure_bwd_kernel(ExpoArgs g, const
             if (SHADE) v_m[int64_t(y) * g.width + x] = vm;
         }
     }
-#pragma unroll
-    for (int k = 0; k < 7; ++k) acc[k] = warp_sum(acc[k]);
-    if ((tid & 31) == 0) {
-#pragma unroll
-        for (int k = 0; k < 7; ++k) s_red[tid >> 5][k] = acc[k];
-    }
-    __syncthreads();
-    if (tid < 7) {
-        float t = 0.f;
-#pragma unroll
-        for (int w = 0; w < BX * BY / 32; ++w) t += s_red[w][tid];
-        partials[int64_t(blockIdx.y * gridDim.x + blockIdx.x) * PARTIAL + tid] = t;
-    }
+    cta_sum_row(acc, s_red, tid, [&] { return partials + int64_t(blockIdx.y * gridDim.x + blockIdx.x) * PARTIAL; });
 }
 
 // pixel range [lo, hi] of one axis whose bilinear footprint may include cell i (widened by one; the caller tests membership)

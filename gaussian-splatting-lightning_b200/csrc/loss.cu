@@ -2,22 +2,19 @@
 // validated against the oracle and the reference-generated golden vectors: tests/test_gpu_loss.py):
 //     loss = (1 - lambda) * mean|img - gt| + lambda * (1 - mean(SSIM(img, gt)))          internal/metrics/vanilla_metrics.py:57-74
 //     SSIM: 11-tap Gaussian window (sigma 1.5), zero padding, C1 = 0.01^2, C2 = 0.03^2     internal/utils/ssim.py:23-63
-// The window is separable.  K9 (forward): one CTA per 16x16 tile and channel loads the tile + 5-pixel halo of both images
-// into shared memory, blurs the five moments (a, b, a^2, b^2, ab) horizontally then vertically, evaluates the SSIM map and
-// writes (i) per-CTA partial sums of |a-b| and SSIM (summed by the caller: deterministic) and (ii) the three partial
-// derivative maps d ssim / d(mu_a), d(E[a^2]), d(E[ab]).  K10 (backward): the image cotangent is the same blur applied to
-// those maps (the window is symmetric),  v_img = w * ( (1-l) sign(a-b) - l * (blur(dmu) + 2 a blur(de11) + b blur(de12)) ) / (C H W).
+// The window is separable; the tile engine is ssim.cuh.  K9 (forward): one CTA per 16x16 tile and channel loads the tile +
+// 5-pixel halo of both images into shared memory, blurs the five moments (a, b, a^2, b^2, ab) horizontally then vertically,
+// evaluates the SSIM map and writes (i) per-CTA partial sums of |a-b| and SSIM (summed by the caller: deterministic) and (ii)
+// the three partial derivative maps d ssim / d(mu_a), d(E[a^2]), d(E[ab]).  K10 (backward): the image cotangent is the same
+// blur applied to those maps (the window is symmetric),
+//     v_img = w * ( (1-l) sign(a-b) - l * (blur(dmu) + 2 a blur(de11) + b blur(de12)) ) / (C H W).
 // Oracle: oracle/loss_oracle.py, pinned to the reference's ssim.py by tests/test_loss_oracle_golden.py.
-#include "common.cuh"
+#include "ssim.cuh"
 
 namespace b200gs {
 
 namespace {
 
-constexpr int LT = 16;             // tile edge
-constexpr int HALO = 5;            // (11 - 1) / 2
-constexpr int LE = LT + 2 * HALO;  // 26
-constexpr int TAPS = 11;
 constexpr float C1 = 0.01f * 0.01f;
 constexpr float C2 = 0.03f * 0.03f;
 
@@ -26,88 +23,41 @@ __device__ __constant__ float c_win[TAPS] = {1.028380124e-03f, 7.598758209e-03f,
                                              2.660117149e-01f, 2.130055279e-01f, 1.093606874e-01f, 3.600077331e-02f, 7.598758209e-03f,
                                              1.028380124e-03f};
 
-// load the (LE x LE) halo tile of one channel plane, zero outside the image
-__device__ __forceinline__ void load_halo(const float* __restrict__ plane, int width, int height, int x0, int y0, float (*dst)[LE]) {
-    for (int i = threadIdx.x; i < LE * LE; i += LT * LT) {
-        const int ly = i / LE, lx = i - ly * LE;
-        const int x = x0 + lx - HALO, y = y0 + ly - HALO;
-        dst[ly][lx] = (x >= 0 && x < width && y >= 0 && y < height) ? __ldg(plane + int64_t(y) * width + x) : 0.f;
-    }
-}
-
 __global__ void __launch_bounds__(LT * LT) loss_fwd_kernel(int width, int height, const float* __restrict__ img, const float* __restrict__ gt,
                                                            float* __restrict__ dmaps, float* __restrict__ partials) {
     __shared__ float s_a[LE][LE], s_b[LE][LE];
     __shared__ float s_h[5][LE][LT];        // horizontally blurred moments: rows with halo, columns of the tile
-    __shared__ float s_red[2][LT * LT / 32];
+    __shared__ float s_red[LT * LT / 32][2];
     const int c = blockIdx.z;
     const int x0 = blockIdx.x * LT, y0 = blockIdx.y * LT;
     const int64_t plane = int64_t(width) * height;
-    load_halo(img + c * plane, width, height, x0, y0, s_a);
-    load_halo(gt + c * plane, width, height, x0, y0, s_b);
+    const float* img_c = img + c * plane;
+    const float* gt_c = gt + c * plane;
+    load_halo(width, height, x0, y0, {s_a}, [=](int, int64_t p) { return __ldg(img_c + p); });
+    load_halo(width, height, x0, y0, {s_b}, [=](int, int64_t p) { return __ldg(gt_c + p); });
     __syncthreads();
-    for (int i = threadIdx.x; i < LE * LT; i += LT * LT) {
-        const int ly = i / LT, lx = i - ly * LT;
-        float m0 = 0.f, m1 = 0.f, m2 = 0.f, m3 = 0.f, m4 = 0.f;
-#pragma unroll
-        for (int k = 0; k < TAPS; ++k) {
-            const float w = c_win[k], a = s_a[ly][lx + k], b = s_b[ly][lx + k];
-            m0 = fmaf(w, a, m0);
-            m1 = fmaf(w, b, m1);
-            m2 = fmaf(w, a * a, m2);
-            m3 = fmaf(w, b * b, m3);
-            m4 = fmaf(w, a * b, m4);
-        }
-        s_h[0][ly][lx] = m0; s_h[1][ly][lx] = m1; s_h[2][ly][lx] = m2; s_h[3][ly][lx] = m3; s_h[4][ly][lx] = m4;
-    }
+    blur_moments_h(c_win, s_a, s_b, s_h);
     __syncthreads();
     const int lx = threadIdx.x % LT, ly = threadIdx.x / LT;
     const int x = x0 + lx, y = y0 + ly;
     const bool inside = x < width && y < height;
-    float mu1 = 0.f, mu2 = 0.f, e11 = 0.f, e22 = 0.f, e12 = 0.f;
-#pragma unroll
-    for (int k = 0; k < TAPS; ++k) {
-        const float w = c_win[k];
-        mu1 = fmaf(w, s_h[0][ly + k][lx], mu1);
-        mu2 = fmaf(w, s_h[1][ly + k][lx], mu2);
-        e11 = fmaf(w, s_h[2][ly + k][lx], e11);
-        e22 = fmaf(w, s_h[3][ly + k][lx], e22);
-        e12 = fmaf(w, s_h[4][ly + k][lx], e12);
-    }
-    float l1 = 0.f, ss = 0.f;
+    float m[5];
+    blur_moments_v(c_win, s_h, ly, lx, m);
+    float acc[2] = {0.f, 0.f};              // |a - b|, SSIM
     if (inside) {
         const float a = s_a[ly + HALO][lx + HALO], b = s_b[ly + HALO][lx + HALO];
-        const float s1 = e11 - mu1 * mu1, s2 = e22 - mu2 * mu2, s12 = e12 - mu1 * mu2;
-        const float A1 = 2.f * mu1 * mu2 + C1, A2 = 2.f * s12 + C2;
-        const float B1 = mu1 * mu1 + mu2 * mu2 + C1, B2 = s1 + s2 + C2;
-        const float iB1 = 1.f / B1, iB2 = 1.f / B2;
-        ss = A1 * A2 * iB1 * iB2;
-        l1 = fabsf(a - b);
-        // partial derivatives of the SSIM map with the blurred moments (mu1, E[a^2], E[ab]) as independent variables;
-        // s1, s12 depend on mu1 through -mu1^2 and -mu1*mu2
-        const float d_mu1 = (2.f * mu2 * A2 - 2.f * mu2 * A1) * iB1 * iB2 - ss * (2.f * mu1 * iB1 - 2.f * mu1 * iB2);
-        const float d_e11 = -ss * iB2;
-        const float d_e12 = 2.f * A1 * iB1 * iB2;
+        const SsimTerms t = ssim_terms<0>(m, C1, C2);
+        acc[0] = fabsf(a - b);
+        acc[1] = t.ssim;
         const int64_t p = c * plane + int64_t(y) * width + x;
         const int64_t stride = int64_t(gridDim.z) * plane;
-        dmaps[p] = d_mu1;
-        dmaps[stride + p] = d_e11;
-        dmaps[2 * stride + p] = d_e12;
+        dmaps[p] = t.d_mu;
+        dmaps[stride + p] = t.d_xx;
+        dmaps[2 * stride + p] = t.d_ab;
     }
     // per-CTA partial sums (summed by the caller in a fixed order)
-    l1 = warp_sum(l1);
-    ss = warp_sum(ss);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (lane == 0) { s_red[0][warp] = l1; s_red[1][warp] = ss; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        float t0 = 0.f, t1 = 0.f;
-#pragma unroll
-        for (int w = 0; w < LT * LT / 32; ++w) { t0 += s_red[0][w]; t1 += s_red[1][w]; }
-        const int64_t blk = (int64_t(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
-        partials[2 * blk] = t0;
-        partials[2 * blk + 1] = t1;
-    }
+    cta_sum_row(acc, s_red, threadIdx.x,
+                [&] { return partials + 2 * ((int64_t(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x); });
 }
 
 __global__ void __launch_bounds__(LT * LT) loss_bwd_kernel(int width, int height, const float* __restrict__ img, const float* __restrict__ gt,
@@ -120,39 +70,25 @@ __global__ void __launch_bounds__(LT * LT) loss_bwd_kernel(int width, int height
     const int64_t plane = int64_t(width) * height;
     const int64_t stride = int64_t(gridDim.z) * plane;
 #pragma unroll
-    for (int m = 0; m < 3; ++m) load_halo(dmaps + m * stride + c * plane, width, height, x0, y0, s_m[m]);
-    __syncthreads();
-    for (int i = threadIdx.x; i < LE * LT; i += LT * LT) {
-        const int ly = i / LT, lx = i - ly * LT;
-        float h0 = 0.f, h1 = 0.f, h2 = 0.f;
-#pragma unroll
-        for (int k = 0; k < TAPS; ++k) {
-            const float w = c_win[k];
-            h0 = fmaf(w, s_m[0][ly][lx + k], h0);
-            h1 = fmaf(w, s_m[1][ly][lx + k], h1);
-            h2 = fmaf(w, s_m[2][ly][lx + k], h2);
-        }
-        s_h[0][ly][lx] = h0; s_h[1][ly][lx] = h1; s_h[2][ly][lx] = h2;
+    for (int m = 0; m < 3; ++m) {
+        const float* map = dmaps + m * stride + c * plane;
+        load_halo(width, height, x0, y0, {s_m[m]}, [=](int, int64_t p) { return __ldg(map + p); });
     }
+    __syncthreads();
+    blur_maps_h(c_win, s_m, s_h);
     __syncthreads();
     const int lx = threadIdx.x % LT, ly = threadIdx.x / LT;
     const int x = x0 + lx, y = y0 + ly;
     if (x >= width || y >= height) return;
-    float g0 = 0.f, g1 = 0.f, g2 = 0.f;
-#pragma unroll
-    for (int k = 0; k < TAPS; ++k) {
-        const float w = c_win[k];
-        g0 = fmaf(w, s_h[0][ly + k][lx], g0);
-        g1 = fmaf(w, s_h[1][ly + k][lx], g1);
-        g2 = fmaf(w, s_h[2][ly + k][lx], g2);
-    }
+    float g[3];
+    blur_maps_v(c_win, s_h, ly, lx, g);
     const int64_t p = c * plane + int64_t(y) * width + x;
     const float a = __ldg(img + p), b = __ldg(gt + p);
     const float d = a - b;
     const float sgn = d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f);          // torch.abs' subgradient at 0 is 0
     const float inv_n = 1.f / (float(gridDim.z) * float(width) * float(height));
     const float up = v_loss ? __ldg(v_loss) : 1.f;
-    v_img[p] = up * inv_n * ((1.f - lambda) * sgn - lambda * (g0 + 2.f * a * g1 + b * g2));
+    v_img[p] = up * inv_n * ((1.f - lambda) * sgn - lambda * ssim_grad(g, a, b));
 }
 
 }  // namespace

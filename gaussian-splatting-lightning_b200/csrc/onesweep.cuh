@@ -134,8 +134,7 @@ __device__ __forceinline__ uint32_t chained_exclusive(uint32_t* state, int t, ui
         if (!stalled) depth = min(2 * depth, DEPTH);
         if (consumed == 0 && ++spins > (1u << 27)) asm volatile("trap;");   // a word that is never published: a logic error, not a hang
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    acc = warp_reduce<Sum>(acc);
     if (lane == 0 && t > 0) st_volatile(state + t, ((acc + value) & VALUE_MASK) | FLAG_PREFIX);
     return acc;
 }

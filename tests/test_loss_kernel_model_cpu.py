@@ -1,7 +1,8 @@
-"""Desk-check of csrc/loss.cu on CPU: the kernels' tiling and index expressions (16x16 tile, 5-pixel halo, LE = 26, horizontal pass
-over LE rows x LT columns, vertical pass over 11 rows, zero padding outside the image, per-CTA partial sums, the derivative-map
-layout dmaps[3][C][H][W]) transcribed block by block into numpy and compared with oracle/loss_oracle.py + autograd.  The CUDA kernels
-themselves are validated on the GPU by tests/test_gpu_loss.py; this pins the indexing they were written with on the CPU."""
+"""Desk-check on CPU of K9/K10 (csrc/loss.cu) on the SSIM tile engine of csrc/ssim.cuh: the tiling and index expressions (16x16 tile,
+5-pixel halo, LE = 26, horizontal pass over LE rows x LT columns, vertical pass over 11 rows, zero padding outside the image,
+per-CTA partial sums, the derivative-map layout dmaps[3][C][H][W]) transcribed block by block into numpy and compared with
+oracle/loss_oracle.py + autograd.  The CUDA kernels themselves are validated on the GPU by tests/test_gpu_loss.py; this pins the
+indexing they were written with on the CPU."""
 import numpy as np
 import pytest
 import torch
