@@ -34,6 +34,10 @@ class B200gsAppearanceMlp(ctypes.Structure):
     ]
 
 
+class B200gsUvGrid(ctypes.Structure):
+    _fields_ = [("n_levels", c_int32), ("base_resolution", c_int32), ("per_level_scale", c_float)]
+
+
 class B200gsError(RuntimeError):
     pass
 
@@ -60,6 +64,16 @@ _SIGNATURES = {
     "b200gs_appearance_mlp_workspace_bytes": (c_size_t, [c_int32] * 5),
     "b200gs_appearance_mlp_fwd": (c_int32, [POINTER(B200gsAppearanceMlp), c_int64] + [_P] * 9 + [_P]),
     "b200gs_appearance_mlp_bwd": (c_int32, [POINTER(B200gsAppearanceMlp), c_int64] + [_P] * 12 + [_P, c_size_t, _P] + [_P]),
+    "b200gs_uv_grid_params": (c_int64, [POINTER(B200gsUvGrid)]),
+    "b200gs_uv_grid_fwd": (c_int32, [POINTER(B200gsUvGrid), c_int32, c_int32, _P, c_int64, _P, c_int32, _P, c_int64, _P, _P]),
+    "b200gs_uv_grid_bwd": (c_int32, [POINTER(B200gsUvGrid), c_int32, c_int32, _P, c_int64, _P, _P, _P]),
+    "b200gs_visibility_mlp_workspace_bytes": (c_size_t, [c_int32] * 3),
+    "b200gs_visibility_mlp_fwd": (c_int32, [POINTER(B200gsAppearanceMlp), c_int64, _P, _P, _P]),
+    "b200gs_visibility_mlp_bwd": (c_int32, [POINTER(B200gsAppearanceMlp), c_int64, _P, _P, _P, _P, c_size_t, _P, _P]),
+    "b200gs_vis_loss_blocks": (c_int64, [c_int32, c_int32]),
+    "b200gs_vis_loss_workspace_bytes": (c_size_t, [c_int32] * 3),
+    "b200gs_vis_loss_fwd": (c_int32, [c_int32, c_int32] + [_P] * 4 + [c_int32, _P, c_size_t, _P]),
+    "b200gs_vis_loss_bwd": (c_int32, [c_int32, c_int32] + [_P] * 5 + [c_size_t, c_float, c_float] + [_P] * 3 + [_P]),
     "b200gs_exposure_workspace_bytes": (c_size_t, [c_int32] * 4),
     "b200gs_exposure_fwd": (c_int32, [c_int32] * 3 + [_P] + [c_int64] * 3 + [c_int32] * 2 + [_P, _P, c_int64, c_int32, _P, c_float, c_float]
                             + [_P, c_size_t, _P, _P]),

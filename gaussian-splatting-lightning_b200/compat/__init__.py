@@ -12,6 +12,8 @@ import importlib.util
 import sys
 import types
 
+import torch
+
 
 def install(force: bool = False):
     from . import diff_gaussian_rasterization as dgr
@@ -77,6 +79,11 @@ def install(force: bool = False):
         sys.modules["fused_ssim"] = _fused_ssim_module()
     elif "fused_ssim" not in sys.modules and not any(isinstance(f, _OnImport) and f.name == "fused_ssim" for f in sys.meta_path):
         sys.meta_path.insert(0, _OnImport("fused_ssim", _fused_ssim_module))
+    # tinycudann.Encoding, 2-D DenseGrid only (gsplat_appearance_embedding_visibility_map_renderer.py:4,114-124), the same way
+    if force:
+        sys.modules["tinycudann"] = _tcnn_module()
+    elif "tinycudann" not in sys.modules and not any(isinstance(f, _OnImport) and f.name == "tinycudann" for f in sys.meta_path):
+        sys.meta_path.insert(0, _OnImport("tinycudann", _tcnn_module))
 
 
 def _fused_ssim_module():
@@ -84,6 +91,34 @@ def _fused_ssim_module():
     fs = types.ModuleType("fused_ssim")
     fs.fused_ssim = metrics.fused_ssim
     return fs
+
+
+def _tcnn_module():
+    from ..visibility import UVGridEncoding
+
+    class Encoding(UVGridEncoding):
+        """tinycudann.Encoding for n_input_dims 2 and otype DenseGrid with linear interpolation and 2 features per level, on K32/K33;
+        anything else raises.  The initial values are uniform(-1e-4, 1e-4) from torch's generator, not tcnn's pcg32 stream."""
+
+        def __init__(self, n_input_dims, encoding_config, seed=1337, dtype=None):
+            c = dict(encoding_config)
+            if n_input_dims != 2 or str(c.get("otype", "")).lower() not in ("densegrid", "dense") or \
+                    str(c.get("interpolation", "Linear")).lower() != "linear" or int(c.get("n_features_per_level", 2)) != 2 or \
+                    dtype not in (None, torch.float32):
+                raise NotImplementedError(f"b200gs provides tinycudann.Encoding for 2-D float32 DenseGrid with linear interpolation "
+                                          f"and 2 features per level only, got n_input_dims={n_input_dims}, {c}, dtype={dtype}")
+            super().__init__(c.get("n_levels", 16), c.get("base_resolution", 16), c.get("per_level_scale", 2.0))
+
+    def refuse(name):
+        def init(self, *args, **kwargs):
+            raise NotImplementedError(f"b200gs provides no tinycudann.{name}: only Encoding with a 2-D DenseGrid")
+        return type(name, (), {"__init__": init})
+
+    m = types.ModuleType("tinycudann")
+    m.Encoding = Encoding
+    m.Network = refuse("Network")
+    m.NetworkWithInputEncoding = refuse("NetworkWithInputEncoding")
+    return m
 
 
 class _OnImport(importlib.abc.MetaPathFinder, importlib.abc.Loader):

@@ -3,6 +3,7 @@
 #include <string.h>
 
 #include <atomic>
+#include <cmath>
 
 #include "common.cuh"
 
@@ -41,7 +42,7 @@ using namespace b200gs;
 extern "C" {
 
 const char* b200gs_last_error(void) { return g_error; }
-int b200gs_version(void) { return 229; }
+int b200gs_version(void) { return 230; }
 int64_t b200gs_launch_count(void) { return (int64_t)g_launches.load(std::memory_order_relaxed); }
 
 int b200gs_project_fwd(const B200gsView* view, int64_t n, const float* means, const float* scales, const float* quats,
@@ -375,6 +376,129 @@ int b200gs_appearance_mlp_bwd(const B200gsAppearanceMlp* mlp, int64_t n, const f
     }
     return launch_appearance_mlp_bwd(*mlp, n, features, mask, base_rgb, dirs, cam, raw_opacity, v_out, v_opacities, v_opacity_offsets,
                                      v_base_rgb, v_features, v_raw_opacity, static_cast<float*>(workspace), v_params, (cudaStream_t)stream);
+}
+
+static bool uv_grid_ok(const B200gsUvGrid* g) {
+    return g && g->n_levels >= 1 && g->n_levels <= 16 && g->base_resolution >= 1 && g->per_level_scale >= 1.f &&
+           std::isfinite(g->per_level_scale) && uv_grid_params(*g) <= INT32_MAX;
+}
+
+int64_t b200gs_uv_grid_params(const B200gsUvGrid* grid) { return uv_grid_ok(grid) ? uv_grid_params(*grid) : 0; }
+
+// shared by the forward and the backward; returns the error code, or 0 when the arguments are valid
+static int check_uv_grid(const char* fn, const B200gsUvGrid* grid, int32_t width, int32_t height, const float* uv, int64_t n) {
+    auto fail = [&](const char* msg) { set_error("%s: %s", fn, msg); return B200GS_EINVAL; };
+    if (!uv_grid_ok(grid)) return fail("bad grid: n_levels 1..16, base_resolution >= 1, per_level_scale >= 1");
+    if (uv == nullptr) {
+        if (width < 2 || height < 2) return fail("the pixel grid needs width and height >= 2 (u = x / (width - 1))");
+        if (int64_t(width) * height > INT32_MAX) return fail("image too large");
+    } else if (n < 0 || n > INT32_MAX) {
+        return fail("n out of range");
+    }
+    return 0;
+}
+
+int b200gs_uv_grid_fwd(const B200gsUvGrid* grid, int32_t width, int32_t height, const float* uv, int64_t n, const float* const* grids,
+                       int32_t n_grids, const int64_t* appearance_id, int64_t host_appearance_id, float* enc, void* stream) {
+    if (int rc = check_uv_grid(__func__, grid, width, height, uv, n)) return rc;
+    B200GS_CHECK_ARG(n_grids >= 1, "n_grids must be >= 1");
+    B200GS_CHECK_ARG(grids && enc, "NULL pointer");
+    B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(enc) & 7u) == 0, "enc must be 8-byte aligned");
+    return launch_uv_grid_fwd(*grid, width, height, uv, n, grids, n_grids, appearance_id, host_appearance_id, enc, (cudaStream_t)stream);
+}
+
+int b200gs_uv_grid_bwd(const B200gsUvGrid* grid, int32_t width, int32_t height, const float* uv, int64_t n, const float* v_enc,
+                       float* v_params, void* stream) {
+    if (int rc = check_uv_grid(__func__, grid, width, height, uv, n)) return rc;
+    B200GS_CHECK_ARG(v_enc && v_params, "NULL pointer");
+    B200GS_CHECK_ARG(((reinterpret_cast<uintptr_t>(v_enc) | reinterpret_cast<uintptr_t>(v_params)) & 7u) == 0,
+                     "v_enc and v_params must be 8-byte aligned");
+    return launch_uv_grid_bwd(*grid, width, height, uv, n, v_enc, v_params, (cudaStream_t)stream);
+}
+
+static bool visibility_shape_ok(int32_t feat_dim, int32_t n_neurons, int32_t n_layers) {
+    return feat_dim >= 8 && feat_dim % 8 == 0 && feat_dim <= 32 && (n_neurons == 64 || n_neurons == 128) && n_layers >= 2 &&
+           n_layers <= B200GS_APPEARANCE_MAX_LAYERS && appearance_mlp_fits(feat_dim, -1, n_neurons, n_layers, 1);
+}
+
+size_t b200gs_visibility_mlp_workspace_bytes(int32_t feat_dim, int32_t n_neurons, int32_t n_layers) {
+    if (!visibility_shape_ok(feat_dim, n_neurons, n_layers)) return 0;
+    return appearance_mlp_workspace_bytes(feat_dim, -1, n_neurons, n_layers, 1);
+}
+
+static int check_visibility(const char* fn, const B200gsAppearanceMlp* m, int64_t n, const float* enc) {
+    auto fail = [&](const char* msg) { set_error("%s: %s", fn, msg); return B200GS_EINVAL; };
+    if (m == nullptr) return fail("mlp is NULL");
+    if (m->n_freq != -1 || m->n_out != 1 || m->normalize || m->normalize_dirs || m->epilogue)
+        return fail("a visibility network has n_freq -1, n_out 1 and no normalisation or epilogue");
+    if (!visibility_shape_ok(m->feat_dim, m->n_neurons, m->n_layers))
+        return fail("feat_dim must be 8, 16, 24 or 32, n_neurons 64 or 128, n_layers 2..4");
+    if (m->w0_stride < m->feat_dim || m->w0_pe_col < m->feat_dim || m->w0_pe_col > m->w0_stride) return fail("bad w0_stride / w0_pe_col");
+    if (n < 0 || n > INT32_MAX) return fail("n out of range");
+    for (int l = 0; l < m->n_layers; ++l)
+        if (!m->weights[l] || !m->biases[l]) return fail("NULL weight or bias pointer");
+    if (n > 0 && !enc) return fail("NULL enc");
+    return B200GS_OK;
+}
+
+int b200gs_visibility_mlp_fwd(const B200gsAppearanceMlp* mlp, int64_t n, const float* enc, float* out, void* stream) {
+    if (int rc = check_visibility(__func__, mlp, n, enc)) return rc;
+    B200GS_CHECK_ARG(n == 0 || out, "NULL out");
+    return launch_appearance_mlp_fwd(*mlp, n, enc, nullptr, nullptr, nullptr, nullptr, nullptr, out, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+int b200gs_visibility_mlp_bwd(const B200gsAppearanceMlp* mlp, int64_t n, const float* enc, const float* v_out, float* v_enc,
+                              void* workspace, size_t workspace_bytes, float* v_params, void* stream) {
+    if (int rc = check_visibility(__func__, mlp, n, enc)) return rc;
+    B200GS_CHECK_ARG(v_params, "NULL v_params");
+    B200GS_CHECK_ARG(n == 0 || (v_out && workspace), "NULL v_out or workspace");
+    B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(v_enc) & 15u) == 0, "v_enc must be 16-byte aligned");
+    if (n > 0 && workspace_bytes < appearance_mlp_workspace_bytes(mlp->feat_dim, -1, mlp->n_neurons, mlp->n_layers, 1)) {
+        set_error("%s: workspace too small", __func__);
+        return B200GS_ENOSPACE;
+    }
+    return launch_appearance_mlp_bwd(*mlp, n, enc, nullptr, nullptr, nullptr, nullptr, nullptr, v_out, nullptr, nullptr, nullptr, v_enc,
+                                     nullptr, static_cast<float*>(workspace), v_params, (cudaStream_t)stream);
+}
+
+static bool vis_loss_size_ok(int32_t width, int32_t height) {
+    return width >= 1 && height >= 1 && height <= 65535 * 16 && int64_t(width) * height <= INT32_MAX / 4;
+}
+
+int64_t b200gs_vis_loss_blocks(int32_t width, int32_t height) { return vis_loss_size_ok(width, height) ? vis_loss_blocks(width, height) : 0; }
+
+size_t b200gs_vis_loss_workspace_bytes(int32_t width, int32_t height, int32_t vis_grad) {
+    return vis_loss_size_ok(width, height) ? vis_loss_workspace_bytes(width, height, vis_grad != 0) : 0;
+}
+
+// shared by the forward and the backward; returns the error code, or 0 when the arguments are valid
+static int check_vis_loss(const char* fn, int32_t width, int32_t height, const float* image, const float* gt, const float* visibility,
+                          const void* workspace, size_t workspace_bytes, bool vis_grad) {
+    auto fail = [&](const char* msg) { set_error("%s: %s", fn, msg); return B200GS_EINVAL; };
+    if (width < 1 || height < 1) return fail("image size must be >= 1");
+    if (!vis_loss_size_ok(width, height)) return fail("image too large");
+    if (!(image && gt && visibility && workspace)) return fail("NULL pointer");
+    if (workspace_bytes < vis_loss_workspace_bytes(width, height, vis_grad)) {
+        set_error("%s: workspace too small", fn);
+        return B200GS_ENOSPACE;
+    }
+    return 0;
+}
+
+int b200gs_vis_loss_fwd(int32_t width, int32_t height, const float* image, const float* gt, const float* visibility, const uint8_t* mask,
+                        int32_t vis_grad, void* workspace, size_t workspace_bytes, void* stream) {
+    if (int rc = check_vis_loss(__func__, width, height, image, gt, visibility, workspace, workspace_bytes, vis_grad != 0)) return rc;
+    return launch_vis_loss_fwd(width, height, image, gt, visibility, mask, vis_grad != 0, static_cast<float*>(workspace), (cudaStream_t)stream);
+}
+
+int b200gs_vis_loss_bwd(int32_t width, int32_t height, const float* image, const float* gt, const float* visibility, const uint8_t* mask,
+                        const void* workspace, size_t workspace_bytes, float lambda_dssim, float vis_reg_factor, const float* v_loss,
+                        float* v_image, float* v_visibility, void* stream) {
+    if (int rc = check_vis_loss(__func__, width, height, image, gt, visibility, workspace, workspace_bytes, v_visibility != nullptr))
+        return rc;
+    B200GS_CHECK_ARG(v_image, "NULL v_image");
+    return launch_vis_loss_bwd(width, height, image, gt, visibility, mask, static_cast<const float*>(workspace), lambda_dssim, vis_reg_factor,
+                               v_loss, v_image, v_visibility, (cudaStream_t)stream);
 }
 
 static bool exposure_size_ok(int32_t height, int32_t width, int32_t shade_size) {

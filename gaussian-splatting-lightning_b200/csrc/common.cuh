@@ -207,6 +207,20 @@ int launch_appearance_mlp_bwd(const B200gsAppearanceMlp& m, int64_t n, const flo
                               const float* v_opacity_offsets, float* v_base_rgb, float* v_features, float* v_raw_opacity, float* workspace,
                               float* v_params, cudaStream_t s);
 
+// transient visibility map (visibility.cu); arguments validated by the caller.  The workspace of the masked loss holds its derivative
+// maps, then its per-CTA partials.
+int64_t uv_grid_params(const B200gsUvGrid& g);
+int launch_uv_grid_fwd(const B200gsUvGrid& g, int width, int height, const float* uv, int64_t n, const float* const* grids, int n_grids,
+                       const int64_t* id_dev, int64_t id_host, float* enc, cudaStream_t s);
+int launch_uv_grid_bwd(const B200gsUvGrid& g, int width, int height, const float* uv, int64_t n, const float* v_enc, float* v_grid,
+                       cudaStream_t s);
+int64_t vis_loss_blocks(int width, int height);
+size_t vis_loss_workspace_bytes(int width, int height, bool vis_grad);
+int launch_vis_loss_fwd(int width, int height, const float* img, const float* gt, const float* vis, const uint8_t* mask, bool vis_grad,
+                        float* ws, cudaStream_t s);
+int launch_vis_loss_bwd(int width, int height, const float* img, const float* gt, const float* vis, const uint8_t* mask, const float* ws,
+                        float lambda_dssim, float vis_reg_factor, const float* v_loss, float* v_img, float* v_vis, cudaStream_t s);
+
 size_t knn_workspace_bytes(int64_t n);
 int launch_knn_mean_dist2(int64_t n, const float* points, float* out, void* ws, size_t ws_bytes, cudaStream_t s);
 

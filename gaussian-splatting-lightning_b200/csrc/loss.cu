@@ -15,14 +15,6 @@ namespace b200gs {
 
 namespace {
 
-constexpr float C1 = 0.01f * 0.01f;
-constexpr float C2 = 0.03f * 0.03f;
-
-// float32 window exactly as the reference builds it (exp in double, cast to float32, divided by its float32 sum)
-__device__ __constant__ float c_win[TAPS] = {1.028380124e-03f, 7.598758209e-03f, 3.600077331e-02f, 1.093606874e-01f, 2.130055279e-01f,
-                                             2.660117149e-01f, 2.130055279e-01f, 1.093606874e-01f, 3.600077331e-02f, 7.598758209e-03f,
-                                             1.028380124e-03f};
-
 __global__ void __launch_bounds__(LT * LT) loss_fwd_kernel(int width, int height, const float* __restrict__ img, const float* __restrict__ gt,
                                                            float* __restrict__ dmaps, float* __restrict__ partials) {
     __shared__ float s_a[LE][LE], s_b[LE][LE];
@@ -36,17 +28,17 @@ __global__ void __launch_bounds__(LT * LT) loss_fwd_kernel(int width, int height
     load_halo(width, height, x0, y0, {s_a}, [=](int, int64_t p) { return __ldg(img_c + p); });
     load_halo(width, height, x0, y0, {s_b}, [=](int, int64_t p) { return __ldg(gt_c + p); });
     __syncthreads();
-    blur_moments_h(c_win, s_a, s_b, s_h);
+    blur_moments_h(c_ssim_win, s_a, s_b, s_h);
     __syncthreads();
     const int lx = threadIdx.x % LT, ly = threadIdx.x / LT;
     const int x = x0 + lx, y = y0 + ly;
     const bool inside = x < width && y < height;
     float m[5];
-    blur_moments_v(c_win, s_h, ly, lx, m);
+    blur_moments_v(c_ssim_win, s_h, ly, lx, m);
     float acc[2] = {0.f, 0.f};              // |a - b|, SSIM
     if (inside) {
         const float a = s_a[ly + HALO][lx + HALO], b = s_b[ly + HALO][lx + HALO];
-        const SsimTerms t = ssim_terms<0>(m, C1, C2);
+        const SsimTerms t = ssim_terms<0>(m, SSIM_C1, SSIM_C2);
         acc[0] = fabsf(a - b);
         acc[1] = t.ssim;
         const int64_t p = c * plane + int64_t(y) * width + x;
@@ -75,13 +67,13 @@ __global__ void __launch_bounds__(LT * LT) loss_bwd_kernel(int width, int height
         load_halo(width, height, x0, y0, {s_m[m]}, [=](int, int64_t p) { return __ldg(map + p); });
     }
     __syncthreads();
-    blur_maps_h(c_win, s_m, s_h);
+    blur_maps_h(c_ssim_win, s_m, s_h);
     __syncthreads();
     const int lx = threadIdx.x % LT, ly = threadIdx.x / LT;
     const int x = x0 + lx, y = y0 + ly;
     if (x >= width || y >= height) return;
     float g[3];
-    blur_maps_v(c_win, s_h, ly, lx, g);
+    blur_maps_v(c_ssim_win, s_h, ly, lx, g);
     const int64_t p = c * plane + int64_t(y) * width + x;
     const float a = __ldg(img + p), b = __ldg(gt + p);
     const float d = a - b;

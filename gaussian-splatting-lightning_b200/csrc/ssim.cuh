@@ -15,6 +15,17 @@ constexpr int TAPS = 11;
 
 using Window = float[TAPS];
 
+// The reference's internal/utils/ssim.py SSIM (the L1+SSIM training loss, K9/K10, and its visibility-masked form, K34/K35):
+// C1 = 0.01^2, C2 = 0.03^2 and the 11-tap sigma-1.5 window in float32 exactly as the reference builds it (exp in double, cast to
+// float32, divided by its float32 sum).  A __constant__ table per translation unit that includes this header.
+constexpr float SSIM_C1 = 0.01f * 0.01f;
+constexpr float SSIM_C2 = 0.03f * 0.03f;
+namespace {
+__device__ __constant__ float c_ssim_win[TAPS] = {1.028380124e-03f, 7.598758209e-03f, 3.600077331e-02f, 1.093606874e-01f, 2.130055279e-01f,
+                                                  2.660117149e-01f, 2.130055279e-01f, 1.093606874e-01f, 3.600077331e-02f, 7.598758209e-03f,
+                                                  1.028380124e-03f};
+}  // namespace
+
 // dst[m] = the (LE x LE) halo tile of the tile at (x0, y0): load(m, p) at the image's pixel p = y * width + x, 0 outside the image
 template <int N, class Load>
 __device__ __forceinline__ void load_halo(int width, int height, int x0, int y0, float (*const (&dst)[N])[LE], Load load) {

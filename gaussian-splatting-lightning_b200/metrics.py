@@ -288,6 +288,28 @@ class B200InverseDepthMetricsModule(B200VanillaMetricsModule):
         return metrics, pbar
 
 
+@dataclass
+class B200VisibilityMapMetrics(B200VanillaMetrics):
+    """``VisibilityMapMetrics``: the RGB loss on image * w and gt * w, w = outputs["visibility"] * the dataset mask, plus
+    ``vis_reg_factor`` mean((1 - visibility)^2), on ``ops.visibility_l1_ssim_loss`` (K34/K35).  Validation metrics are
+    ``B200VanillaMetrics``', as in the reference."""
+    vis_reg_factor: float = 0.2
+
+    def instantiate(self, *args, **kwargs) -> "B200VisibilityMapMetricsModule":
+        self._check()
+        return B200VisibilityMapMetricsModule(self)
+
+
+class B200VisibilityMapMetricsModule(B200VanillaMetricsModule):
+    def get_train_metrics(self, pl_module, gaussian_model, step: int, batch, outputs):
+        camera, image_info, extra_data = batch
+        image_name, gt_image, masked_pixels = image_info
+        loss, stats = ops.visibility_l1_ssim_loss(outputs["render"], gt_image, outputs["visibility"], masked_pixels, self.lambda_dssim,
+                                                  self.config.vis_reg_factor)
+        metrics = {"loss": loss, "rgb_diff": stats[0], "ssim": stats[1], "vis_reg": stats[2]}
+        return metrics, {k: True for k in metrics}
+
+
 # ---- fused_ssim.fused_ssim (the name VanillaMetrics(fused_ssim=True) and the Taming density controller import) --------------
 def fused_ssim(img1, img2, padding="same", train=True):
     """fused-ssim's ``fused_ssim``: the mean SSIM of img1 and img2 [1,C,H,W] (11-tap Gaussian, sigma 1.5, zero padding,

@@ -1040,3 +1040,209 @@ def appearance_mlp(features, embedding, weights, biases, *, dirs=None, cam=None,
     return _AppearanceMlp.apply(cfg, _f32c(features, "features"), mask, _f32c(base_rgb, "base_rgb") if epilogue else None,
                                 _f32c(dirs, "dirs") if n_freq >= 0 else None, _f32c(cam.reshape(-1), "cam") if cam is not None and n_freq >= 0 else None,
                                 _f32c(raw_opacity, "raw_opacity") if raw_opacity is not None else None, e, *params)
+
+
+# ---- transient visibility map (csrc/visibility.cu; the visibility MLP runs on the appearance kernels) ------------------------------
+UV_GRID_FWD_LAUNCHES = 1        # library launches of one uv_grid_encode forward (K32)
+UV_GRID_BWD_LAUNCHES = 1        # and of its backward (K33)
+VISIBILITY_MLP_FWD_LAUNCHES = 1
+VISIBILITY_MLP_BWD_LAUNCHES = 2
+VISIBILITY_LOSS_FWD_LAUNCHES = 1    # K34
+VISIBILITY_LOSS_BWD_LAUNCHES = 1    # K35
+
+
+def uv_grid_params(n_levels: int = 8, base_resolution: int = 16, per_level_scale: float = 1.405) -> int:
+    """Floats of one DenseGrid of the given config (tcnn's ``n_params``; 121760 for the defaults), 0 when not supported."""
+    return int(lib().b200gs_uv_grid_params(ctypes.byref(_lib.B200gsUvGrid(n_levels, base_resolution, per_level_scale))))
+
+
+_GRID_TABLES = {}
+
+
+def _grid_table(grids, device) -> torch.Tensor:
+    """int64 [n] device table of the grids' addresses, built once per set of addresses: the kernels pick the row on the device."""
+    key = (str(device),) + tuple(g.data_ptr() for g in grids)
+    t = _GRID_TABLES.get(key)
+    if t is None:
+        if len(_GRID_TABLES) >= 16:
+            _GRID_TABLES.clear()
+        t = _GRID_TABLES[key] = torch.tensor(key[1:], dtype=torch.int64).to(device)
+    return t
+
+
+class _UvGridEncode(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, grid, width, height, uv, table, id_dev, host_id, selected):
+        n = width * height if uv is None else uv.shape[0]
+        enc = torch.empty(n, 2 * grid.n_levels, dtype=torch.float32, device=table.device)
+        check(lib().b200gs_uv_grid_fwd(ctypes.byref(grid), width, height, ptr(uv), n, ptr(table), table.shape[0], ptr(id_dev), host_id,
+                                       ptr(enc), _stream()), "b200gs_uv_grid_fwd")
+        ctx.grid, ctx.size = grid, (width, height, n)
+        ctx.save_for_backward(uv)
+        return enc
+
+    @staticmethod
+    def backward(ctx, v_enc):
+        (uv,) = ctx.saved_tensors
+        width, height, n = ctx.size
+        v_enc = _f32c(v_enc, "grad")
+        v_params = torch.empty(int(lib().b200gs_uv_grid_params(ctypes.byref(ctx.grid))), dtype=torch.float32, device=v_enc.device)
+        check(lib().b200gs_uv_grid_bwd(ctypes.byref(ctx.grid), width, height, ptr(uv), n, ptr(v_enc), ptr(v_params), _stream()),
+              "b200gs_uv_grid_bwd")
+        return None, None, None, None, None, None, None, v_params
+
+
+def uv_grid_encode(grids, appearance_id, *, width=None, height=None, uv=None, selected=None, n_levels=8, base_resolution=16,
+                   per_level_scale=1.405):
+    """tiny-cuda-nn's 2-D ``DenseGrid`` encoding (linear interpolation, 2 features per level) on K32/K33: enc [n, 2 n_levels].
+
+    ``grids``: the per-image flat parameter vectors (tcnn layout, ``uv_grid_params`` floats each); the one used is
+    ``grids[appearance_id]``, with ``appearance_id`` an int, a CPU tensor or a one-element CUDA tensor read on the device (an id out of
+    range gives NaN).  Coordinates: ``uv`` [n, 2], or, when None, the pixel grid of a ``width`` x ``height`` image (row-major, u =
+    x / (width - 1), v = y / (height - 1), both sizes >= 2).  The gradient goes to ``grids[selected]`` (default: the host id), the
+    pixel grid's without atomics, so two backwards are bit-identical.  With a CUDA ``appearance_id`` the caller passes ``selected``,
+    which must be the value that tensor holds: the kernels read the grid the device id names, and autograd can only route the
+    gradient to a tensor named on the host (``visibility.host_appearance_id`` reads and caches it per camera)."""
+    grid = _lib.B200gsUvGrid(int(n_levels), int(base_resolution), float(per_level_scale))
+    if not grids or any(g.dtype != torch.float32 or not g.is_cuda or not g.is_contiguous() for g in grids):
+        raise ValueError("grids must be contiguous float32 CUDA tensors")
+    if any(g.numel() != uv_grid_params(n_levels, base_resolution, per_level_scale) for g in grids):
+        raise ValueError(f"every grid must hold {uv_grid_params(n_levels, base_resolution, per_level_scale)} floats")
+    device = grids[0].device
+    if isinstance(appearance_id, torch.Tensor) and appearance_id.is_cuda:
+        if appearance_id.numel() != 1 or appearance_id.is_floating_point():
+            raise ValueError("appearance_id must be one integer")
+        id_dev, host_id = appearance_id.reshape(1).to(device=device, dtype=torch.int64), 0
+    else:
+        id_dev, host_id = None, int(appearance_id)
+        selected = host_id if selected is None else selected
+    if uv is None:
+        if width is None or height is None or int(width) < 2 or int(height) < 2:
+            raise ValueError("the pixel grid needs width and height >= 2")
+        width, height = int(width), int(height)
+    else:
+        uv = _f32c(uv, "uv")
+        if uv.dim() != 2 or uv.shape[1] != 2:
+            raise ValueError("uv must be [n, 2]")
+        width = height = 0
+    if selected is None or not 0 <= selected < len(grids):
+        if torch.is_grad_enabled() and any(g.requires_grad for g in grids):
+            raise ValueError("the grid that receives the gradient is unknown: pass `selected` with a CUDA appearance_id")
+        target = grids[0].detach()
+    else:
+        target = grids[selected]
+    return _UvGridEncode.apply(grid, width, height, uv, _grid_table(grids, device), id_dev, host_id, target)
+
+
+def visibility_supported(feat_dim: int, n_neurons: int, n_layers: int) -> bool:
+    """Whether the visibility MLP kernels take this network (no device needed)."""
+    return int(lib().b200gs_visibility_mlp_workspace_bytes(feat_dim, n_neurons, n_layers)) > 0
+
+
+class _VisibilityMlp(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, enc, *params):
+        n, feat_dim = enc.shape
+        weights, biases = params[0::2], params[1::2]
+        n_layers, n_neurons = len(weights), weights[0].shape[0]
+        m = _lib.B200gsAppearanceMlp(feat_dim, -1, n_neurons, n_layers, 1, 0, 0, 0, weights[0].shape[1], weights[0].shape[1])
+        for l in range(n_layers):
+            m.weights[l], m.biases[l] = weights[l].data_ptr(), biases[l].data_ptr()
+        out = torch.empty(n, dtype=torch.float32, device=enc.device)
+        check(lib().b200gs_visibility_mlp_fwd(ctypes.byref(m), n, ptr(enc), ptr(out), _stream()), "b200gs_visibility_mlp_fwd")
+        ctx.m = m
+        ctx.save_for_backward(enc, *params)
+        return out
+
+    @staticmethod
+    def backward(ctx, v_out):
+        enc, *params = ctx.saved_tensors
+        m, L_ = ctx.m, lib()
+        n, feat_dim = enc.shape
+        ws, bs, total = _appearance_offsets(feat_dim, -1, m.n_neurons, m.n_layers, 1)
+        v_out = _f32c(v_out, "grad")
+        v_enc = torch.empty_like(enc) if ctx.needs_input_grad[0] else None
+        ws_bytes = int(L_.b200gs_visibility_mlp_workspace_bytes(feat_dim, m.n_neurons, m.n_layers))
+        workspace = torch.empty(ws_bytes // 4, dtype=torch.float32, device=enc.device)
+        v_params = torch.empty(total, dtype=torch.float32, device=enc.device)
+        check(L_.b200gs_visibility_mlp_bwd(ctypes.byref(m), n, ptr(enc), ptr(v_out), ptr(v_enc), ptr(workspace), ws_bytes, ptr(v_params),
+                                           _stream()), "b200gs_visibility_mlp_bwd")
+        grads = []
+        for l, ((wo, r, c), (bo, _)) in enumerate(zip(ws, bs)):
+            v_w = v_params[wo:wo + r * c].view(r, c)
+            if l == 0:      # the encoding's columns; the embedding's get theirs through biases[0]
+                full = torch.zeros_like(params[0])
+                full[:, :feat_dim] = v_w
+                v_w = full
+            grads += [v_w, v_params[bo:bo + r]]
+        return (v_enc, *grads)
+
+
+def visibility_mlp(enc, embedding, weights, biases):
+    """The reference's ``visibility_network`` on ``[enc | embedding]`` rows: sigmoid outputs [n].  ``enc`` [n, F] (F = 8, 16, 24 or 32),
+    ``embedding`` [E] the image's transient embedding, ``weights[0]`` [H, F + E].  The embedding is the same for every row, so it is
+    folded into the first bias here (torch, differentiable) and the kernels see F inputs.  Gradients reach enc, the embedding and
+    every weight and bias."""
+    feat_dim, e = enc.shape[1], embedding.shape[0]
+    b0 = torch.addmv(biases[0], weights[0][:, feat_dim:feat_dim + e], embedding)
+    params = []
+    for l, (w, b) in enumerate(zip(weights, biases)):
+        params += [_f32c(w, "weight"), _f32c(b0 if l == 0 else b, "bias")]
+    return _VisibilityMlp.apply(_f32c(enc, "enc"), *params)
+
+
+class _VisibilityLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, image, gt, visibility, mask, lambda_dssim, vis_reg_factor):
+        _, H, W = image.shape
+        L_ = lib()
+        vis_grad = ctx.needs_input_grad[2]
+        nbytes = int(L_.b200gs_vis_loss_workspace_bytes(W, H, int(vis_grad)))
+        ws = torch.empty(nbytes // 4, dtype=torch.float32, device=image.device)
+        with _stage("vis_loss_fwd"):
+            check(L_.b200gs_vis_loss_fwd(W, H, ptr(image), ptr(gt), ptr(visibility), ptr(mask), int(vis_grad), ptr(ws), nbytes, _stream()),
+                  "b200gs_vis_loss_fwd")
+        blocks = int(L_.b200gs_vis_loss_blocks(W, H))
+        sums = ws[nbytes // 4 - 3 * blocks:].view(blocks, 3).sum(dim=0)     # fixed summation order
+        stats = torch.stack([sums[0] / float(3 * H * W), sums[1] / float(3 * H * W), sums[2] * (vis_reg_factor / float(H * W))])
+        loss = (1.0 - lambda_dssim) * stats[0] + lambda_dssim * (1.0 - stats[1]) + stats[2]
+        ctx.save_for_backward(image, gt, visibility, mask, ws)
+        ctx.args = (float(lambda_dssim), float(vis_reg_factor), vis_grad)
+        ctx.mark_non_differentiable(stats)
+        return loss, stats
+
+    @staticmethod
+    def backward(ctx, v_loss, _v_stats):
+        image, gt, visibility, mask, ws = ctx.saved_tensors
+        lambda_dssim, vis_reg_factor, vis_grad = ctx.args
+        _, H, W = image.shape
+        v = _f32c(v_loss.reshape(1), "grad_loss")
+        v_image = torch.empty_like(image)
+        v_vis = torch.empty_like(visibility) if vis_grad else None
+        with _stage("vis_loss_bwd"):
+            check(lib().b200gs_vis_loss_bwd(W, H, ptr(image), ptr(gt), ptr(visibility), ptr(mask), ptr(ws), ws.numel() * 4, lambda_dssim,
+                                            vis_reg_factor, ptr(v), ptr(v_image), ptr(v_vis), _stream()), "b200gs_vis_loss_bwd")
+        return v_image, None, v_vis, None, None, None
+
+
+def visibility_l1_ssim_loss(image, gt, visibility, mask=None, lambda_dssim: float = 0.2, vis_reg_factor: float = 0.2):
+    """``VisibilityMapMetricsImpl.get_train_metrics``' loss of one view in two kernels: with w = visibility * mask,
+    (1 - lambda) mean|w image - w gt| + lambda (1 - SSIM(w image, w gt)) + vis_reg_factor mean((1 - visibility)^2), the SSIM of
+    ``l1_ssim_loss``.  image, gt [3,H,W], visibility [1,H,W] or [H,W], float32 CUDA; mask None or [H,W] / [1,H,W] (bool or uint8,
+    nonzero keeps; a [C,H,W] mask is read at channel 0).  Gradients reach image and visibility (none to gt).  Returns (loss, stats),
+    stats = [mean |a' - b'|, mean SSIM, the weighted regulariser]."""
+    image, gt = _f32c(image, "image"), _f32c(gt, "gt").detach()
+    if image.dim() != 3 or image.shape[0] != 3 or image.shape != gt.shape:
+        raise ValueError(f"image and gt must both be [3,H,W], got {tuple(image.shape)} and {tuple(gt.shape)}")
+    _, H, W = image.shape
+    vis = _f32c(visibility, "visibility")
+    if tuple(vis.shape[-2:]) != (H, W) or vis.numel() != H * W:
+        raise ValueError(f"visibility must be [1,H,W] or [H,W] of the image's size, got {tuple(vis.shape)}")
+    vis = vis.reshape(H, W)
+    if mask is not None:
+        if mask.dim() == 3:
+            mask = mask[0]
+        if tuple(mask.shape) != (H, W) or mask.dtype not in (torch.bool, torch.uint8) or mask.device != image.device:
+            raise ValueError(f"mask must be bool or uint8 [H,W] on the image's device, got {mask.dtype} {tuple(mask.shape)}")
+        mask = (mask != 0).contiguous().view(torch.uint8)
+    return _VisibilityLoss.apply(image, gt, vis, mask, float(lambda_dssim), float(vis_reg_factor))

@@ -216,6 +216,54 @@ B200GS_API int b200gs_appearance_mlp_bwd(const B200gsAppearanceMlp* mlp, int64_t
                                          float* v_features, float* v_raw_opacity, void* workspace, size_t workspace_bytes, float* v_params,
                                          void* stream);
 
+/* ---- Transient visibility map (internal/renderers/gsplat_appearance_embedding_visibility_map_renderer.py, Model.visibility_forward
+ *      :140-157; internal/metrics/visibility_map_metrics.py) ---------------------------------------------------------------------
+ * B200gsUvGrid (host struct): tiny-cuda-nn's 2-D DenseGrid encoding, linear interpolation, 2 features per level:
+ *     n_levels 1..16, base_resolution >= 1, per_level_scale >= 1.  Level l: scale_l = exp2f(l log2f(per_level_scale)) base - 1 (fp32,
+ *     on the host), res_l = ceil(scale_l) + 1, size_l = res_l^2 rounded up to a multiple of 8 vertices of 2 floats; a grid is the
+ *     levels in order (b200gs_uv_grid_params floats; 121760 for 8 / 16 / 1.405).  Coordinate (u, v): pos = fmaf(scale_l, u, 0.5f),
+ *     cell = floor(pos), frac = pos - cell per axis; corners k = 0..3 (bit 0: x) with weight (frac or 1 - frac in x) * (.. in y) at
+ *     vertex ((cell_x + k&1) + (cell_y + k>>1) res_l) % size_l; enc[row, 2 l + f] = the weighted sum in corner order.
+ * b200gs_uv_grid_fwd: enc float[n, 2 n_levels] (8-byte aligned).  uv NULL: the pixel grid of one image, n = width * height rows in
+ *     row-major (y, x) order with u = x / (width - 1), v = y / (height - 1) in fp32 (width, height >= 2); else uv float[n, 2].
+ *     grids: a DEVICE array of n_grids device pointers to grids; the one used is grids[*appearance_id] (int64 read on the device), or
+ *     grids[host_appearance_id] when appearance_id is NULL.  An id outside [0, n_grids) reads no grid and makes enc NaN.
+ * b200gs_uv_grid_bwd: v_params float[b200gs_uv_grid_params] <- the gradient of the selected grid from v_enc, written whole.  Pixel grid:
+ *     one warp per vertex gathers its pixels in a fixed order (no atomics; bit-identical on every call).  uv given: float atomics.
+ * Launches: forward 1 (0 when n == 0), backward 1.
+ * Visibility MLP: the appearance kernels (K20-K22) with one sigmoid output and no epilogue.  mlp->feat_dim = 2 n_levels (a multiple of
+ *     8), n_freq = -1, n_out = 1, normalize = normalize_dirs = epilogue = 0; the transient embedding is folded into biases[0] by the
+ *     caller as for the appearance network.  out float[n]; v_enc float[n, feat_dim] (16-byte aligned, NULL: not computed); v_params
+ *     as b200gs_appearance_mlp_bwd's.  b200gs_visibility_mlp_workspace_bytes: 0 for shapes the kernels do not take.
+ * b200gs_vis_loss_fwd: the masked L1 + SSIM of VisibilityMapMetricsImpl.get_train_metrics on image, gt float[3, H, W], visibility
+ *     float[H, W] and mask (NULL or uint8[H, W], 0 or 1), all contiguous: a' = w image, b' = w gt with w = visibility * mask, the SSIM
+ *     of b200gs_loss_fwd.  Writes the derivative maps and partials[b200gs_vis_loss_blocks][3] = per-CTA sums of |a' - b'|, SSIM and
+ *     (1 - visibility)^2 into the workspace (maps first, then partials; b200gs_vis_loss_workspace_bytes).  vis_grad: also the map the
+ *     visibility gradient needs.
+ * b200gs_vis_loss_bwd: with loss = (1 - lambda) mean|a' - b'| + lambda (1 - mean SSIM) + vis_reg_factor mean((1 - visibility)^2):
+ *     v_image <- (*v_loss or 1) d loss / d image; v_visibility (NULL: not computed; needs vis_grad in the forward) <- d loss / d
+ *     visibility, the three channels summed in the CTA.  Launches: forward 1, backward 1.  No atomics. */
+typedef struct B200gsUvGrid {
+    int32_t n_levels, base_resolution;
+    float per_level_scale;
+} B200gsUvGrid;
+B200GS_API int64_t b200gs_uv_grid_params(const B200gsUvGrid* grid);
+B200GS_API int b200gs_uv_grid_fwd(const B200gsUvGrid* grid, int32_t width, int32_t height, const float* uv, int64_t n, const float* const* grids,
+                                  int32_t n_grids, const int64_t* appearance_id, int64_t host_appearance_id, float* enc, void* stream);
+B200GS_API int b200gs_uv_grid_bwd(const B200gsUvGrid* grid, int32_t width, int32_t height, const float* uv, int64_t n, const float* v_enc,
+                                  float* v_params, void* stream);
+B200GS_API size_t b200gs_visibility_mlp_workspace_bytes(int32_t feat_dim, int32_t n_neurons, int32_t n_layers);
+B200GS_API int b200gs_visibility_mlp_fwd(const B200gsAppearanceMlp* mlp, int64_t n, const float* enc, float* out, void* stream);
+B200GS_API int b200gs_visibility_mlp_bwd(const B200gsAppearanceMlp* mlp, int64_t n, const float* enc, const float* v_out, float* v_enc,
+                                         void* workspace, size_t workspace_bytes, float* v_params, void* stream);
+B200GS_API int64_t b200gs_vis_loss_blocks(int32_t width, int32_t height);
+B200GS_API size_t b200gs_vis_loss_workspace_bytes(int32_t width, int32_t height, int32_t vis_grad);
+B200GS_API int b200gs_vis_loss_fwd(int32_t width, int32_t height, const float* image, const float* gt, const float* visibility,
+                                   const uint8_t* mask, int32_t vis_grad, void* workspace, size_t workspace_bytes, void* stream);
+B200GS_API int b200gs_vis_loss_bwd(int32_t width, int32_t height, const float* image, const float* gt, const float* visibility,
+                                   const uint8_t* mask, const void* workspace, size_t workspace_bytes, float lambda_dssim,
+                                   float vis_reg_factor, const float* v_loss, float* v_image, float* v_visibility, void* stream);
+
 /* ---- Learned exposure correction (internal/output_processors/exposure.py, ExposureProcessorModule.forward :112-143) ------------
  * b200gs_exposure_fwd: one view's colour transform.  render and out are float[3,H,W] addressed as base[c sc + y sy + x sx] (element
  *     strides, so the permuted [H,W,3] render of the v1 and appearance renderers needs no copy); channels must be 3.
