@@ -82,6 +82,9 @@ _SIGNATURES = {
     "b200gs_depth_loss_workspace_bytes": (c_size_t, [c_int32] * 3),
     "b200gs_depth_loss_fwd": (c_int32, [c_int32] * 2 + [_P] * 3 + [c_int64] * 2 + [c_int32] * 2 + [c_float] * 2 + [_P, c_size_t, _P, _P, _P]),
     "b200gs_depth_loss_bwd": (c_int32, [c_int32] * 2 + [_P] * 3 + [c_int64] * 2 + [c_int32] * 2 + [c_float] * 2 + [_P, c_size_t, _P, _P, _P]),
+    "b200gs_gaussian_reg_workspace_bytes": (c_size_t, [c_int64]),
+    "b200gs_gaussian_reg_fwd": (c_int32, [c_int64, _P, _P, c_int32] + [c_float] * 6 + [_P, c_size_t, _P, _P, _P]),
+    "b200gs_gaussian_reg_bwd": (c_int32, [c_int64, _P, _P, c_int32] + [c_float] * 6 + [_P, c_size_t, _P, _P, _P, _P]),
     "b200gs_knn_workspace_bytes": (c_size_t, [c_int64]),
     "b200gs_knn_mean_dist2": (c_int32, [c_int64, _P, _P, _P, c_size_t, _P]),
     "b200gs_sh_fwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P]),

@@ -42,7 +42,7 @@ using namespace b200gs;
 extern "C" {
 
 const char* b200gs_last_error(void) { return g_error; }
-int b200gs_version(void) { return 230; }
+int b200gs_version(void) { return 231; }
 int64_t b200gs_launch_count(void) { return (int64_t)g_launches.load(std::memory_order_relaxed); }
 
 int b200gs_project_fwd(const B200gsView* view, int64_t n, const float* means, const float* scales, const float* quats,
@@ -603,6 +603,50 @@ int b200gs_depth_loss_bwd(int32_t height, int32_t width, const float* pred, cons
     B200GS_CHECK_ARG(v_pred, "NULL pointer");
     return launch_depth_loss_bwd(height, width, pred, gt, mask, mask_sy, mask_sx, loss_type, norm, median, ssim_weight,
                                  static_cast<const float*>(workspace), v_loss, v_pred, (cudaStream_t)stream);
+}
+
+static bool gaussian_reg_size_ok(int64_t n) { return n >= 1 && n <= INT32_MAX; }
+
+size_t b200gs_gaussian_reg_workspace_bytes(int64_t n) { return gaussian_reg_size_ok(n) ? gaussian_reg_workspace_bytes(n) : 0; }
+
+// shared by the forward and the backward; returns the error code, or 0 when the arguments are valid
+static int check_gaussian_reg(const char* fn, int64_t n, const float* opacities, const float* scales, int32_t flags, bool stats,
+                              const void* workspace, size_t workspace_bytes) {
+    auto fail = [&](const char* msg) { set_error("%s: %s", fn, msg); return B200GS_EINVAL; };
+    constexpr int32_t all = B200GS_GREG_RAW | B200GS_GREG_OPACITY | B200GS_GREG_SCALE | B200GS_GREG_OVER_SCALE | B200GS_GREG_OVER_RATIO;
+    if (n < 1) return fail("n must be >= 1");
+    if (!gaussian_reg_size_ok(n)) return fail("n too large (> 2^31 - 1)");
+    if (flags & ~all) return fail("unknown flags");
+    if ((flags & B200GS_GREG_OPACITY) && !opacities) return fail("NULL pointer: opacities");
+    if (((flags & (B200GS_GREG_SCALE | B200GS_GREG_OVER_SCALE | B200GS_GREG_OVER_RATIO)) || stats) && !scales)
+        return fail("NULL pointer: scales");
+    if (!workspace) return fail("NULL pointer: workspace");
+    if (workspace_bytes < gaussian_reg_workspace_bytes(n)) {
+        set_error("%s: workspace too small", fn);
+        return B200GS_ENOSPACE;
+    }
+    return 0;
+}
+
+int b200gs_gaussian_reg_fwd(int64_t n, const float* opacities, const float* scales, int32_t flags, float opacity_weight, float scale_weight,
+                            float max_scale, float max_scale_ratio, float scale_lambda, float ratio_lambda, void* workspace,
+                            size_t workspace_bytes, float* terms, float* stats, void* stream) {
+    if (int rc = check_gaussian_reg(__func__, n, opacities, scales, flags, stats != nullptr, workspace, workspace_bytes)) return rc;
+    B200GS_CHECK_ARG(terms, "NULL pointer: terms");
+    return launch_gaussian_reg_fwd(n, opacities, scales, flags, opacity_weight, scale_weight, max_scale, max_scale_ratio, scale_lambda,
+                                   ratio_lambda, static_cast<float*>(workspace), terms, stats, (cudaStream_t)stream);
+}
+
+int b200gs_gaussian_reg_bwd(int64_t n, const float* opacities, const float* scales, int32_t flags, float opacity_weight, float scale_weight,
+                            float max_scale, float max_scale_ratio, float scale_lambda, float ratio_lambda, const void* workspace,
+                            size_t workspace_bytes, const float* v_terms, float* v_opacities, float* v_scales, void* stream) {
+    if (int rc = check_gaussian_reg(__func__, n, opacities, scales, flags, false, workspace, workspace_bytes)) return rc;
+    B200GS_CHECK_ARG(v_terms, "NULL pointer: v_terms");
+    B200GS_CHECK_ARG(!opacities || v_opacities, "NULL pointer: v_opacities");
+    B200GS_CHECK_ARG(!scales || v_scales, "NULL pointer: v_scales");
+    return launch_gaussian_reg_bwd(n, opacities, scales, flags, opacity_weight, scale_weight, max_scale, max_scale_ratio, scale_lambda,
+                                   ratio_lambda, static_cast<const float*>(workspace), v_terms, opacities ? v_opacities : nullptr,
+                                   scales ? v_scales : nullptr, (cudaStream_t)stream);
 }
 
 size_t b200gs_knn_workspace_bytes(int64_t n) { return n < 0 ? 0 : knn_workspace_bytes(n); }

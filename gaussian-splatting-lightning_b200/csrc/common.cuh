@@ -196,6 +196,15 @@ int launch_depth_loss_bwd(int height, int width, const float* pred, const float*
                           int loss_type, int norm, float median, float w, const float* ws, const float* v_loss, float* v_pred,
                           cudaStream_t st);
 
+// Gaussian regularisers (gauss_reg.cu): opacities [n,1] and scales [n,3] contiguous, either NULL when no term reads it; flags of
+// b200gs.h.  The backward reads the coefficients its forward wrote to the workspace.
+size_t gaussian_reg_workspace_bytes(int64_t n);
+int launch_gaussian_reg_fwd(int64_t n, const float* opac, const float* scales, int flags, float w_o, float w_s, float max_scale,
+                            float max_ratio, float lam, float lam_r, float* ws, float* terms, float* stats, cudaStream_t st);
+int launch_gaussian_reg_bwd(int64_t n, const float* opac, const float* scales, int flags, float w_o, float w_s, float max_scale,
+                            float max_ratio, float lam, float lam_r, const float* ws, const float* v_terms, float* v_opac,
+                            float* v_scales, cudaStream_t st);
+
 // appearance MLP (appearance.cu); the shape arguments are those of B200gsAppearanceMlp, validated by the caller
 bool appearance_mlp_fits(int feat_dim, int n_freq, int n_neurons, int n_layers, int n_out);
 size_t appearance_mlp_workspace_bytes(int feat_dim, int n_freq, int n_neurons, int n_layers, int n_out);

@@ -1,4 +1,5 @@
-"""Training metrics (the reference's ``internal/metrics/vanilla_metrics.py`` and ``inverse_depth_metrics.py``) on the b200gs kernels.
+"""Training metrics (the reference's ``internal/metrics/vanilla_metrics.py``, ``inverse_depth_metrics.py``, ``mcmc_metrics.py`` and
+``scale_regularization_metrics.py``) on the b200gs kernels.
 Select them as the model's metric:
 
     model:
@@ -10,10 +11,12 @@ Select them as the model's metric:
 ``fused_ssim`` settings.  ``B200InverseDepthMetrics`` has ``HasInverseDepthMetrics``' fields, defaults and ``WeightScheduler``, and its
 module the same methods, output keys and progress-bar flags; the depth loss is ``inverse_depth_loss``: four kernel launches forward,
 one backward, no host synchronisation.  PSNR and LPIPS for validation stay torchmetrics objects, created in ``setup`` when
-torchmetrics imports.
+torchmetrics imports.  ``B200MCMCMetrics``, ``B200ScaleRegularizationMetrics`` and ``B200ScaleRegularizationWithDepthMetrics`` have
+``MCMCMetrics``', ``ScaleRegularizationMetrics``' and ``ScaleRegularizationWithDepthMetrics``' fields, defaults, output keys and
+progress-bar flags; their per-Gaussian terms are ``gaussian_regularizers``: two kernel launches forward, one backward.
 """
 from dataclasses import dataclass, field
-from typing import Literal
+from typing import Literal, Optional
 
 import torch
 
@@ -107,6 +110,92 @@ def inverse_depth_loss(gt, pred, *, loss_type="l1", ssim_weight=0.2, normalized=
     norm = 1 if normalized else (2 if median is not None else (3 if mean_normalization else 0))
     return _InverseDepthLoss.apply(pred.contiguous(), gt.detach().contiguous(), mask, _LOSS_TYPES[loss_type], norm,
                                    float(median) if norm == 2 else 0.0, float(ssim_weight))
+
+
+GAUSSIAN_REG_FWD_LAUNCHES = 2   # library launches of one gaussian_regularizers forward: per-CTA partials, reduce
+GAUSSIAN_REG_BWD_LAUNCHES = 1   # and of its backward
+_GREG_RAW, _GREG_OPACITY, _GREG_SCALE, _GREG_OVER_SCALE, _GREG_OVER_RATIO = 1, 2, 4, 8, 16
+
+
+class _GaussianRegularizers(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, opacities, scales, flags, args, statistics):
+        n = (opacities if opacities is not None else scales).shape[0]
+        dev = (opacities if opacities is not None else scales).device
+        L = lib()
+        nbytes = int(L.b200gs_gaussian_reg_workspace_bytes(n))
+        ws = torch.empty(nbytes // 4, dtype=torch.float32, device=dev)
+        terms = torch.empty(4, dtype=torch.float32, device=dev)
+        stats = torch.empty(5, dtype=torch.float32, device=dev) if statistics else None
+        check(L.b200gs_gaussian_reg_fwd(n, ptr(opacities), ptr(scales), flags, *args, ptr(ws), nbytes, ptr(terms), ptr(stats), _stream()),
+              "b200gs_gaussian_reg_fwd")
+        ctx.save_for_backward(opacities, scales, ws)
+        ctx.args = (flags, args)
+        if stats is None:
+            return terms
+        ctx.mark_non_differentiable(stats)
+        return terms, stats
+
+    @staticmethod
+    def backward(ctx, v_terms, *_v_stats):
+        opacities, scales, ws = ctx.saved_tensors
+        flags, args = ctx.args
+        n = (opacities if opacities is not None else scales).shape[0]
+        v = v_terms.to(torch.float32).contiguous()
+        v_o = torch.empty_like(opacities) if opacities is not None else None
+        v_s = torch.empty_like(scales) if scales is not None else None
+        check(lib().b200gs_gaussian_reg_bwd(n, ptr(opacities), ptr(scales), flags, *args, ptr(ws), ws.numel() * 4, ptr(v), ptr(v_o),
+                                            ptr(v_s), _stream()), "b200gs_gaussian_reg_bwd")
+        return v_o, v_s, None, None, None
+
+
+def gaussian_regularizers(opacities, scales, *, raw, opacity_weight=0.0, scale_weight=0.0, max_scale=-1.0, max_scale_ratio=10.0,
+                          scale_lambda=0.0, ratio_lambda=0.0, statistics=True):
+    """The per-Gaussian regularisers of ``MCMCMetrics`` and ``ScaleRegularizationMetrics`` in one fused pass (K36/K37, backward
+    K38): opacities float32 CUDA [N,1] and scales [N,3], either None when no term reads it.  ``raw``: they are the logits and
+    log-scales and the kernels apply torch's fp32 sigmoid / exp; otherwise they are the activated values (the getters' output).
+    Returns (terms, stats), or terms alone with ``statistics=False``:
+        terms [4] = [opacity_weight mean|o|, scale_weight mean|s|, scale_lambda sum(s [s > max_scale]) / (n_s + 1),
+                     ratio_lambda sum(r [r > max_scale_ratio]) / (n_r + 1)],   r = max / (mid + 1e-8) of each sorted row
+        stats [5] = [n_s, n_r, max of the largest scale, max r, mean r]        (not differentiable; needs scales)
+    A term whose weight is 0 (or whose tensor is None) is an exact 0 and adds nothing to the gradient.  Gradients go to the
+    tensors passed.  Tied scales are ranked as torch.sort ranks them on the GPU (csrc/gauss_reg.cu's table)."""
+    t = opacities if opacities is not None else scales
+    if t is None:
+        raise ValueError("gaussian_regularizers needs opacities or scales")
+    n = t.shape[0]
+    if n == 0:
+        raise ValueError("gaussian_regularizers needs at least one Gaussian")
+    if opacities is not None and (opacities.dim() != 2 or opacities.shape[1] != 1):
+        raise ValueError(f"opacities must be [N, 1], got {tuple(opacities.shape)}")
+    if scales is not None and (scales.dim() != 2 or scales.shape[1] != 3):
+        raise ValueError(f"scales must be [N, 3], got {tuple(scales.shape)}")
+    if opacities is not None and scales is not None and opacities.shape[0] != scales.shape[0]:
+        raise ValueError(f"opacities and scales hold {opacities.shape[0]} and {scales.shape[0]} Gaussians")
+    if any(x is not None and (x.dtype != torch.float32 or not x.is_cuda) for x in (opacities, scales)):
+        raise ValueError("opacities and scales must be float32 CUDA tensors")
+    if statistics and scales is None:
+        raise ValueError("the statistics need the scales")
+    flags = _GREG_RAW if raw else 0
+    if opacities is not None:
+        flags |= _GREG_OPACITY
+        opacities = opacities.contiguous()
+    if scales is not None:
+        flags |= _GREG_SCALE | _GREG_OVER_SCALE | _GREG_OVER_RATIO
+        scales = scales.contiguous()
+    args = tuple(float(a) for a in (opacity_weight, scale_weight, max_scale, max_scale_ratio, scale_lambda, ratio_lambda))
+    return _GaussianRegularizers.apply(opacities, scales, flags, args, bool(statistics))
+
+
+def _regularized_parameters(gaussian_model, opacities: bool, scales_getter):
+    """(opacities or None, scales or None, raw): the raw parameters of a vanilla model that is not pre-activated
+    (``renderers._raw_parameters``' rule), activated in the kernels; any other model's getters, which autograd chains.
+    ``scales_getter`` None: no scales."""
+    from .renderers import _raw_parameters
+    params = None if getattr(gaussian_model, "is_pre_activated", False) else _raw_parameters(gaussian_model)
+    if params is not None:
+        return (params["opacities"] if opacities else None), (params["scales"] if scales_getter else None), True
+    return ((gaussian_model.get_opacity if opacities else None), (scales_getter(gaussian_model) if scales_getter else None), False)
 
 
 def _torchmetrics():
@@ -321,3 +410,152 @@ def fused_ssim(img1, img2, padding="same", train=True):
         raise ValueError(f"fused_ssim takes two [1,C,H,W] images, got {tuple(img1.shape)} and {tuple(img2.shape)}")
     loss, stats = ops.l1_ssim_loss(img1[0], img2[0].detach(), 1.0)     # loss = 1 - SSIM, K10's gradient
     return stats[1] - (loss - loss.detach())
+
+
+# ---- MCMCMetrics and ScaleRegularization*Metrics (internal/metrics/mcmc_metrics.py, scale_regularization_metrics.py) -------------
+_SCALE_KEYS = ("scale_reg", "scale_ratio_reg", "n_over_scales", "n_over_ratios", "max_scale", "max_ratio", "mean_ratio")
+
+
+@dataclass
+class B200MCMCMetricsMixin:
+    mcmc_reg_until_iter: int = -1
+
+    opacity_reg: float = 0.01
+
+    scale_reg: float = 0.01
+
+    reg_weight_decay: float = 1.
+
+
+class B200MCMCMetricsModuleMixin:
+    """The MCMC regularisers: ``opacity_reg`` mean|get_opacity| and ``scale_reg`` mean|get_scaling|, both weights divided by
+    ``reg_weight_decay`` capped at 5; the scale term is added only with a positive weight.  In training they stop at step
+    ``mcmc_reg_until_iter`` when that is not negative; validation always reports them.  Keys ``o_reg`` and ``s_reg``, off the
+    progress bar."""
+
+    def setup(self, *args, **kwargs):
+        super().setup(*args, **kwargs)
+        divisor = min(self.config.reg_weight_decay, 5.)
+        self.opacity_reg_weight, self.scale_reg_weight = self.config.opacity_reg / divisor, self.config.scale_reg / divisor
+
+    def _mcmc_terms_apply(self, step: int) -> bool:
+        until = self.config.mcmc_reg_until_iter
+        return until < 0 or step < until
+
+    def reg_loss(self, gaussian_model, basic_metrics):
+        metrics, pbar = basic_metrics
+        with_scale = self.scale_reg_weight > 0
+        opacities, scales, raw = _regularized_parameters(gaussian_model, True, (lambda m: m.get_scaling) if with_scale else None)
+        terms = gaussian_regularizers(opacities, scales, raw=raw, opacity_weight=self.opacity_reg_weight,
+                                      scale_weight=self.scale_reg_weight if with_scale else 0.0, statistics=False)
+        metrics["loss"] = metrics["loss"] + terms[0] + terms[1]
+        metrics["o_reg"], metrics["s_reg"] = terms[0], terms[1]
+        pbar["o_reg"] = pbar["s_reg"] = False
+        return metrics, pbar
+
+    def get_train_metrics(self, pl_module, gaussian_model, step: int, batch, outputs):
+        result = super().get_train_metrics(pl_module, gaussian_model, step, batch, outputs)
+        return self.reg_loss(gaussian_model, result) if self._mcmc_terms_apply(step) else result
+
+    def get_validate_metrics(self, pl_module, gaussian_model, batch, outputs):
+        return self.reg_loss(gaussian_model, super().get_validate_metrics(pl_module, gaussian_model, batch, outputs))
+
+
+@dataclass
+class B200MCMCMetrics(B200MCMCMetricsMixin, B200VanillaMetrics):
+    def instantiate(self, *args, **kwargs) -> "B200MCMCMetricsModule":
+        self._check()
+        return B200MCMCMetricsModule(self)
+
+
+class B200MCMCMetricsModule(B200MCMCMetricsModuleMixin, B200VanillaMetricsModule):
+    pass
+
+
+@dataclass
+class B200ScaleRegularizationMetricsMixin:
+    """Fields of the over-scale / over-ratio regularisers.  ``max_scale`` <= 0 is resolved in ``setup``; the configuration is
+    rejected when ``scale_reg_from`` is negative, or when the ratio term is on (``scale_ratio_reg_lambda`` > 0) with a ratio
+    threshold that is not positive."""
+
+    scale_reg_from: int = 3100
+
+    max_scale: float = -1
+
+    max_scale_outside_partition: Optional[float] = None
+
+    max_scale_ratio: float = 10
+
+    scale_reg_lambda: float = 0.05
+
+    scale_ratio_reg_lambda: float = 0.05
+
+    def __post_init__(self):
+        # no base of these configs defines __post_init__, so there is nothing to chain to
+        assert self.scale_reg_from >= 0, f"scale_reg_from must not be negative, got {self.scale_reg_from}"
+        assert self.scale_ratio_reg_lambda <= 0. or self.max_scale_ratio > 0, \
+            f"max_scale_ratio must be positive when the ratio term is on, got {self.max_scale_ratio}"
+
+    def _check(self):
+        super()._check()
+        if self.max_scale_outside_partition is not None:
+            raise NotImplementedError("max_scale_outside_partition needs the partition store's distance_factors, which is not provided")
+
+
+class B200ScaleRegularizationMetricsModuleMixin:
+    """The over-scale and over-ratio regularisers of get_scales() with their statistics: added in training from step
+    ``scale_reg_from`` on and always in validation.  A term whose lambda is not positive is a device 0, and so is its count; the
+    ratio statistics are reported whatever ``scale_ratio_reg_lambda`` is.  The loss grows as (basic [+ d_reg]) + scale_reg +
+    scale_ratio_reg.  Keys in _SCALE_KEYS, off the progress bar."""
+
+    def setup(self, stage: str, pl_module):
+        super().setup(stage, pl_module)
+        c = self.config
+        if stage == "fit" and c.max_scale <= 0:
+            extent = pl_module.trainer.datamodule.dataparser_outputs.camera_extent
+            c.max_scale = extent * 1.1
+            assert c.max_scale > 0., f"the camera extent gives max_scale {c.max_scale}"
+
+    def get_scale_regularization_metrics(self, gaussian_model, pl_module, metrics, pbar):
+        c = self.config
+        positive = lambda v: v if v > 0. else 0.0      # noqa: E731
+        _, scales, raw = _regularized_parameters(gaussian_model, False, lambda m: m.get_scales())
+        terms, stats = gaussian_regularizers(None, scales, raw=raw, max_scale=c.max_scale, max_scale_ratio=c.max_scale_ratio,
+                                             scale_lambda=positive(c.scale_reg_lambda), ratio_lambda=positive(c.scale_ratio_reg_lambda))
+        metrics["loss"] = metrics["loss"] + terms[2] + terms[3]
+        for key, value in zip(_SCALE_KEYS, (terms[2], terms[3], *stats.unbind())):
+            metrics[key] = value
+            pbar[key] = False
+
+    def get_train_metrics(self, pl_module, gaussian_model, step: int, batch, outputs):
+        metrics, pbar = super().get_train_metrics(pl_module, gaussian_model, step, batch, outputs)
+        if step >= self.config.scale_reg_from:
+            self.get_scale_regularization_metrics(gaussian_model, pl_module, metrics, pbar)
+        return metrics, pbar
+
+    def get_validate_metrics(self, pl_module, gaussian_model, batch, outputs):
+        metrics, pbar = super().get_validate_metrics(pl_module, gaussian_model, batch, outputs)
+        self.get_scale_regularization_metrics(gaussian_model, pl_module, metrics, pbar)
+        return metrics, pbar
+
+
+@dataclass
+class B200ScaleRegularizationMetrics(B200ScaleRegularizationMetricsMixin, B200VanillaMetrics):
+    def instantiate(self, *args, **kwargs) -> "B200ScaleRegularizationMetricsModule":
+        self._check()
+        return B200ScaleRegularizationMetricsModule(self)
+
+
+class B200ScaleRegularizationMetricsModule(B200ScaleRegularizationMetricsModuleMixin, B200VanillaMetricsModule):
+    pass
+
+
+@dataclass
+class B200ScaleRegularizationWithDepthMetrics(B200ScaleRegularizationMetricsMixin, B200InverseDepthMetrics):
+    def instantiate(self, *args, **kwargs) -> "B200ScaleRegularizationWithDepthMetricsModule":
+        self._check()
+        return B200ScaleRegularizationWithDepthMetricsModule(self)
+
+
+class B200ScaleRegularizationWithDepthMetricsModule(B200ScaleRegularizationMetricsModuleMixin, B200InverseDepthMetricsModule):
+    pass

@@ -322,6 +322,41 @@ B200GS_API int b200gs_depth_loss_bwd(int32_t height, int32_t width, const float*
                                      int64_t mask_sy, int64_t mask_sx, int32_t loss_type, int32_t norm, float median, float ssim_weight,
                                      const void* workspace, size_t workspace_bytes, const float* v_loss, float* v_pred, void* stream);
 
+/* ---- Gaussian regularisers (internal/metrics/mcmc_metrics.py:39-59, MCMCMetricsModuleMixin.reg_loss, and
+ *      internal/metrics/scale_regularization_metrics.py:51-115, get_scale_regularization_metrics) --------------------------------
+ * b200gs_gaussian_reg_fwd: opacities float[n,1] and scales float[n,3] contiguous: with B200GS_GREG_RAW the logits and log-scales
+ *     (activated here as torch's fp32 sigmoid and exp), otherwise the activated values (get_opacity / get_scales()).  Writes
+ *     terms[0..3] = [opacity_weight mean|o|                                         (mcmc_metrics.py:42, flag OPACITY)
+ *                    scale_weight mean|s|                                           (mcmc_metrics.py:46, flag SCALE)
+ *                    scale_lambda sum(s [s > max_scale]) / (n_s + 1)                 (scale_regularization_metrics.py:74-82, OVER_SCALE)
+ *                    ratio_lambda sum(r [r > max_scale_ratio]) / (n_r + 1)]          (scale_regularization_metrics.py:84-90, OVER_RATIO)
+ *     with n_s = #{s > max_scale} elementwise, r = max / (mid + 1e-8) of each row sorted ascending (tied values routed as torch.sort
+ *     routes them on the GPU, a table measured on an H100: it decides which column takes the "mid" gradient), both thresholds strict.  A term whose flag is clear or whose weight is 0 is 0.  stats NULL
+ *     or float[5] <- [n_s, n_r, max of the largest scale, max r, mean r] (scale_regularization_metrics.py:92-98; n_s / n_r are 0
+ *     when their term is off).  opacities may be NULL when OPACITY is clear, scales when no scale flag is set and stats is NULL.
+ * b200gs_gaussian_reg_bwd: v_opacities float[n,1] (when opacities is given) and v_scales float[n,3] (when scales is given) <-
+ *     sum_k v_terms[k] d terms[k] / d input, dense, exact zeros wherever no term applies (torch.abs' subgradient at 0 is 0); with
+ *     RAW chained through the activations as torch does (y (1 - y) and y from the fp32 output).  v_terms float[4] is read on the
+ *     device.  It reads the coefficients its forward wrote to the workspace, and takes the same arguments.  No float atomics: two
+ *     calls give bit-identical results.
+ * b200gs_gaussian_reg_workspace_bytes: device scratch shared by the forward and the backward; 0 for n < 1 or n > 2^31 - 1.
+ * Launches: forward 2 (per-CTA partials, reduce), backward 1.  No host synchronisation.
+ * Algorithmic bytes: forward 16 in per Gaussian (4 without the scale terms and statistics, 12 without the opacity term); backward
+ *     16 in + 16 out per Gaussian. */
+#define B200GS_GREG_RAW 1
+#define B200GS_GREG_OPACITY 2
+#define B200GS_GREG_SCALE 4
+#define B200GS_GREG_OVER_SCALE 8
+#define B200GS_GREG_OVER_RATIO 16
+B200GS_API size_t b200gs_gaussian_reg_workspace_bytes(int64_t n);
+B200GS_API int b200gs_gaussian_reg_fwd(int64_t n, const float* opacities, const float* scales, int32_t flags, float opacity_weight,
+                                       float scale_weight, float max_scale, float max_scale_ratio, float scale_lambda, float ratio_lambda,
+                                       void* workspace, size_t workspace_bytes, float* terms, float* stats, void* stream);
+B200GS_API int b200gs_gaussian_reg_bwd(int64_t n, const float* opacities, const float* scales, int32_t flags, float opacity_weight,
+                                       float scale_weight, float max_scale, float max_scale_ratio, float scale_lambda, float ratio_lambda,
+                                       const void* workspace, size_t workspace_bytes, const float* v_terms, float* v_opacities,
+                                       float* v_scales, void* stream);
+
 /* b200gs_knn_mean_dist2: simple_knn's distCUDA2 (vanilla_gaussian.py:122-125, the scale initialiser): mean_dist2[i] = mean of the squared
  *     distances from points[i] (float[n,3]) to its 3 nearest neighbours (exact).  Synchronises the stream once (the hash grid is sized
  *     on the host from the bounding box); init-time only. */
