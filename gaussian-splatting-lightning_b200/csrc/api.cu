@@ -808,23 +808,37 @@ int b200gs_publish_i64(const int64_t* d_values, int64_t* host_values, int32_t n,
     return publish_i64(d_values, host_values, n, (cudaStream_t)stream);
 }
 
-// ---- fused L1 + SSIM loss (experimental) ----------------------------------------------------------------------------------
+// ---- fused L1 + SSIM loss -----------------------------------------------------------------------------------------------------
+// the grid is (ceil(W/16), ceil(H/16), C): C and ceil(H/16) are at most 65535, and ceil(W/16) is computed in int
+static bool loss_size_ok(int32_t channels, int32_t width, int32_t height) {
+    return channels >= 1 && width >= 1 && height >= 1 && channels <= 65535 && height <= 65535 * 16 && width <= INT32_MAX - 15;
+}
+
 int64_t b200gs_loss_blocks(int32_t channels, int32_t width, int32_t height) {
-    if (channels <= 0 || width <= 0 || height <= 0) return 0;
-    return loss_blocks(channels, width, height);
+    return loss_size_ok(channels, width, height) ? loss_blocks(channels, width, height) : 0;
+}
+
+// shared by the forward and the backward; returns the error code, or 0 when the arguments are valid
+static int check_loss(const char* fn, int32_t channels, int32_t width, int32_t height, const void* image, const void* target,
+                      const void* maps, const void* out) {
+    auto fail = [&](const char* msg) { set_error("%s: %s", fn, msg); return B200GS_EINVAL; };
+    if (channels < 1 || width < 1 || height < 1) return fail("bad size: channels, width and height must be >= 1");
+    if (channels > 65535) return fail("too many channels (> 65535)");
+    if (height > 65535 * 16) return fail("image too tall (height > 65535 * 16)");
+    if (width > INT32_MAX - 15) return fail("image too wide (width > 2^31 - 16)");
+    if (!(image && target && maps && out)) return fail("NULL pointer");
+    return 0;
 }
 
 int b200gs_loss_fwd(int32_t channels, int32_t width, int32_t height, const float* image, const float* target, float* dmaps,
                     float* partials, void* stream) {
-    B200GS_CHECK_ARG(channels > 0 && width > 0 && height > 0, "bad size");
-    B200GS_CHECK_ARG(image && target && dmaps && partials, "NULL pointer");
+    if (int rc = check_loss(__func__, channels, width, height, image, target, dmaps, partials)) return rc;
     return launch_loss_fwd(channels, width, height, image, target, dmaps, partials, (cudaStream_t)stream);
 }
 
 int b200gs_loss_bwd(int32_t channels, int32_t width, int32_t height, const float* image, const float* target, const float* dmaps,
                     float lambda_dssim, const float* v_loss, float* v_image, void* stream) {
-    B200GS_CHECK_ARG(channels > 0 && width > 0 && height > 0, "bad size");
-    B200GS_CHECK_ARG(image && target && dmaps && v_image, "NULL pointer");
+    if (int rc = check_loss(__func__, channels, width, height, image, target, dmaps, v_image)) return rc;
     return launch_loss_bwd(channels, width, height, image, target, dmaps, lambda_dssim, v_loss, v_image, (cudaStream_t)stream);
 }
 

@@ -501,7 +501,10 @@ B200GS_API int b200gs_blend_feat_bwd(int32_t width, int32_t height, int32_t chan
  * internal/utils/ssim.py:17-63: 11-tap Gaussian window sigma 1.5, zero padding, C1 = 0.01^2, C2 = 0.03^2).  image/target [C,H,W].
  * b200gs_loss_fwd: partials[b200gs_loss_blocks(...)][2] <- per-CTA sums of |image-target| and of the SSIM map (the caller sums them
  *     and divides by C*H*W); dmaps[3][C][H][W] <- partial derivatives of the SSIM map, kept for the backward.
- * b200gs_loss_bwd: v_image[C,H,W] <- (*v_loss or 1) * dloss/dimage. */
+ * b200gs_loss_bwd: v_image[C,H,W] <- (*v_loss or 1) * dloss/dimage.
+ * Sizes: 1 <= channels <= 65535, 1 <= height <= 65535 * 16 and 1 <= width <= 2^31 - 16 (the launch grid is ceil(W/16) x ceil(H/16)
+ * x C); fwd and bwd return B200GS_EINVAL for other sizes or a NULL pointer (v_loss may be NULL) before any CUDA call, and
+ * b200gs_loss_blocks returns 0 for them. */
 B200GS_API int64_t b200gs_loss_blocks(int32_t channels, int32_t width, int32_t height);
 B200GS_API int b200gs_loss_fwd(int32_t channels, int32_t width, int32_t height, const float* image, const float* target, float* dmaps,
                                float* partials, void* stream);
