@@ -84,6 +84,11 @@ def install(force: bool = False):
         sys.modules["tinycudann"] = _tcnn_module()
     elif "tinycudann" not in sys.modules and not any(isinstance(f, _OnImport) and f.name == "tinycudann" for f in sys.meta_path):
         sys.meta_path.insert(0, _OnImport("tinycudann", _tcnn_module))
+    # gsplat.utils.depth_to_normal (internal/metrics/normal_reg.py:3, VanillaWithNormalRegMetrics), the same way
+    if force:
+        sys.modules["gsplat.utils"] = _gsplat_utils_module()
+    elif "gsplat.utils" not in sys.modules and not any(isinstance(f, _OnImport) and f.name == "gsplat.utils" for f in sys.meta_path):
+        sys.meta_path.insert(0, _OnImport("gsplat.utils", _gsplat_utils_module))
 
 
 def _fused_ssim_module():
@@ -91,6 +96,13 @@ def _fused_ssim_module():
     fs = types.ModuleType("fused_ssim")
     fs.fused_ssim = metrics.fused_ssim
     return fs
+
+
+def _gsplat_utils_module():
+    from .. import metrics
+    m = types.ModuleType("gsplat.utils")
+    m.depth_to_normal = metrics.depth_to_normal
+    return m
 
 
 def _tcnn_module():

@@ -42,7 +42,7 @@ using namespace b200gs;
 extern "C" {
 
 const char* b200gs_last_error(void) { return g_error; }
-int b200gs_version(void) { return 231; }
+int b200gs_version(void) { return 232; }
 int64_t b200gs_launch_count(void) { return (int64_t)g_launches.load(std::memory_order_relaxed); }
 
 int b200gs_project_fwd(const B200gsView* view, int64_t n, const float* means, const float* scales, const float* quats,
@@ -647,6 +647,62 @@ int b200gs_gaussian_reg_bwd(int64_t n, const float* opacities, const float* scal
     return launch_gaussian_reg_bwd(n, opacities, scales, flags, opacity_weight, scale_weight, max_scale, max_scale_ratio, scale_lambda,
                                    ratio_lambda, static_cast<const float*>(workspace), v_terms, opacities ? v_opacities : nullptr,
                                    scales ? v_scales : nullptr, (cudaStream_t)stream);
+}
+
+size_t b200gs_normal_reg_workspace_bytes(int32_t height, int32_t width) {
+    return depth_size_ok(height, width) ? normal_reg_workspace_bytes(height, width) : 0;
+}
+
+// shared by the three normal entry points; returns the error code, or 0 when the arguments are valid
+static int check_normal_maps(const char* fn, int32_t height, int32_t width, const float* depth, const float* cam, int64_t ms0, int64_t ms1,
+                             const float* K, int64_t ks0, int64_t ks1) {
+    auto fail = [&](const char* msg) { set_error("%s: %s", fn, msg); return B200GS_EINVAL; };
+    if (height < 1 || width < 1) return fail("image size must be >= 1");
+    if (!depth_size_ok(height, width)) return fail("image too large");
+    if (ms0 < 0 || ms1 < 0 || ks0 < 0 || ks1 < 0) return fail("negative matrix stride");
+    if (!(depth && cam && K)) return fail("NULL pointer");
+    return 0;
+}
+
+static int check_normal_reg_workspace(const char* fn, int32_t height, int32_t width, const float* alpha, const void* workspace,
+                                      size_t workspace_bytes) {
+    if (!(alpha && workspace)) {
+        set_error("%s: NULL pointer", fn);
+        return B200GS_EINVAL;
+    }
+    if (workspace_bytes < normal_reg_workspace_bytes(height, width)) {
+        set_error("%s: workspace too small", fn);
+        return B200GS_ENOSPACE;
+    }
+    return 0;
+}
+
+int b200gs_normal_reg_fwd(int32_t height, int32_t width, const float* normal, int64_t normal_sc, int64_t normal_sy, int64_t normal_sx,
+                          const float* depth, const float* alpha, const float* w2c, int64_t w2c_s0, int64_t w2c_s1, const float* K,
+                          int64_t K_s0, int64_t K_s1, float weight, void* workspace, size_t workspace_bytes, float* loss, void* stream) {
+    if (int rc = check_normal_maps(__func__, height, width, depth, w2c, w2c_s0, w2c_s1, K, K_s0, K_s1)) return rc;
+    if (int rc = check_normal_reg_workspace(__func__, height, width, alpha, workspace, workspace_bytes)) return rc;
+    B200GS_CHECK_ARG(normal && loss, "NULL pointer");
+    B200GS_CHECK_ARG(normal_sc >= 0 && normal_sy >= 0 && normal_sx >= 0, "negative normal stride");
+    return launch_normal_reg_fwd(height, width, normal, normal_sc, normal_sy, normal_sx, depth, alpha, w2c, w2c_s0, w2c_s1, K, K_s0, K_s1,
+                                 weight, static_cast<float*>(workspace), loss, (cudaStream_t)stream);
+}
+
+int b200gs_normal_reg_bwd(int32_t height, int32_t width, const float* depth, const float* alpha, const float* w2c, int64_t w2c_s0,
+                          int64_t w2c_s1, const float* K, int64_t K_s0, int64_t K_s1, const void* workspace, size_t workspace_bytes,
+                          const float* v_loss, float* v_normal, void* stream) {
+    if (int rc = check_normal_maps(__func__, height, width, depth, w2c, w2c_s0, w2c_s1, K, K_s0, K_s1)) return rc;
+    if (int rc = check_normal_reg_workspace(__func__, height, width, alpha, workspace, workspace_bytes)) return rc;
+    B200GS_CHECK_ARG(v_loss && v_normal, "NULL pointer");
+    return launch_normal_reg_bwd(height, width, depth, alpha, w2c, w2c_s0, w2c_s1, K, K_s0, K_s1, static_cast<const float*>(workspace),
+                                 v_loss, v_normal, (cudaStream_t)stream);
+}
+
+int b200gs_depth_to_normal(int32_t height, int32_t width, const float* depth, const float* c2w, int64_t c2w_s0, int64_t c2w_s1,
+                           const float* K, int64_t K_s0, int64_t K_s1, float* normals, void* stream) {
+    if (int rc = check_normal_maps(__func__, height, width, depth, c2w, c2w_s0, c2w_s1, K, K_s0, K_s1)) return rc;
+    B200GS_CHECK_ARG(normals, "NULL pointer");
+    return launch_depth_to_normal(height, width, depth, c2w, c2w_s0, c2w_s1, K, K_s0, K_s1, normals, (cudaStream_t)stream);
 }
 
 size_t b200gs_knn_workspace_bytes(int64_t n) { return n < 0 ? 0 : knn_workspace_bytes(n); }

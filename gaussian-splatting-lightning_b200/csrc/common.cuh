@@ -205,6 +205,18 @@ int launch_gaussian_reg_bwd(int64_t n, const float* opac, const float* scales, i
                             float max_ratio, float lam, float lam_r, const float* ws, const float* v_terms, float* v_opac,
                             float* v_scales, cudaStream_t st);
 
+// depth-normal consistency (normal_reg.cu): depth, alpha [H,W] contiguous; normal [3,H,W] read at normal[c sc + y sy + x sx];
+// v_normal [3,H,W] and the depth_to_normal output [H,W,3] contiguous; the 4x4 camera matrix (w2c for the loss, c2w for
+// depth_to_normal) at m[i ms0 + j ms1] and K [3,3] at K[i ks0 + j ks1].  The backward reads the coefficient its forward wrote.
+size_t normal_reg_workspace_bytes(int height, int width);
+int launch_normal_reg_fwd(int height, int width, const float* normal, int64_t sc, int64_t sy, int64_t sx, const float* depth,
+                          const float* alpha, const float* w2c, int64_t ms0, int64_t ms1, const float* K, int64_t ks0, int64_t ks1,
+                          float weight, float* ws, float* loss, cudaStream_t st);
+int launch_normal_reg_bwd(int height, int width, const float* depth, const float* alpha, const float* w2c, int64_t ms0, int64_t ms1,
+                          const float* K, int64_t ks0, int64_t ks1, const float* ws, const float* v_loss, float* v_normal, cudaStream_t st);
+int launch_depth_to_normal(int height, int width, const float* depth, const float* c2w, int64_t ms0, int64_t ms1, const float* K,
+                           int64_t ks0, int64_t ks1, float* out, cudaStream_t st);
+
 // appearance MLP (appearance.cu); the shape arguments are those of B200gsAppearanceMlp, validated by the caller
 bool appearance_mlp_fits(int feat_dim, int n_freq, int n_neurons, int n_layers, int n_out);
 size_t appearance_mlp_workspace_bytes(int feat_dim, int n_freq, int n_neurons, int n_layers, int n_out);

@@ -1,5 +1,5 @@
-"""Training metrics (the reference's ``internal/metrics/vanilla_metrics.py``, ``inverse_depth_metrics.py``, ``mcmc_metrics.py`` and
-``scale_regularization_metrics.py``) on the b200gs kernels.
+"""Training metrics (the reference's ``internal/metrics/vanilla_metrics.py``, ``inverse_depth_metrics.py``, ``mcmc_metrics.py``,
+``scale_regularization_metrics.py`` and ``normal_reg.py``) on the b200gs kernels.
 Select them as the model's metric:
 
     model:
@@ -14,6 +14,9 @@ one backward, no host synchronisation.  PSNR and LPIPS for validation stay torch
 torchmetrics imports.  ``B200MCMCMetrics``, ``B200ScaleRegularizationMetrics`` and ``B200ScaleRegularizationWithDepthMetrics`` have
 ``MCMCMetrics``', ``ScaleRegularizationMetrics``' and ``ScaleRegularizationWithDepthMetrics``' fields, defaults, output keys and
 progress-bar flags; their per-Gaussian terms are ``gaussian_regularizers``: two kernel launches forward, one backward.
+``B200VanillaWithNormalRegMetrics`` has ``VanillaWithNormalRegMetrics``' fields, defaults, ``setup`` mutation, output keys and
+progress-bar flags; its depth-normal term is ``normal_consistency_loss``: two kernel launches forward, one backward.
+``depth_to_normal`` is gsplat's ``utils.depth_to_normal`` for the reference's call, which ``compat.install()`` registers.
 """
 from dataclasses import dataclass, field
 from typing import Literal, Optional
@@ -558,4 +561,157 @@ class B200ScaleRegularizationWithDepthMetrics(B200ScaleRegularizationMetricsMixi
 
 
 class B200ScaleRegularizationWithDepthMetricsModule(B200ScaleRegularizationMetricsModuleMixin, B200InverseDepthMetricsModule):
+    pass
+
+
+# ---- VanillaWithNormalRegMetrics (internal/metrics/normal_reg.py) and gsplat.utils.depth_to_normal ------------------------------------
+NORMAL_REG_FWD_LAUNCHES = 2     # library launches of one normal_consistency_loss forward: per-tile partials, reduce
+NORMAL_REG_BWD_LAUNCHES = 1     # and of its backward
+
+
+def _image_map(t, name):
+    """[1,H,W] or [H,W] float32 CUDA -> detached contiguous [H,W] (a view when it already is one)"""
+    if t.dim() == 3 and t.shape[0] == 1:
+        t = t[0]
+    if t.dim() != 2:
+        raise ValueError(f"{name} must be [1, H, W] or [H, W], got {tuple(t.shape)}")
+    if t.dtype != torch.float32 or not t.is_cuda:
+        raise ValueError(f"{name} must be a float32 CUDA tensor")
+    return t.detach().contiguous()
+
+
+def _camera_matrix(t, rows, name, device):
+    """[rows, rows] or [1, rows, rows] float32 on `device`, read in place through its strides"""
+    if t.dim() == 3 and t.shape[0] == 1:
+        t = t[0]
+    if tuple(t.shape) != (rows, rows):
+        raise ValueError(f"{name} must be [{rows}, {rows}] or [1, {rows}, {rows}], got {tuple(t.shape)}")
+    if t.dtype != torch.float32 or t.device != device:
+        raise ValueError(f"{name} must be float32 on {device}, got {t.dtype} on {t.device}")
+    return t.detach()
+
+
+class _NormalConsistencyLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, normal, depth, alpha, w2c, K, weight):
+        H, W = depth.shape
+        L = lib()
+        nbytes = int(L.b200gs_normal_reg_workspace_bytes(H, W))
+        ws = torch.empty(nbytes // 4, dtype=torch.float32, device=depth.device)
+        loss = torch.empty((), dtype=torch.float32, device=depth.device)
+        check(L.b200gs_normal_reg_fwd(H, W, ptr(normal), *normal.stride(), ptr(depth), ptr(alpha), ptr(w2c), *w2c.stride(), ptr(K), *K.stride(),
+                                      weight, ptr(ws), nbytes, ptr(loss), _stream()), "b200gs_normal_reg_fwd")
+        ctx.save_for_backward(depth, alpha, w2c, K, ws)
+        return loss
+
+    @staticmethod
+    def backward(ctx, v_loss):
+        depth, alpha, w2c, K, ws = ctx.saved_tensors
+        H, W = depth.shape
+        v = v_loss.reshape(1).to(torch.float32).contiguous()
+        v_normal = torch.empty((3, H, W), dtype=torch.float32, device=depth.device)
+        check(lib().b200gs_normal_reg_bwd(H, W, ptr(depth), ptr(alpha), ptr(w2c), w2c.stride(0), w2c.stride(1), ptr(K), K.stride(0),
+                                          K.stride(1), ptr(ws), ws.numel() * 4, ptr(v), ptr(v_normal), _stream()), "b200gs_normal_reg_bwd")
+        return v_normal, None, None, None, None, None
+
+
+def normal_consistency_loss(normal, exp_depth, alpha, w2c, K, weight):
+    """``NormalRegModuleMixin.get_normal_reg_metrics``' normal term of one view on K39/K40 (backward K41):
+        weight mean(1 - sum_c normal[c] n_d[c]),   n_d = depth_to_normal(exp_depth, inv(w2c), K) * alpha
+    normal float32 CUDA [3,H,W], read in place through its strides (the render's channel slice needs no copy); exp_depth and alpha
+    [1,H,W] or [H,W], detached as the reference detaches them; w2c the world-to-camera matrix [4,4] or [1,4,4] and K [3,3] or
+    [1,3,3], float32 on the same device, read there (the 3x3 block of w2c is inverted in the kernels: no torch.linalg.inv, no host
+    synchronisation).  Returns a device scalar; the gradient goes to normal only, -weight / (H W) n_d."""
+    if normal.dim() != 3 or normal.shape[0] != 3:
+        raise ValueError(f"normal must be [3, H, W], got {tuple(normal.shape)}")
+    if normal.dtype != torch.float32 or not normal.is_cuda:
+        raise ValueError("normal must be a float32 CUDA tensor")
+    depth, alpha = _image_map(exp_depth, "exp_depth"), _image_map(alpha, "alpha")
+    if depth.shape != normal.shape[1:] or alpha.shape != depth.shape or depth.device != normal.device or alpha.device != normal.device:
+        raise ValueError(f"normal {tuple(normal.shape)}, exp_depth {tuple(exp_depth.shape)} and alpha {tuple(alpha.shape)} must be one "
+                         "image size on one device")
+    w2c, K = _camera_matrix(w2c, 4, "w2c", normal.device), _camera_matrix(K, 3, "K", normal.device)
+    return _NormalConsistencyLoss.apply(normal, depth, alpha, w2c, K, float(weight))
+
+
+def depth_to_normal(depths, camtoworlds, Ks, z_depth: bool = True):
+    """gsplat's ``utils.depth_to_normal`` for the call ``NormalRegModuleMixin`` makes, on K42: depths [H,W,1] (or [1,H,W,1]) of z
+    depth, camtoworlds [4,4] and Ks [3,3] (or with a leading 1), float32 CUDA.  Returns the [H,W,3] (or [1,H,W,3]) map of
+    normalize(cross(p[y+1,x] - p[y-1,x], p[y,x+1] - p[y,x-1])), 0 on the one-pixel border.  Not differentiable: depths that require
+    grad raise NotImplementedError, and so does z_depth=False (ray distance)."""
+    if not z_depth:
+        raise NotImplementedError("depth_to_normal with z_depth=False is not provided")
+    if depths.requires_grad:
+        raise NotImplementedError("depth_to_normal has no backward: pass depths.detach()")
+    batched = depths.dim() == 4
+    d = depths[0] if batched and depths.shape[0] == 1 else depths
+    if d.dim() != 3 or d.shape[-1] != 1:
+        raise ValueError(f"depths must be [H, W, 1] or [1, H, W, 1], got {tuple(depths.shape)}")
+    d = _image_map(d[..., 0], "depths")
+    H, W = d.shape
+    c2w, K = _camera_matrix(camtoworlds, 4, "camtoworlds", d.device), _camera_matrix(Ks, 3, "Ks", d.device)
+    out = torch.empty((H, W, 3), dtype=torch.float32, device=d.device)
+    check(lib().b200gs_depth_to_normal(H, W, ptr(d), ptr(c2w), c2w.stride(0), c2w.stride(1), ptr(K), K.stride(0), K.stride(1), ptr(out),
+                                       _stream()), "b200gs_depth_to_normal")
+    return out[None] if batched else out
+
+
+_NORMAL_REG_OUTPUTS = ("exp_depth", "alpha", "normal", "preprocessed_camera")
+
+
+@dataclass
+class B200NormalRegMixin:
+    normal_reg_lambda: float = 0.05
+
+    flatten_reg: float = 0.02
+
+    def instantiate(self, *args, **kwargs):
+        raise NotImplementedError()
+
+
+class B200NormalRegModuleMixin:
+    """The depth-normal consistency and flatten terms, in training only: ``normal_loss`` = ``normal_consistency_loss`` of the render's
+    ``normal``, ``exp_depth``, ``alpha`` and ``preprocessed_camera`` times ``normal_reg_lambda``, and ``flatten_loss`` =
+    ``flatten_reg`` mean(get_scales()[..., -1]) (the last scale column, in torch).  Both are added to the loss; keys off the progress
+    bar.  ``setup("fit")`` changes the model as the reference does: uniform random rotations and the last log-scale lowered by log 5,
+    both from torch's global generator."""
+
+    def setup(self, stage: str, pl_module):
+        super().setup(stage, pl_module)
+        if stage == "fit":
+            with torch.no_grad():
+                gaussians = pl_module.gaussian_model.gaussians
+                gaussians["rotations"].copy_(torch.rand_like(gaussians["rotations"]))
+                gaussians["scales"][..., -1] -= torch.log(torch.tensor(5., dtype=torch.float, device=gaussians["scales"].device))
+
+    def get_normal_reg_metrics(self, gaussian_model, outputs, pl_module, metrics, pbar):
+        missing = [k for k in _NORMAL_REG_OUTPUTS if outputs.get(k) is None]
+        if missing:
+            raise ValueError(f"the normal regulariser needs the render outputs {missing}: render with renderer_output_types "
+                             "[rgb, alpha, exp_depth, normal] on a gsplat v1 renderer")
+        w2c, K, _ = outputs["preprocessed_camera"]
+        normal_loss = normal_consistency_loss(outputs["normal"], outputs["exp_depth"], outputs["alpha"], w2c[0], K[0],
+                                              self.config.normal_reg_lambda)
+        flatten_loss = gaussian_model.get_scales()[..., -1].mean() * self.config.flatten_reg
+
+        metrics["loss"] = metrics["loss"] + normal_loss + flatten_loss
+        metrics["normal_loss"] = normal_loss
+        metrics["flatten_loss"] = flatten_loss
+        pbar["normal_loss"] = False
+        pbar["flatten_loss"] = False
+
+    def get_train_metrics(self, pl_module, gaussian_model, step: int, batch, outputs):
+        metrics, pbar = super().get_train_metrics(pl_module, gaussian_model, step, batch, outputs)
+        self.get_normal_reg_metrics(gaussian_model, outputs, pl_module, metrics, pbar)
+        return metrics, pbar
+
+
+@dataclass
+class B200VanillaWithNormalRegMetrics(B200NormalRegMixin, B200VanillaMetrics):
+    def instantiate(self, *args, **kwargs) -> "B200VanillaWithNormalRegMetricsModule":
+        self._check()
+        return B200VanillaWithNormalRegMetricsModule(self)
+
+
+class B200VanillaWithNormalRegMetricsModule(B200NormalRegModuleMixin, B200VanillaMetricsModule):
     pass

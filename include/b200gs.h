@@ -357,6 +357,40 @@ B200GS_API int b200gs_gaussian_reg_bwd(int64_t n, const float* opacities, const 
                                        const void* workspace, size_t workspace_bytes, const float* v_terms, float* v_opacities,
                                        float* v_scales, void* stream);
 
+/* ---- Depth-normal consistency (internal/metrics/normal_reg.py:27-38, NormalRegModuleMixin.get_normal_reg_metrics, and gsplat's
+ *      utils.depth_to_normal as it calls it) ---------------------------------------------------------------------------------------
+ * n_d[y,x] = alpha[y,x] normalize(cross(p[y+1,x] - p[y-1,x], p[y,x+1] - p[y,x-1])) with p[y,x] = o + depth[y,x] R ((x - cx + 0.5) / fx,
+ *     (y - cy + 0.5) / fy, 1), R / o the camera-to-world rotation / origin, normalize dividing by max(|v|, 1e-12); 0 on the one-pixel
+ *     border (everywhere when height or width < 3).  The origin cancels and is never formed (exact in real arithmetic; in fp32 it
+ *     avoids the reference's cancellation at large camera translations).  Every entry point computes n_d with the same code, so the
+ *     forward, the backward and depth_to_normal agree bit for bit.
+ * Matrices are read on the device, never copied to the host: the 4x4 camera matrix at m[i s0 + j s1] (only its 3x3 block is read) and
+ *     K float[3,3] at K[i K_s0 + j K_s1] (fx = K[0,0], fy = K[1,1], cx = K[0,2], cy = K[1,2]).
+ * b200gs_normal_reg_fwd: normal float[3,H,W] at normal[c normal_sc + y normal_sy + x normal_sx] (a channel slice of the permuted
+ *     render, read in place), depth and alpha float[H,W] contiguous, w2c the world-to-camera matrix (normal_reg.py:29-31 inverts it
+ *     with torch.linalg.inv, which synchronises; here the 3x3 block is inverted in double once per CTA, equal to the 3x3 block of
+ *     the inverse for an affine [R t; 0 1]).  loss float[1] <- weight mean_{H W}(1 - sum_c normal[c] n_d[c]) (normal_reg.py:31-35,
+ *     err * normal_reg_lambda).
+ * b200gs_normal_reg_bwd: v_normal float[3,H,W] contiguous <- -v_loss[0] weight / (H W) n_d, v_loss read on the device; it reads the
+ *     coefficient its forward wrote to the workspace and takes the same depth, alpha and matrices.
+ * b200gs_depth_to_normal: normals float[H,W,3] contiguous <- n_d with alpha = 1 from depth float[H,W] contiguous and c2w the
+ *     camera-to-world matrix (gsplat utils.depth_to_normal with z_depth = True, normal_reg.py:29-32).
+ * b200gs_normal_reg_workspace_bytes: device scratch shared by the forward and the backward; 0 for a size that is not accepted.
+ * Sizes: 1 <= height <= 65535 * 16, width >= 1, height * width <= 2^31 - 1.
+ * Launches: forward 2 (per-tile partials, reduce), backward 1, depth_to_normal 1.  No host synchronisation, no float atomics: two
+ *     calls give bit-identical results.
+ * Algorithmic bytes per pixel: forward 4 depth + 4 alpha + 12 normal in; backward 8 in + 12 out; depth_to_normal 4 in + 12 out. */
+B200GS_API size_t b200gs_normal_reg_workspace_bytes(int32_t height, int32_t width);
+B200GS_API int b200gs_normal_reg_fwd(int32_t height, int32_t width, const float* normal, int64_t normal_sc, int64_t normal_sy,
+                                     int64_t normal_sx, const float* depth, const float* alpha, const float* w2c, int64_t w2c_s0,
+                                     int64_t w2c_s1, const float* K, int64_t K_s0, int64_t K_s1, float weight, void* workspace,
+                                     size_t workspace_bytes, float* loss, void* stream);
+B200GS_API int b200gs_normal_reg_bwd(int32_t height, int32_t width, const float* depth, const float* alpha, const float* w2c, int64_t w2c_s0,
+                                     int64_t w2c_s1, const float* K, int64_t K_s0, int64_t K_s1, const void* workspace,
+                                     size_t workspace_bytes, const float* v_loss, float* v_normal, void* stream);
+B200GS_API int b200gs_depth_to_normal(int32_t height, int32_t width, const float* depth, const float* c2w, int64_t c2w_s0, int64_t c2w_s1,
+                                      const float* K, int64_t K_s0, int64_t K_s1, float* normals, void* stream);
+
 /* b200gs_knn_mean_dist2: simple_knn's distCUDA2 (vanilla_gaussian.py:122-125, the scale initialiser): mean_dist2[i] = mean of the squared
  *     distances from points[i] (float[n,3]) to its 3 nearest neighbours (exact).  Synchronises the stream once (the hash grid is sized
  *     on the host from the bounding box); init-time only. */
