@@ -171,6 +171,37 @@ __device__ __forceinline__ void gather_splat(int g, const SplatStrides& st, cons
     for (int c = 0; c < CH; ++c) col[c] = __ldg(colors + int64_t(g) * st.ks + c);
 }
 
+// A staged splat (record r0, r1) sampled at the pixel of t.  Every blend kernel evaluates its samples here, so the forward and
+// the backward see the same alpha; each applies its own alpha test.
+struct Sample {
+    float dx, dy, p2, G, oG, a;   // splat centre - pixel, power * log2(e), Gaussian, opacity * Gaussian, clamped alpha
+};
+
+__device__ __forceinline__ Sample eval_sample(const TilePixel& t, const float4& r0, const float4& r1) {
+    const float dx = r0.x - t.pxf, dy = r0.y - t.pyf;
+    // power * log2(e) = a' dx^2 + b' dx dy + c' dy^2
+    const float p2 = fmaf(r1.x * dy, dy, fmaf(r0.w, dy, r0.z * dx) * dx);
+    const float G = ex2_approx(p2);
+    const float oG = r1.y * G;
+    return {dx, dy, p2, G, oG, fminf(t.amax, oG)};
+}
+
+// Forward step of a sample of alpha a (0 if it failed the alpha test): composite(w) adds it to the pixel with weight w, which is
+// returned.  Tc, the transmittance used for compositing, drops to exactly 0 when the pixel stops, so every later sample weighs
+// nothing without a `done` predicate; T keeps the value in front of the stopping sample.  Calling composite before the state
+// update, and forming base + j + 1 here, keep K6's instruction schedule.
+template <bool GSPLAT, typename Composite>
+__device__ __forceinline__ float fwd_step(float a, int base, int j, float& T, float& Tc, int& last, Composite composite) {
+    const float nT = fmaf(-a, Tc, Tc);
+    const bool stop = GSPLAT ? (nT <= T_STOP) : (nT < T_STOP);
+    const float w = stop ? 0.f : a * Tc;
+    composite(w);
+    last = (w > 0.f) ? base + j + 1 : last;
+    T = stop ? T : nT;
+    Tc = stop ? 0.f : nT;
+    return w;
+}
+
 // Composites the four list entries list[0..3] of the batch that starts at slab index `base` into the pixel.
 // HITS: also mark every splat that contributed to at least one pixel (gsplat's `means2d.has_hit_any_pixels`, read by
 // SelectiveAdam, optimizers.py:39, and exported as `acc_vis`, gsplat_v1_renderer.py:287): one byte store per (warp, contributing entry).
@@ -183,26 +214,17 @@ __device__ __forceinline__ void composite4(float& T, float& Tc, int& last, float
         const int j = list[u];                         // entries past the list's end are DUMMY (alpha 0)
         const float4 r0 = s_rec[j * 3 + 0];
         const float4 r1 = s_rec[j * 3 + 1];
-        const float dx = r0.x - t.pxf, dy = r0.y - t.pyf;
-        // power * log2(e) = a' dx^2 + b' dx dy + c' dy^2
-        const float p2 = fmaf(r1.x * dy, dy, fmaf(r0.w, dy, r0.z * dx) * dx);
-        float a = fminf(t.amax, r1.y * ex2_approx(p2));
-        a = (!(p2 > 0.0f) && !(a < ALPHA_MIN)) ? a : 0.f;             // a sample that fails the alpha test composites nothing
-        // Tc is the transmittance used for compositing; it drops to exactly 0 when the pixel stops, so every later sample
-        // weighs nothing without a `done` predicate in the arithmetic; T keeps the value in front of the stopping sample
-        const float nT = fmaf(-a, Tc, Tc);
-        const bool stop = GSPLAT ? (nT <= T_STOP) : (nT < T_STOP);
-        const float w = stop ? 0.f : a * Tc;
-        C[0] = fmaf(r1.z, w, C[0]);
-        if (CH > 1) C[1] = fmaf(r1.w, w, C[1]);
-        if (CH > 2) {
-            const float2 r2 = *reinterpret_cast<const float2*>(&s_rec[j * 3 + 2]);
-            C[2] = fmaf(r2.x, w, C[2]);
-            if (CH > 3) C[3] = fmaf(r2.y, w, C[3]);
-        }
-        last = (w > 0.f) ? base + j + 1 : last;
-        T = stop ? T : nT;
-        Tc = stop ? 0.f : nT;
+        const Sample sp = eval_sample(t, r0, r1);
+        const float a = (!(sp.p2 > 0.0f) && !(sp.a < ALPHA_MIN)) ? sp.a : 0.f;   // a sample that fails the alpha test composites nothing
+        const float w = fwd_step<GSPLAT>(a, base, j, T, Tc, last, [&](float w) {
+            C[0] = fmaf(r1.z, w, C[0]);
+            if (CH > 1) C[1] = fmaf(r1.w, w, C[1]);
+            if (CH > 2) {
+                const float2 r2 = *reinterpret_cast<const float2*>(&s_rec[j * 3 + 2]);
+                C[2] = fmaf(r2.x, w, C[2]);
+                if (CH > 3) C[3] = fmaf(r2.y, w, C[3]);
+            }
+        });
         if (HITS) {
             if (__any_sync(FULL, w > 0.f) && lane == 0) hit_any[s_gid[j]] = 1;
         }
@@ -415,6 +437,120 @@ struct TrSmem {
 };
 static_assert(sizeof(TrSmem<false>) <= 57344, "4 CTAs per SM need <= 56 KB each");
 
+// The deepest contributor of the warp (wmax) and of the CTA (returned); s_wmax holds NWARP ints of shared memory.
+__device__ __forceinline__ int deepest_contributor(int last, int* s_wmax, int warp, unsigned lane, int& wmax) {
+    wmax = __reduce_max_sync(FULL, last);
+    if (lane == 0) s_wmax[warp] = wmax;
+    __syncthreads();
+    int max_last = 0;
+#pragma unroll
+    for (int w = 0; w < NWARP; ++w) max_last = max(max_last, s_wmax[w]);
+    return max_last;
+}
+
+// Reverse transmittance step over a sample of alpha a that passed the alpha test: T becomes the transmittance in front of it,
+// ra = 1 / (1 - a), and the sample's compositing weight a T is returned.
+__device__ __forceinline__ float unblend(float a, float& T, float& ra) {
+    ra = 1.0f / (1.0f - a);
+    T *= ra;
+    return a * T;
+}
+
+// Gradient terms of that sample from S = <colour, v>, unblend's ra, T and fac, and D = <colour accumulated behind it, v>: D advanced
+// past the sample, go = dL/d(opacity-weighted Gaussian) and, ABS, |dL/dmean2D| of the sample.
+struct SampleGrad {
+    float D, go, gax, gay;
+};
+
+template <bool GSPLAT, bool ABS>
+__device__ __forceinline__ SampleGrad sample_grad(const Sample& sp, const float4& r0, const float4& r1, float S, float ra, float T,
+                                                  float fac, float tail, float D) {
+    // dL/dalpha = T <c, v> - (<colour behind, v> + T_final (bg.v - v_alpha)) / (1 - alpha)
+    const float v_al = fmaf(T, S, ra * (tail - D));
+    SampleGrad g = {fmaf(fac, S, D), 0.f, 0.f, 0.f};
+    if (!GSPLAT || (sp.oG <= 0.999f)) g.go = sp.G * v_al;
+    if (ABS) {   // |v_sigma (A dx + B dy)|, |v_sigma (B dx + C dy)|, v_sigma = -opacity * go
+        const float vsg = r1.y * g.go * (2.0f / LOG2E);
+        g.gax = fabsf(vsg * fmaf(r0.z, sp.dx, 0.5f * r0.w * sp.dy));
+        g.gay = fabsf(vsg * fmaf(0.5f * r0.w, sp.dx, r1.x * sp.dy));
+    }
+    return g;
+}
+
+// Sums of go * {1, x, y, x^2, xy, y^2} over the warp's 32 pixels (x, y: pixel position in the warp's 8x4 block) and, ABS, of
+// |gx| and |gy|: the mean / conic gradients of an entry are linear in them.
+struct Moments {
+    float S0, Sx, Sy, Sxx, Sxy, Syy, Ax, Ay;
+};
+
+// Lane (re, rh) sums its row of the value tile (entry re, pixels 16 rh .. 16 rh + 15) with compile-time x as FFMA immediates; one
+// xor-16 exchange combines the halves.  per_pixel(k, fac) sees each pixel's fac and exchange() runs between the moment and absgrad
+// shuffles: K7 sums and exchanges its colour sums there (after the absgrad shuffles, two of its instantiations schedule differently).
+template <bool ABS, typename PerPixel, typename Exchange>
+__device__ __forceinline__ Moments reduce_moments(const float4* my_row, float hh, PerPixel per_pixel, Exchange exchange) {
+    float R0 = 0.f, R0x = 0.f, R0xx = 0.f, R1 = 0.f, R1x = 0.f, R1xx = 0.f;
+    float Ax = 0.f, Ay = 0.f;
+#pragma unroll
+    for (int k2 = 0; k2 < 8; ++k2) {
+        float4 v;                             // {go, fac} of pixels 2 k2, 2 k2 + 1
+        if (ABS) {
+            const float4 va = my_row[2 * k2], vb = my_row[2 * k2 + 1];
+            v = make_float4(va.x, va.y, vb.x, vb.y);
+            Ax += va.z + vb.z;
+            Ay += va.w + vb.w;
+        } else {
+            v = my_row[k2];
+        }
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int k = 2 * k2 + e;
+            const float gk = e ? v.z : v.x;
+            const float x = float(k & 7);
+            if (k < 8) { R0 += gk; if (k & 7) { R0x = fmaf(gk, x, R0x); R0xx = fmaf(gk, x * x, R0xx); } }
+            else       { R1 += gk; if (k & 7) { R1x = fmaf(gk, x, R1x); R1xx = fmaf(gk, x * x, R1xx); } }
+            per_pixel(k, e ? v.w : v.y);
+        }
+    }
+    // moments in block coordinates (x = 0..7, y = 2 rh + {0, 1}), then both halves
+    float S0 = R0 + R1, Sx = R0x + R1x, Sxx = R0xx + R1xx;
+    float Sy = fmaf(hh, S0, R1), Sxy = fmaf(hh, Sx, R1x), Syy = fmaf(hh * hh, S0, fmaf(2.0f * hh, R1, R1));
+    S0 += __shfl_xor_sync(FULL, S0, 16);
+    Sx += __shfl_xor_sync(FULL, Sx, 16);
+    Sy += __shfl_xor_sync(FULL, Sy, 16);
+    Sxx += __shfl_xor_sync(FULL, Sxx, 16);
+    Sxy += __shfl_xor_sync(FULL, Sxy, 16);
+    Syy += __shfl_xor_sync(FULL, Syy, 16);
+    exchange();
+    if (ABS) {
+        Ax += __shfl_xor_sync(FULL, Ax, 16);
+        Ay += __shfl_xor_sync(FULL, Ay, 16);
+    }
+    return {S0, Sx, Sy, Sxx, Sxy, Syy, Ax, Ay};
+}
+
+// Gradient of an entry (record r0, r1) w.r.t. its mean2D and conic, from its moments over the warp's block at (bx0, by0).
+// The accessors form each component where the caller uses it, which keeps K7's instruction schedule.
+struct EntryGrad {
+    float A, B, C;   // conic
+    float M1, M2, M3, M4, M5;
+    __device__ __forceinline__ float mean_x() const { return A * M1 + B * M2; }
+    __device__ __forceinline__ float mean_y() const { return B * M1 + C * M2; }
+    __device__ __forceinline__ float conic0() const { return 0.5f * M3; }
+    __device__ __forceinline__ float conic1() const { return M4; }
+    __device__ __forceinline__ float conic2() const { return 0.5f * M5; }
+};
+
+__device__ __forceinline__ EntryGrad entry_grad(const float4& r0, const float4& r1, float bx0, float by0, const Moments& m) {
+    const float A = r0.z * (-2.0f / LOG2E), B = r0.w * (-1.0f / LOG2E), Cc = r1.x * (-2.0f / LOG2E);
+    const float ex = r0.x - bx0, ey = r0.y - by0;   // dx = ex - x, dy = ey - y
+    const float no = -r1.y;                        // dL/dsigma = -opacity * go
+    const float M1 = no * fmaf(ex, m.S0, -m.Sx), M2 = no * fmaf(ey, m.S0, -m.Sy);
+    const float M3 = no * fmaf(ex, fmaf(ex, m.S0, -2.0f * m.Sx), m.Sxx);
+    const float M4 = no * (fmaf(ex, fmaf(ey, m.S0, -m.Sy), m.Sxy) - ey * m.Sx);
+    const float M5 = no * fmaf(ey, fmaf(ey, m.S0, -2.0f * m.Sy), m.Syy);
+    return {A, B, Cc, M1, M2, M3, M4, M5};
+}
+
 // VROWS: the gradient outputs are the columns of one [n,12] row buffer (include/b200gs.h row layout; v_xy = its base): the nine
 // sums of an entry leave as THREE 128-bit reductions (REDG.E.ADD.F32x4: {xy, -, conic0} {conic1, conic2, -, opacity} {rgb, -})
 // instead of nine 32-bit ones — a third of the L2 atomic operations, which bound this kernel once the shuffles were gone.
@@ -456,12 +592,8 @@ __global__ void __launch_bounds__(BLOCK_PIX, ABS ? 3 : 4) blend_bwd_tr_kernel(in
     const float va = (v_alpha && t.inside) ? __ldg(v_alpha + pix) : 0.f;
     const float tail = Tf * (va - bg_dot);  // d(out)/d(alpha_i) through everything behind the last contributor
 
-    const int wmax = __reduce_max_sync(FULL, last);
-    if (lane == 0) sm.wmax[warp] = wmax;
-    __syncthreads();
-    int max_last = 0;
-#pragma unroll
-    for (int w = 0; w < NWARP; ++w) max_last = max(max_last, sm.wmax[w]);
+    int wmax;
+    const int max_last = deepest_contributor(last, sm.wmax, warp, lane, wmax);
     if (max_last == 0) return;
 
     float T = Tf;
@@ -497,18 +629,12 @@ __global__ void __launch_bounds__(BLOCK_PIX, ABS ? 3 : 4) blend_bwd_tr_kernel(in
                 const int j = my_list[ii - u];
                 const float4 r0 = s_rec[j * 3 + 0];
                 const float4 r1 = s_rec[j * 3 + 1];
-                const float dx = r0.x - t.pxf, dy = r0.y - t.pyf;
-                // same arithmetic as the forward: power * log2(e) = a' dx^2 + b' dx dy + c' dy^2
-                const float p2 = fmaf(r1.x * dy, dy, fmaf(r0.w, dy, r0.z * dx) * dx);
-                const float G = ex2_approx(p2);
-                const float oG = r1.y * G;
-                const float a = fminf(t.amax, oG);
-                const bool valid = (j < rel_last) && !(p2 > 0.0f) && (a >= ALPHA_MIN);
+                const Sample sp = eval_sample(t, r0, r1);
+                const bool valid = (j < rel_last) && !(sp.p2 > 0.0f) && (sp.a >= ALPHA_MIN);
                 float go = 0.f, fac = 0.f, gax = 0.f, gay = 0.f;
                 if (valid) {
-                    const float ra = 1.0f / (1.0f - a);
-                    T *= ra;
-                    fac = a * T;
+                    float ra;
+                    fac = unblend(sp.a, T, ra);
                     float S = r1.z * vo[0];
                     if (CH > 1) S = fmaf(r1.w, vo[1], S);
                     if (CH > 2) {
@@ -516,16 +642,9 @@ __global__ void __launch_bounds__(BLOCK_PIX, ABS ? 3 : 4) blend_bwd_tr_kernel(in
                         S = fmaf(r2.x, vo[2], S);
                         if (CH > 3) S = fmaf(r2.y, vo[3], S);
                     }
-                    // dL/dalpha = T <c, v> - (<colour behind, v> + T_final (bg.v - v_alpha)) / (1 - alpha);  D = <colour behind, v>
-                    const float v_al = fmaf(T, S, ra * (tail - D));
-                    D = fmaf(fac, S, D);
-                    if (!GSPLAT || (oG <= 0.999f)) go = G * v_al;
+                    const SampleGrad sg = sample_grad<GSPLAT, ABS>(sp, r0, r1, S, ra, T, fac, tail, D);
+                    D = sg.D; go = sg.go; gax = sg.gax; gay = sg.gay;
                     vm |= 1u << u;
-                    if (ABS) {   // |dL/dmean2D| of this sample: |v_sigma (A dx + B dy)|, |v_sigma (B dx + C dy)|, v_sigma = -opacity * go
-                        const float vsg = r1.y * go * (2.0f / LOG2E);
-                        gax = fabsf(vsg * fmaf(r0.z, dx, 0.5f * r0.w * dy));
-                        gay = fabsf(vsg * fmaf(0.5f * r0.w, dx, r1.x * dy));
-                    }
                 }
                 if (ABS) *reinterpret_cast<float4*>(my_val + u * VAL_ROW) = make_float4(go, fac, gax, gay);
                 else *reinterpret_cast<float2*>(my_val + u * VAL_ROW) = make_float2(go, fac);
@@ -533,88 +652,50 @@ __global__ void __launch_bounds__(BLOCK_PIX, ABS ? 3 : 4) blend_bwd_tr_kernel(in
             const unsigned present = __reduce_or_sync(FULL, vm);
             __syncwarp();   // the tile stores of all lanes are visible to the row loads below
             if (present != 0u) {
-                // ---- reduce: lane (re, rh) sums entry ii-re over pixels 16 rh .. 16 rh + 15 (local x = k & 7, local row = k >> 3)
-                float R0 = 0.f, R0x = 0.f, R0xx = 0.f, R1 = 0.f, R1x = 0.f, R1xx = 0.f;
+                // ---- reduce: lane (re, rh) sums entry ii-re, and its colour sums sum(fac * v_image)
                 float Cs[4] = {0.f, 0.f, 0.f, 0.f};
-                float Ax = 0.f, Ay = 0.f;
+                const Moments mo = reduce_moments<ABS>(my_row, hh, [&](int k, float fk) {
+                    const float4 w = my_vo[k];
+                    Cs[0] = fmaf(fk, w.x, Cs[0]);
+                    if (CH > 1) Cs[1] = fmaf(fk, w.y, Cs[1]);
+                    if (CH > 2) Cs[2] = fmaf(fk, w.z, Cs[2]);
+                    if (CH > 3) Cs[3] = fmaf(fk, w.w, Cs[3]);
+                }, [&]() {
 #pragma unroll
-                for (int k2 = 0; k2 < 8; ++k2) {
-                    float4 v;                             // {go, fac} of pixels 2 k2, 2 k2 + 1
-                    if (ABS) {
-                        const float4 va = my_row[2 * k2], vb = my_row[2 * k2 + 1];
-                        v = make_float4(va.x, va.y, vb.x, vb.y);
-                        Ax += va.z + vb.z;
-                        Ay += va.w + vb.w;
-                    } else {
-                        v = my_row[k2];
-                    }
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int k = 2 * k2 + e;
-                        const float gk = e ? v.z : v.x, fk = e ? v.w : v.y;
-                        const float x = float(k & 7);
-                        if (k < 8) { R0 += gk; if (k & 7) { R0x = fmaf(gk, x, R0x); R0xx = fmaf(gk, x * x, R0xx); } }
-                        else       { R1 += gk; if (k & 7) { R1x = fmaf(gk, x, R1x); R1xx = fmaf(gk, x * x, R1xx); } }
-                        const float4 w = my_vo[k];
-                        Cs[0] = fmaf(fk, w.x, Cs[0]);
-                        if (CH > 1) Cs[1] = fmaf(fk, w.y, Cs[1]);
-                        if (CH > 2) Cs[2] = fmaf(fk, w.z, Cs[2]);
-                        if (CH > 3) Cs[3] = fmaf(fk, w.w, Cs[3]);
-                    }
-                }
-                // moments in block coordinates (x = 0..7, y = 2 rh + {0, 1}), then both halves
-                float S0 = R0 + R1, Sx = R0x + R1x, Sxx = R0xx + R1xx;
-                float Sy = fmaf(hh, S0, R1), Sxy = fmaf(hh, Sx, R1x), Syy = fmaf(hh * hh, S0, fmaf(2.0f * hh, R1, R1));
-                S0 += __shfl_xor_sync(FULL, S0, 16);
-                Sx += __shfl_xor_sync(FULL, Sx, 16);
-                Sy += __shfl_xor_sync(FULL, Sy, 16);
-                Sxx += __shfl_xor_sync(FULL, Sxx, 16);
-                Sxy += __shfl_xor_sync(FULL, Sxy, 16);
-                Syy += __shfl_xor_sync(FULL, Syy, 16);
-#pragma unroll
-                for (int c = 0; c < CH; ++c) Cs[c] += __shfl_xor_sync(FULL, Cs[c], 16);
-                if (ABS) {
-                    Ax += __shfl_xor_sync(FULL, Ax, 16);
-                    Ay += __shfl_xor_sync(FULL, Ay, 16);
-                }
+                    for (int c = 0; c < CH; ++c) Cs[c] += __shfl_xor_sync(FULL, Cs[c], 16);
+                });
                 if ((present >> re) & 1u) {
                     const int j = my_list[ii - re];
                     const int g = __float_as_int(s_rec[j * 3 + 2].z);
                     if (rh == 0) {
                         const float4 r0 = s_rec[j * 3 + 0];
                         const float4 r1 = s_rec[j * 3 + 1];
-                        const float A = r0.z * (-2.0f / LOG2E), B = r0.w * (-1.0f / LOG2E), Cc = r1.x * (-2.0f / LOG2E);
-                        const float ex = r0.x - bx0, ey = r0.y - by0;   // dx = ex - x, dy = ey - y
-                        const float no = -r1.y;                        // dL/dsigma = -opacity * go
-                        const float M1 = no * fmaf(ex, S0, -Sx), M2 = no * fmaf(ey, S0, -Sy);
-                        const float M3 = no * fmaf(ex, fmaf(ex, S0, -2.0f * Sx), Sxx);
-                        const float M4 = no * (fmaf(ex, fmaf(ey, S0, -Sy), Sxy) - ey * Sx);
-                        const float M5 = no * fmaf(ey, fmaf(ey, S0, -2.0f * Sy), Syy);
-                        const float gx = (A * M1 + B * M2) * sx, gy = (B * M1 + Cc * M2) * sy;
+                        const EntryGrad eg = entry_grad(r0, r1, bx0, by0, mo);
+                        const float gx = eg.mean_x() * sx, gy = eg.mean_y() * sy;
                         if (VROWS) {
                             float4* row = reinterpret_cast<float4*>(v_xy + int64_t(g) * B200GS_ROW_FLOATS);
-                            atomicAdd(row, make_float4(gx, gy, 0.f, 0.5f * M3));
-                            atomicAdd(row + 1, make_float4(M4, 0.5f * M5, 0.f, S0));
+                            atomicAdd(row, make_float4(gx, gy, 0.f, eg.conic0()));
+                            atomicAdd(row + 1, make_float4(eg.conic1(), eg.conic2(), 0.f, mo.S0));
                         } else {
                             float* vx = v_xy + int64_t(g) * st.xs;
                             float* vc = v_conic + int64_t(g) * st.cs;
                             atomicAdd(vx, gx);
                             atomicAdd(vx + 1, gy);
-                            atomicAdd(vc, 0.5f * M3);
-                            atomicAdd(vc + 1, M4);
-                            atomicAdd(vc + 2, 0.5f * M5);
+                            atomicAdd(vc, eg.conic0());
+                            atomicAdd(vc + 1, eg.conic1());
+                            atomicAdd(vc + 2, eg.conic2());
                         }
                     } else {
                         if (VROWS) {
                             atomicAdd(reinterpret_cast<float4*>(v_xy + int64_t(g) * B200GS_ROW_FLOATS) + 2, make_float4(Cs[0], Cs[1], Cs[2], 0.f));
                         } else {
-                            atomicAdd(v_opacity + int64_t(g) * st.os, S0);
+                            atomicAdd(v_opacity + int64_t(g) * st.os, mo.S0);
 #pragma unroll
                             for (int c = 0; c < CH; ++c) atomicAdd(v_colors + int64_t(g) * st.ks + c, Cs[c]);
                         }
                         if (ABS) {
-                            atomicAdd(v_xy_abs + 2 * int64_t(g), Ax);
-                            atomicAdd(v_xy_abs + 2 * int64_t(g) + 1, Ay);
+                            atomicAdd(v_xy_abs + 2 * int64_t(g), mo.Ax);
+                            atomicAdd(v_xy_abs + 2 * int64_t(g) + 1, mo.Ay);
                         }
                     }
                 }
@@ -661,20 +742,19 @@ int fwd_dispatch(bool rows, int width, int height, const int32_t* ranges, const 
     return B200GS_OK;
 }
 
-// Launches K7 instantiation <CH, GSPLAT, ABS, VROWS>.  Its first launch also sets the kernel's dynamic shared-memory limit.
-template <int CH, bool GSPLAT, bool ABS, bool VROWS, typename... Args>
-int bwd_launch(dim3 grid, cudaStream_t s, Args... args) {
-    const auto kernel = blend_bwd_tr_kernel<CH, GSPLAT, ABS, VROWS>;
-    static const cudaError_t attr_rc = [kernel]() {
-        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TrSmem<ABS>));
+// Launches `kernel` with `smem` bytes of dynamic shared memory; its first launch sets the kernel's shared-memory limit.
+template <auto kernel, size_t smem, typename... Args>
+int launch_dyn(dim3 grid, cudaStream_t s, const char* what, Args... args) {
+    static const cudaError_t attr_rc = [] {
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e == cudaSuccess) e = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
         return e;
     }();
     if (attr_rc != cudaSuccess) {
-        set_error("blend_bwd: cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_rc));
+        set_error("%s: cudaFuncSetAttribute failed: %s", what, cudaGetErrorString(attr_rc));
         return B200GS_ECUDA;
     }
-    kernel<<<grid, BLOCK_PIX, sizeof(TrSmem<ABS>), s>>>(args...);
+    kernel<<<grid, BLOCK_PIX, smem, s>>>(args...);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
@@ -688,9 +768,10 @@ int bwd_dispatch(bool rows, int width, int height, const int32_t* ranges, const 
     const dim3 grid(gx * div_up(height, TILE));
     const SplatStrides st = splat_strides<CH>(rows);
     const auto launch = [&](auto abs, auto vrows) {
-        return bwd_launch<CH, GSPLAT, decltype(abs)::value, decltype(vrows)::value>(
-            grid, s, width, height, gx, reinterpret_cast<const int2*>(ranges), ids, st, xy, conic, opacity, colors, bg, final_T, n_contrib,
-            v_image, ps, cs, v_alpha, sx, sy, v_xy, v_conic, v_opacity, v_colors, v_xy_abs);
+        constexpr bool ABS = decltype(abs)::value;
+        return launch_dyn<blend_bwd_tr_kernel<CH, GSPLAT, ABS, decltype(vrows)::value>, sizeof(TrSmem<ABS>)>(
+            grid, s, "blend_bwd", width, height, gx, reinterpret_cast<const int2*>(ranges), ids, st, xy, conic, opacity, colors, bg, final_T,
+            n_contrib, v_image, ps, cs, v_alpha, sx, sy, v_xy, v_conic, v_opacity, v_colors, v_xy_abs);
     };
     if (v_xy_abs) return launch(std::true_type{}, std::false_type{});
     if (!rows) return launch(std::false_type{}, std::false_type{});
@@ -711,11 +792,10 @@ int bwd_dispatch(bool rows, int width, int height, const int32_t* ranges, const 
 // instantiation that holds it (the channels past D are masked at load and store).
 //
 // Forward: the geometry record is staged as in K6; the batch's feature rows go to their own [257][CH] array (row DUMMY zero),
-// loaded by the whole CTA with coalesced reads.  Per sample the alpha / Tc / stop arithmetic is composite4's, then CH FMAs on
-// warp-uniform LDS.128 broadcasts of the feature row: each channel sees the same operations in the same order as in K6, so a
-// chunk's composite is bit-identical to the <= 4-channel groups of rasterize_binned.  The background term is one FMA here; K6
-// leaves C + T * bg to nvcc, which fuses it for some channels and rounds T * bg first for others, so with a background a
-// channel may differ from K6's by that one rounding.
+// loaded by the whole CTA with coalesced reads.  Each sample goes through composite4's eval_sample and fwd_step, with CH FMAs on
+// warp-uniform LDS.128 broadcasts of the feature row, so a chunk's composite is bit-identical to the <= 4-channel groups of
+// rasterize_binned.  The background term is one FMA here; K6 leaves C + T * bg to nvcc, which fuses it for some channels and
+// rounds T * bg first for others, so with a background a channel may differ from K6's by that one rounding.
 template <int CH>
 struct FeatFwdSmem {
     float4 rec[REC_SLAB];
@@ -788,25 +868,19 @@ __global__ void __launch_bounds__(BLOCK_PIX, CH > 16 ? 2 : CH > 8 ? 3 : 4) blend
                 const int j = my_list[i0 + u];                 // warp-uniform: the feature reads below are broadcasts
                 const float4 r0 = s_rec[j * 3 + 0];
                 const float4 r1 = s_rec[j * 3 + 1];
-                const float dx = r0.x - t.pxf, dy = r0.y - t.pyf;
-                const float p2 = fmaf(r1.x * dy, dy, fmaf(r0.w, dy, r0.z * dx) * dx);
-                float a = fminf(t.amax, r1.y * ex2_approx(p2));
-                a = (!(p2 > 0.0f) && !(a < ALPHA_MIN)) ? a : 0.f;
-                const float nT = fmaf(-a, Tc, Tc);
-                const bool stop = nT <= T_STOP;
-                const float w = stop ? 0.f : a * Tc;
-                const float4* f = reinterpret_cast<const float4*>(sm.feat[j]);
+                const Sample sp = eval_sample(t, r0, r1);
+                const float a = (!(sp.p2 > 0.0f) && !(sp.a < ALPHA_MIN)) ? sp.a : 0.f;
+                fwd_step<true>(a, base, j, T, Tc, last, [&](float w) {
+                    const float4* f = reinterpret_cast<const float4*>(sm.feat[j]);
 #pragma unroll
-                for (int q = 0; q < CH / 4; ++q) {
-                    const float4 fq = f[q];
-                    C[4 * q + 0] = fmaf(fq.x, w, C[4 * q + 0]);
-                    C[4 * q + 1] = fmaf(fq.y, w, C[4 * q + 1]);
-                    C[4 * q + 2] = fmaf(fq.z, w, C[4 * q + 2]);
-                    C[4 * q + 3] = fmaf(fq.w, w, C[4 * q + 3]);
-                }
-                last = (w > 0.f) ? base + j + 1 : last;
-                T = stop ? T : nT;
-                Tc = stop ? 0.f : nT;
+                    for (int q = 0; q < CH / 4; ++q) {
+                        const float4 fq = f[q];
+                        C[4 * q + 0] = fmaf(fq.x, w, C[4 * q + 0]);
+                        C[4 * q + 1] = fmaf(fq.y, w, C[4 * q + 1]);
+                        C[4 * q + 2] = fmaf(fq.z, w, C[4 * q + 2]);
+                        C[4 * q + 3] = fmaf(fq.w, w, C[4 * q + 3]);
+                    }
+                });
             }
         }
     }
@@ -837,14 +911,14 @@ __global__ void __launch_bounds__(BLOCK_PIX, CH > 16 ? 2 : CH > 8 ? 3 : 4) blend
     }
 }
 
-// Backward: blend_bwd_tr_kernel's reverse walk (up to the warp's deepest contributor), per-warp value tile of GE entries and
-// reduce phase.  The warp's v_image tile [32 pixels][CH] sits in shared memory; the feature gradient is reduced lane = channel:
-// for each entry lane c sums fac[pixel] * v[pixel][c] over the warp's 32 pixels (fac broadcast, v rows conflict-free, no
-// shuffles) and issues one atomic, so a 32-channel entry leaves as one coalesced 128-byte reduction.  At CH < 32 the warp takes
-// 32 / CH entries at a time.
-// GEOM = false (the geometry needs no gradient): per sample only the transmittance walk and fac = alpha T; no <f, v> product, no
-// moments, no geometry atomics, no feature staging.  GEOM = true: S = <f_j, v_pix> over the chunk's CH channels (the pixel's v row
-// in registers, the feature row broadcast from shared memory), then K7's moment reduction and geometry atomics; ABS: absgrad.
+// Backward: blend_bwd_tr_kernel's reverse walk, per-warp value tile of GE entries and reduce phase, on the same helpers
+// (deepest_contributor, eval_sample, unblend, sample_grad, reduce_moments, entry_grad).  The warp's v_image tile [32 pixels][CH]
+// sits in shared memory; the feature gradient is reduced lane = channel: for each entry lane c sums fac[pixel] * v[pixel][c] over
+// the warp's 32 pixels (fac broadcast, v rows conflict-free, no shuffles) and issues one atomic, so a 32-channel entry leaves as
+// one coalesced 128-byte reduction.  At CH < 32 the warp takes 32 / CH entries at a time.
+// GEOM = false (the geometry needs no gradient): per sample only unblend; no <f, v> product, no moments, no geometry atomics, no
+// feature staging.  GEOM = true: S = <f_j, v_pix> over the chunk's CH channels (the pixel's v row in registers, the feature row
+// broadcast from shared memory) for sample_grad, then the moments and geometry atomics; ABS: absgrad.
 template <int CH, bool GEOM, bool ABS>
 struct FeatBwdSmem {
     static constexpr int VAL_BYTES = GEOM ? (ABS ? 16 : 8) : 4;   // per (entry, pixel): {fac}, {go, fac} or {go, fac, |gx|, |gy|}
@@ -913,12 +987,8 @@ __global__ void __launch_bounds__(BLOCK_PIX, GEOM ? (CH > 16 ? 1 : 2) : 3) blend
         tail = Tf * (va - bg_dot);   // d(out)/d(alpha_i) through everything behind the last contributor
     }
 
-    const int wmax = __reduce_max_sync(FULL, last);
-    if (lane == 0) sm.wmax[warp] = wmax;
-    __syncthreads();
-    int max_last = 0;
-#pragma unroll
-    for (int w = 0; w < NWARP; ++w) max_last = max(max_last, sm.wmax[w]);
+    int wmax;
+    const int max_last = deepest_contributor(last, sm.wmax, warp, lane, wmax);
     if (max_last == 0) return;
 
     float T = Tf;
@@ -958,17 +1028,12 @@ __global__ void __launch_bounds__(BLOCK_PIX, GEOM ? (CH > 16 ? 1 : 2) : 3) blend
                 const int j = my_list[ii - u];
                 const float4 r0 = s_rec[j * 3 + 0];
                 const float4 r1 = s_rec[j * 3 + 1];
-                const float dx = r0.x - t.pxf, dy = r0.y - t.pyf;
-                const float p2 = fmaf(r1.x * dy, dy, fmaf(r0.w, dy, r0.z * dx) * dx);
-                const float G = ex2_approx(p2);
-                const float oG = r1.y * G;
-                const float a = fminf(t.amax, oG);
-                const bool valid = (j < rel_last) && !(p2 > 0.0f) && (a >= ALPHA_MIN);
+                const Sample sp = eval_sample(t, r0, r1);
+                const bool valid = (j < rel_last) && !(sp.p2 > 0.0f) && (sp.a >= ALPHA_MIN);
                 float go = 0.f, fac = 0.f, gax = 0.f, gay = 0.f;
                 if (valid) {
-                    const float ra = 1.0f / (1.0f - a);
-                    T *= ra;
-                    fac = a * T;
+                    float ra;
+                    fac = unblend(sp.a, T, ra);
                     vm |= 1u << u;
                     if (GEOM) {
                         const float4* f = reinterpret_cast<const float4*>(sm.feat[GEOM ? j : 0]);
@@ -981,14 +1046,8 @@ __global__ void __launch_bounds__(BLOCK_PIX, GEOM ? (CH > 16 ? 1 : 2) : 3) blend
                             S = fmaf(fq.z, vo[4 * q + 2], S);
                             S = fmaf(fq.w, vo[4 * q + 3], S);
                         }
-                        const float v_al = fmaf(T, S, ra * (tail - Dacc));
-                        Dacc = fmaf(fac, S, Dacc);
-                        if (oG <= 0.999f) go = G * v_al;
-                        if (ABS) {
-                            const float vsg = r1.y * go * (2.0f / LOG2E);
-                            gax = fabsf(vsg * fmaf(r0.z, dx, 0.5f * r0.w * dy));
-                            gay = fabsf(vsg * fmaf(0.5f * r0.w, dx, r1.x * dy));
-                        }
+                        const SampleGrad sg = sample_grad<true, ABS>(sp, r0, r1, S, ra, T, fac, tail, Dacc);
+                        Dacc = sg.D; go = sg.go; gax = sg.gax; gay = sg.gay;
                     }
                 }
                 if (!GEOM) *reinterpret_cast<float*>(my_val + u * VAL_ROW) = fac;
@@ -1016,64 +1075,24 @@ __global__ void __launch_bounds__(BLOCK_PIX, GEOM ? (CH > 16 ? 1 : 2) : 3) blend
                 }
             }
             if (GEOM) {
-                // ---- geometry: blend_bwd_tr_kernel's moment reduction, lane (re, rh) over pixels 16 rh .. 16 rh + 15
-                float R0 = 0.f, R0x = 0.f, R0xx = 0.f, R1 = 0.f, R1x = 0.f, R1xx = 0.f;
-                float Ax = 0.f, Ay = 0.f;
-#pragma unroll
-                for (int k2 = 0; k2 < 8; ++k2) {
-                    float4 v;                             // {go, fac} of pixels 2 k2, 2 k2 + 1
-                    if (ABS) {
-                        const float4 va = my_row[2 * k2], vb = my_row[2 * k2 + 1];
-                        v = make_float4(va.x, va.y, vb.x, vb.y);
-                        Ax += va.z + vb.z;
-                        Ay += va.w + vb.w;
-                    } else {
-                        v = my_row[k2];
-                    }
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int k = 2 * k2 + e;
-                        const float gk = e ? v.z : v.x;
-                        const float x = float(k & 7);
-                        if (k < 8) { R0 += gk; if (k & 7) { R0x = fmaf(gk, x, R0x); R0xx = fmaf(gk, x * x, R0xx); } }
-                        else       { R1 += gk; if (k & 7) { R1x = fmaf(gk, x, R1x); R1xx = fmaf(gk, x * x, R1xx); } }
-                    }
-                }
-                float S0 = R0 + R1, Sx = R0x + R1x, Sxx = R0xx + R1xx;
-                float Sy = fmaf(hh, S0, R1), Sxy = fmaf(hh, Sx, R1x), Syy = fmaf(hh * hh, S0, fmaf(2.0f * hh, R1, R1));
-                S0 += __shfl_xor_sync(FULL, S0, 16);
-                Sx += __shfl_xor_sync(FULL, Sx, 16);
-                Sy += __shfl_xor_sync(FULL, Sy, 16);
-                Sxx += __shfl_xor_sync(FULL, Sxx, 16);
-                Sxy += __shfl_xor_sync(FULL, Sxy, 16);
-                Syy += __shfl_xor_sync(FULL, Syy, 16);
-                if (ABS) {
-                    Ax += __shfl_xor_sync(FULL, Ax, 16);
-                    Ay += __shfl_xor_sync(FULL, Ay, 16);
-                }
+                const Moments mo = reduce_moments<ABS>(my_row, hh, [](int, float) {}, []() {});
                 if ((present >> re) & 1u) {
                     const int j = my_list[ii - re];
                     const int g = __float_as_int(s_rec[j * 3 + 2].z);
                     if (rh == 0) {
                         const float4 r0 = s_rec[j * 3 + 0];
                         const float4 r1 = s_rec[j * 3 + 1];
-                        const float A = r0.z * (-2.0f / LOG2E), B = r0.w * (-1.0f / LOG2E), Cc = r1.x * (-2.0f / LOG2E);
-                        const float ex = r0.x - bx0, ey = r0.y - by0;
-                        const float no = -r1.y;
-                        const float M1 = no * fmaf(ex, S0, -Sx), M2 = no * fmaf(ey, S0, -Sy);
-                        const float M3 = no * fmaf(ex, fmaf(ex, S0, -2.0f * Sx), Sxx);
-                        const float M4 = no * (fmaf(ex, fmaf(ey, S0, -Sy), Sxy) - ey * Sx);
-                        const float M5 = no * fmaf(ey, fmaf(ey, S0, -2.0f * Sy), Syy);
-                        atomicAdd(v_xy + 2 * int64_t(g), A * M1 + B * M2);
-                        atomicAdd(v_xy + 2 * int64_t(g) + 1, B * M1 + Cc * M2);
-                        atomicAdd(v_conic + 3 * int64_t(g), 0.5f * M3);
-                        atomicAdd(v_conic + 3 * int64_t(g) + 1, M4);
-                        atomicAdd(v_conic + 3 * int64_t(g) + 2, 0.5f * M5);
+                        const EntryGrad eg = entry_grad(r0, r1, bx0, by0, mo);
+                        atomicAdd(v_xy + 2 * int64_t(g), eg.mean_x());
+                        atomicAdd(v_xy + 2 * int64_t(g) + 1, eg.mean_y());
+                        atomicAdd(v_conic + 3 * int64_t(g), eg.conic0());
+                        atomicAdd(v_conic + 3 * int64_t(g) + 1, eg.conic1());
+                        atomicAdd(v_conic + 3 * int64_t(g) + 2, eg.conic2());
                     } else {
-                        atomicAdd(v_opacity + g, S0);
+                        atomicAdd(v_opacity + g, mo.S0);
                         if (ABS) {
-                            atomicAdd(v_xy_abs + 2 * int64_t(g), Ax);
-                            atomicAdd(v_xy_abs + 2 * int64_t(g) + 1, Ay);
+                            atomicAdd(v_xy_abs + 2 * int64_t(g), mo.Ax);
+                            atomicAdd(v_xy_abs + 2 * int64_t(g) + 1, mo.Ay);
                         }
                     }
                 }
@@ -1083,34 +1102,13 @@ __global__ void __launch_bounds__(BLOCK_PIX, GEOM ? (CH > 16 ? 1 : 2) : 3) blend
     }
 }
 
-// Sets the dynamic shared-memory limit of a kernel once (first launch) and launches it.
-template <typename Kernel, typename... Args>
-int launch_dyn(Kernel kernel, const cudaError_t& attr_rc, size_t smem, dim3 grid, cudaStream_t s, const char* what, Args... args) {
-    if (attr_rc != cudaSuccess) {
-        set_error("%s: cudaFuncSetAttribute failed: %s", what, cudaGetErrorString(attr_rc));
-        return B200GS_ECUDA;
-    }
-    kernel<<<grid, BLOCK_PIX, smem, s>>>(args...);
-    B200GS_LAUNCH_CHECK();
-    return B200GS_OK;
-}
-
-template <typename Kernel>
-cudaError_t set_smem(Kernel kernel, size_t smem) {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    return e;
-}
-
 template <int CH>
 int feat_fwd_chunk(dim3 grid, int gx, int width, int height, const int32_t* ranges, const int32_t* ids, const float* xy, const float* conic,
                    const float* opacity, const float* features, int D, int c0, int cw, const float* bg, float* image, float* final_T,
                    int32_t* n_contrib, float* alpha, cudaStream_t s) {
-    const auto kernel = blend_feat_fwd_kernel<CH>;
-    static const cudaError_t attr_rc = set_smem(kernel, sizeof(FeatFwdSmem<CH>));
-    return launch_dyn(kernel, attr_rc, sizeof(FeatFwdSmem<CH>), grid, s, "blend_feat_fwd", width, height, gx,
-                      reinterpret_cast<const int2*>(ranges), ids, xy, conic, opacity, features, D, c0, cw, bg, image, final_T, n_contrib,
-                      alpha);
+    return launch_dyn<blend_feat_fwd_kernel<CH>, sizeof(FeatFwdSmem<CH>)>(grid, s, "blend_feat_fwd", width, height, gx,
+                                                                        reinterpret_cast<const int2*>(ranges), ids, xy, conic, opacity,
+                                                                        features, D, c0, cw, bg, image, final_T, n_contrib, alpha);
 }
 
 template <int CH, bool GEOM, bool ABS>
@@ -1118,12 +1116,9 @@ int feat_bwd_chunk(dim3 grid, int gx, int width, int height, const int32_t* rang
                    const float* opacity, const float* features, int D, int c0, int cw, const float* bg, const float* final_T,
                    const int32_t* n_contrib, const float* v_image, const float* v_alpha, float* v_features, float* v_xy, float* v_conic,
                    float* v_opacity, float* v_xy_abs, cudaStream_t s) {
-    typedef FeatBwdSmem<CH, GEOM, ABS> Smem;
-    const auto kernel = blend_feat_bwd_kernel<CH, GEOM, ABS>;
-    static const cudaError_t attr_rc = set_smem(kernel, sizeof(Smem));
-    return launch_dyn(kernel, attr_rc, sizeof(Smem), grid, s, "blend_feat_bwd", width, height, gx, reinterpret_cast<const int2*>(ranges), ids,
-                      xy, conic, opacity, features, D, c0, cw, bg, final_T, n_contrib, v_image, v_alpha, v_features, v_xy, v_conic,
-                      v_opacity, v_xy_abs);
+    return launch_dyn<blend_feat_bwd_kernel<CH, GEOM, ABS>, sizeof(FeatBwdSmem<CH, GEOM, ABS>)>(
+        grid, s, "blend_feat_bwd", width, height, gx, reinterpret_cast<const int2*>(ranges), ids, xy, conic, opacity, features, D, c0, cw,
+        bg, final_T, n_contrib, v_image, v_alpha, v_features, v_xy, v_conic, v_opacity, v_xy_abs);
 }
 
 }  // namespace
