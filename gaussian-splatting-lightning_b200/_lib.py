@@ -92,6 +92,10 @@ _SIGNATURES = {
     "b200gs_depth_to_normal": (c_int32, [c_int32] * 2 + [_P] * 2 + [c_int64] * 2 + [_P] + [c_int64] * 2 + [_P, _P]),
     "b200gs_knn_workspace_bytes": (c_size_t, [c_int64]),
     "b200gs_knn_mean_dist2": (c_int32, [c_int64, _P, _P, _P, c_size_t, _P]),
+    "b200gs_knn_points": (c_int32, [c_int64, _P, c_int64, _P, c_int32, _P, _P, _P, c_size_t, _P]),
+    "b200gs_similarity_reg_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int32, c_int32, c_int32]),
+    "b200gs_similarity_reg_fwd": (c_int32, [c_int64, c_int32, _P, c_int64, c_int32, _P, _P, c_int32, c_float, c_float, _P, c_size_t, _P, _P, _P]),
+    "b200gs_similarity_reg_bwd": (c_int32, [c_int64, c_int32, _P, c_int64, c_int32, _P, _P, c_int32, c_float, c_float, _P, c_size_t, _P, _P, _P]),
     "b200gs_sh_fwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P]),
     "b200gs_sh_bwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P, _P, _P]),
     "b200gs_sh_split_fwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P, _P, _P]),

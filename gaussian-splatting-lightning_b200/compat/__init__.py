@@ -11,6 +11,7 @@ import importlib.abc
 import importlib.util
 import sys
 import types
+from collections import namedtuple
 
 import torch
 
@@ -89,6 +90,16 @@ def install(force: bool = False):
         sys.modules["gsplat.utils"] = _gsplat_utils_module()
     elif "gsplat.utils" not in sys.modules and not any(isinstance(f, _OnImport) and f.name == "gsplat.utils" for f in sys.meta_path):
         sys.meta_path.insert(0, _OnImport("gsplat.utils", _gsplat_utils_module))
+    # pytorch3d.ops.knn_points (internal/metrics/appearance_feature_similarity_regularization_metrics.py:8, segany_splatting.py:276),
+    # the same way; pytorch3d.ops.iou_box3d (partition_lod_renderer.py:8) raises ImportError on import
+    for name, make in (("pytorch3d", _pytorch3d_module), ("pytorch3d.ops", _pytorch3d_ops_module),
+                       ("pytorch3d.ops.iou_box3d", _pytorch3d_refused)):
+        if force and make is not _pytorch3d_refused:
+            sys.modules[name] = make()
+        elif name not in sys.modules and not any(isinstance(f, _OnImport) and f.name == name for f in sys.meta_path):
+            sys.meta_path.insert(0, _OnImport(name, make))      # the refusal always goes through the hook, so it names what exists
+    if force:
+        sys.modules["pytorch3d"].ops = sys.modules["pytorch3d.ops"]
 
 
 def _fused_ssim_module():
@@ -103,6 +114,55 @@ def _gsplat_utils_module():
     m = types.ModuleType("gsplat.utils")
     m.depth_to_normal = metrics.depth_to_normal
     return m
+
+
+KNN = namedtuple("KNN", ["dists", "idx", "knn"])
+
+
+def knn_points(p1, p2, lengths1=None, lengths2=None, norm: int = 2, K: int = 1, version: int = -1, return_nn: bool = False,
+               return_sorted: bool = True):
+    """pytorch3d.ops.knn_points on ``ops.knn_points`` (one search per batch entry): p1 [B,S,3] and p2 [B,N,3] float32 CUDA,
+    ``lengths1`` / ``lengths2`` None, ``norm`` 2, ``return_sorted`` True, ``return_nn`` False, 1 <= K <= min(32, N), and no
+    gradient (inputs that require grad while grad is enabled are refused).  ``version`` is ignored.  Returns KNN(dists [B,S,K] squared
+    distances, idx [B,S,K] int64, None), ascending."""
+    from .. import ops
+    unsupported = []
+    if lengths1 is not None or lengths2 is not None:
+        unsupported.append("lengths1 / lengths2")
+    if norm != 2:
+        unsupported.append(f"norm={norm}")
+    if return_nn:
+        unsupported.append("return_nn=True")
+    if not return_sorted:
+        unsupported.append("return_sorted=False")
+    if torch.is_grad_enabled() and (p1.requires_grad or p2.requires_grad):
+        unsupported.append("inputs that require grad")
+    if unsupported:
+        raise NotImplementedError(f"b200gs's pytorch3d.ops.knn_points does not support {', '.join(unsupported)}: it provides norm=2, "
+                                  "return_sorted=True, return_nn=False and lengths=None without gradients")
+    if p1.dim() != 3 or p2.dim() != 3 or p1.shape[0] != p2.shape[0]:
+        raise ValueError(f"p1 and p2 must be [B, S, 3] and [B, N, 3], got {tuple(p1.shape)} and {tuple(p2.shape)}")
+    results = [ops.knn_points(p1[b], p2[b], K) for b in range(p1.shape[0])]
+    return KNN(torch.stack([r[0] for r in results]), torch.stack([r[1] for r in results]), None)
+
+
+def _pytorch3d_module():
+    m = types.ModuleType("pytorch3d")
+    m.__path__ = []
+    return m
+
+
+def _pytorch3d_ops_module():
+    m = types.ModuleType("pytorch3d.ops")
+    m.__path__ = []
+    m.knn_points = knn_points
+    m.KNN = KNN
+    return m
+
+
+def _pytorch3d_refused():
+    raise ImportError("b200gs provides only pytorch3d.ops.knn_points; pytorch3d.ops.iou_box3d (partition_lod_renderer.py) is not "
+                      "provided")
 
 
 def _tcnn_module():

@@ -42,7 +42,7 @@ using namespace b200gs;
 extern "C" {
 
 const char* b200gs_last_error(void) { return g_error; }
-int b200gs_version(void) { return 232; }
+int b200gs_version(void) { return 233; }
 int64_t b200gs_launch_count(void) { return (int64_t)g_launches.load(std::memory_order_relaxed); }
 
 int b200gs_project_fwd(const B200gsView* view, int64_t n, const float* means, const float* scales, const float* quats,
@@ -711,6 +711,53 @@ int b200gs_knn_mean_dist2(int64_t n, const float* points, float* mean_dist2, voi
     B200GS_CHECK_ARG(n >= 0, "n < 0");
     B200GS_CHECK_ARG(n == 0 || (points && mean_dist2 && workspace), "NULL pointer");
     return launch_knn_mean_dist2(n, points, mean_dist2, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int b200gs_knn_points(int64_t s, const float* queries, int64_t n, const float* points, int32_t k, float* dists, int64_t* idx, void* workspace,
+                      size_t workspace_bytes, void* stream) {
+    B200GS_CHECK_ARG(s >= 0 && n >= 0, "negative size");
+    B200GS_CHECK_ARG(k >= 1 && k <= 32, "K must be 1..32");
+    B200GS_CHECK_ARG(k <= n, "K exceeds the number of reference points");
+    B200GS_CHECK_ARG(points && workspace, "NULL pointer");
+    B200GS_CHECK_ARG(s == 0 || (queries && dists && idx), "NULL pointer");
+    return launch_knn_points(s, queries, n, points, k, dists, idx, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+// shared by the similarity entry points; returns the error code, or 0 when the arguments are valid
+static int check_similarity(const char* fn, int64_t n, int32_t d, const float* features, int64_t s, int32_t k, const int64_t* idx,
+                            const float* dists, int32_t kind, const void* workspace, size_t workspace_bytes, bool backward) {
+    auto fail = [&](int rc, const char* msg) { set_error("%s: %s", fn, msg); return rc; };
+    if (kind != 0 && kind != 1) return fail(B200GS_EINVAL, "kind must be 0 (Cosine) or 1 (Euclidean)");
+    if (d < 1 || d > 256) return fail(B200GS_EINVAL, "feature dimension must be 1..256");
+    if (k < 2 || k > 32) return fail(B200GS_EINVAL, "K must be 2..32");
+    if (s < 1 || n < 1) return fail(B200GS_EINVAL, "S and N must be >= 1");
+    if (n >= (int64_t(1) << 30) || s * k >= (int64_t(1) << 30)) return fail(B200GS_EINVAL, "N and S K must be < 2^30");
+    if (!(features && idx && dists && workspace)) return fail(B200GS_EINVAL, "NULL pointer");
+    if (workspace_bytes < similarity_reg_workspace_bytes(n, s, k, d, backward)) return fail(B200GS_ENOSPACE, "workspace too small");
+    return 0;
+}
+
+size_t b200gs_similarity_reg_workspace_bytes(int64_t n, int64_t s, int32_t k, int32_t d, int32_t backward) {
+    const bool ok = n >= 1 && n < (int64_t(1) << 30) && s >= 1 && k >= 2 && k <= 32 && s * k < (int64_t(1) << 30) && d >= 1 && d <= 256;
+    return ok ? similarity_reg_workspace_bytes(n, s, k, d, backward != 0) : 0;
+}
+
+int b200gs_similarity_reg_fwd(int64_t n, int32_t d, const float* features, int64_t s, int32_t k, const int64_t* idx, const float* dists,
+                              int32_t kind, float decay, float lambda, void* workspace, size_t workspace_bytes, float* out, float* weights,
+                              void* stream) {
+    if (int rc = check_similarity(__func__, n, d, features, s, k, idx, dists, kind, workspace, workspace_bytes, false)) return rc;
+    B200GS_CHECK_ARG(out, "NULL pointer");
+    return launch_similarity_reg_fwd(n, d, features, s, k, idx, dists, kind, decay, lambda, static_cast<float*>(workspace), out, weights,
+                                     (cudaStream_t)stream);
+}
+
+int b200gs_similarity_reg_bwd(int64_t n, int32_t d, const float* features, int64_t s, int32_t k, const int64_t* idx, const float* dists,
+                              int32_t kind, float decay, float lambda, void* workspace, size_t workspace_bytes, const float* v_loss,
+                              float* v_features, void* stream) {
+    if (int rc = check_similarity(__func__, n, d, features, s, k, idx, dists, kind, workspace, workspace_bytes, true)) return rc;
+    B200GS_CHECK_ARG(v_loss && v_features, "NULL pointer");
+    return launch_similarity_reg_bwd(n, d, features, s, k, idx, dists, kind, decay, lambda, static_cast<float*>(workspace), v_loss,
+                                     v_features, (cudaStream_t)stream);
 }
 
 int b200gs_sh_fwd(int32_t degree, int32_t sh_stride, int64_t n, const float* dirs, const float* coeffs, float* rgb, void* stream) {

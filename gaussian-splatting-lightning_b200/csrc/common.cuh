@@ -242,8 +242,23 @@ int launch_vis_loss_fwd(int width, int height, const float* img, const float* gt
 int launch_vis_loss_bwd(int width, int height, const float* img, const float* gt, const float* vis, const uint8_t* mask, const float* ws,
                         float lambda_dssim, float vis_reg_factor, const float* v_loss, float* v_img, float* v_vis, cudaStream_t s);
 
+// k nearest neighbours on one hash grid over the reference points (knn.cu); both entry points share its workspace layout
 size_t knn_workspace_bytes(int64_t n);
 int launch_knn_mean_dist2(int64_t n, const float* points, float* out, void* ws, size_t ws_bytes, cudaStream_t s);
+int launch_knn_points(int64_t s_q, const float* queries, int64_t n, const float* points, int k, float* dists, int64_t* idx, void* ws,
+                      size_t ws_bytes, cudaStream_t s);
+// Stable LSD sort of uint2 {key, payload} records by the low `bits` bits of the key (knn.cu: a histogram launch, then one onesweep
+// pass per 8 bits), a and b ping-pong buffers of n records; *out is the one that holds the result.  The scratch must be zero.
+int record_key_bits(int64_t max_key);
+size_t record_sort_scratch_bytes(int64_t n);
+int launch_record_sort(int64_t n, int bits, uint2* a, uint2* b, void* scratch, cudaStream_t s, const uint2** out);
+
+// similarity regulariser (similarity_reg.cu): features [N,D] contiguous, idx [S,K] int64, dists [S,K]; kind 0 Cosine, 1 Euclidean
+size_t similarity_reg_workspace_bytes(int64_t n, int64_t s, int k, int d, bool backward);
+int launch_similarity_reg_fwd(int64_t n, int d, const float* features, int64_t s, int k, const int64_t* idx, const float* dists, int kind,
+                              float decay, float lambda, float* ws, float* out, float* weights, cudaStream_t st);
+int launch_similarity_reg_bwd(int64_t n, int d, const float* features, int64_t s, int k, const int64_t* idx, const float* dists, int kind,
+                              float decay, float lambda, float* ws, const float* v_loss, float* v_features, cudaStream_t st);
 
 int64_t loss_blocks(int channels, int width, int height);
 int launch_loss_fwd(int channels, int width, int height, const float* img, const float* gt, float* dmaps, float* partials, cudaStream_t s);

@@ -1,54 +1,72 @@
 // distCUDA2 of simple-knn (the initialiser of the Gaussians' scales: internal/models/vanilla_gaussian.py:122-125 calls
 // `simple_knn._C.distCUDA2(points)` once per run): for every point the MEAN of the squared distances to its 3 nearest neighbours.
 // simple-knn@44f7642 orders the points along a Morton curve and prunes with bounding boxes; the result is the exact 3-NN mean.
-// Here: a uniform hash grid (about two points per cell), the points sorted by cell with the library's own onesweep radix
-// passes, a dense first/last table per cell, and one thread per point that searches growing shells of cells until the third
-// best distance is no larger than the distance to the unsearched region — also the exact 3-NN (ties aside).
+// pytorch3d's knn_points (the similarity regulariser of internal/metrics/appearance_feature_similarity_regularization_metrics.py
+// and SegAny's feature smoothing): for every query the K <= 32 nearest reference points, self included, in ascending order.
+// Both run on one grid build: a uniform hash grid (about two points per cell) sized on the device from the bounding box, the points
+// sorted by cell with the library's own onesweep radix passes, a dense first/last table per cell; then one thread per point or query
+// searches growing shells of cells until its K-th best distance is no larger than the distance to the unsearched region.  Nothing is
+// copied to the host: the radix pass count follows from the host-known cell capacity, and the kernels read the grid from the
+// workspace.
 #include <float.h>
 
 #include "common.cuh"
+#include "knn_grid.h"
 #include "onesweep.cuh"
 
 namespace b200gs {
 
 namespace {
 
-struct KnnGrid {
-    float lox, loy, loz, cs, inv_cs;
-    int gx, gy, gz;
-};
+// clamped before the conversion, so an infinite or NaN offset (a non-finite point, an overflowing difference) lands in an edge cell
+__device__ __forceinline__ int cell_coord(float v, float lo, float inv_cs, int g) { return (int)fminf(fmaxf((v - lo) * inv_cs, 0.f), (float)(g - 1)); }
 
-__device__ __forceinline__ int cell_coord(float v, float lo, float inv_cs, int g) { return min(g - 1, max(0, (int)((v - lo) * inv_cs))); }
+// float -> uint32 with the same order (finite values), and back
+__device__ __forceinline__ uint32_t ordered_key(float f) {
+    const uint32_t u = __float_as_uint(f);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float from_ordered_key(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
 
-__global__ void __launch_bounds__(256) knn_bounds_kernel(int64_t n, const float* __restrict__ pts, float* __restrict__ bounds /*[6]: min xyz, max xyz*/) {
+// bounds[0..2] = ~key(min xyz), bounds[3..5] = key(max xyz) over the points whose three coordinates are finite: both maxima, so the
+// zero-initialised workspace is the identity (and decodes to NaN bounds, which the sizing treats as empty, when no point is finite)
+__global__ void __launch_bounds__(256) knn_bounds_kernel(int64_t n, const float* __restrict__ pts, uint32_t* __restrict__ bounds) {
     float lo[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, hi[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
-    for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += int64_t(gridDim.x) * blockDim.x)
-#pragma unroll
-        for (int a = 0; a < 3; ++a) {
-            const float v = pts[3 * i + a];
-            lo[a] = fminf(lo[a], v);
-            hi[a] = fmaxf(hi[a], v);
-        }
+    for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += int64_t(gridDim.x) * blockDim.x) {
+        const float x = pts[3 * i], y = pts[3 * i + 1], z = pts[3 * i + 2];
+        if (!(isfinite(x) && isfinite(y) && isfinite(z))) continue;
+        lo[0] = fminf(lo[0], x); lo[1] = fminf(lo[1], y); lo[2] = fminf(lo[2], z);
+        hi[0] = fmaxf(hi[0], x); hi[1] = fmaxf(hi[1], y); hi[2] = fmaxf(hi[2], z);
+    }
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            lo[a] = fminf(lo[a], __shfl_xor_sync(0xffffffffu, lo[a], o));
-            hi[a] = fmaxf(hi[a], __shfl_xor_sync(0xffffffffu, hi[a], o));
-        }
+        lo[a] = warp_reduce<Min>(lo[a]);
+        hi[a] = warp_reduce<Max>(hi[a]);
     }
     if ((threadIdx.x & 31) == 0) {
 #pragma unroll
-        for (int a = 0; a < 3; ++a) {   // float atomics through the order-preserving int view (all values finite)
-            atomicMin(reinterpret_cast<int*>(bounds + a), lo[a] >= 0.f ? __float_as_int(lo[a]) : (int)(0x80000000u - (unsigned)__float_as_int(lo[a])));
-            atomicMax(reinterpret_cast<int*>(bounds + 3 + a), hi[a] >= 0.f ? __float_as_int(hi[a]) : (int)(0x80000000u - (unsigned)__float_as_int(hi[a])));
+        for (int a = 0; a < 3; ++a) {
+            atomicMax(bounds + a, ~ordered_key(lo[a]));
+            atomicMax(bounds + 3 + a, ordered_key(hi[a]));
         }
     }
 }
 
-__global__ void __launch_bounds__(256) knn_keys_kernel(int64_t n, const float* __restrict__ pts, const KnnGrid g, uint2* __restrict__ rec) {
+// size_knn_grid (knn_grid.h) in one thread
+__global__ void knn_grid_kernel(int64_t n, const uint32_t* __restrict__ bounds, int64_t max_cells, KnnGrid* __restrict__ grid) {
+    float lo[3], hi[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        lo[a] = from_ordered_key(~bounds[a]);
+        hi[a] = from_ordered_key(bounds[3 + a]);
+    }
+    *grid = size_knn_grid(lo, hi, n, max_cells);
+}
+
+__global__ void __launch_bounds__(256) knn_keys_kernel(int64_t n, const float* __restrict__ pts, const KnnGrid* __restrict__ grid, uint2* __restrict__ rec) {
     const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    const KnnGrid g = *grid;
     const int cx = cell_coord(pts[3 * i], g.lox, g.inv_cs, g.gx), cy = cell_coord(pts[3 * i + 1], g.loy, g.inv_cs, g.gy),
               cz = cell_coord(pts[3 * i + 2], g.loz, g.inv_cs, g.gz);
     rec[i] = make_uint2((uint32_t)((cz * g.gy + cy) * g.gx + cx), (uint32_t)i);
@@ -75,9 +93,10 @@ __device__ __forceinline__ void knn_insert(float d, float& b0, float& b1, float&
 }
 
 __global__ void __launch_bounds__(128) knn_search_kernel(int64_t n, const float4* __restrict__ sorted, const int* __restrict__ cell_lo,
-                                                         const int* __restrict__ cell_hi, const KnnGrid g, float* __restrict__ out) {
+                                                         const int* __restrict__ cell_hi, const KnnGrid* __restrict__ grid, float* __restrict__ out) {
     const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    const KnnGrid g = *grid;
     const float4 p = sorted[i];
     const int cx = cell_coord(p.x, g.lox, g.inv_cs, g.gx), cy = cell_coord(p.y, g.loy, g.inv_cs, g.gy), cz = cell_coord(p.z, g.loz, g.inv_cs, g.gz);
     float b0 = FLT_MAX, b1 = FLT_MAX, b2 = FLT_MAX;
@@ -120,6 +139,7 @@ __global__ void __launch_bounds__(128) knn_search_kernel(int64_t n, const float4
 
 // histograms of the four key bytes of the uint2 records: the digit counts of all the radix passes at once
 constexpr int HIST_THREADS = 256;
+constexpr int SORT_IPT = 8;
 
 __global__ void __launch_bounds__(HIST_THREADS) hist4_kernel(const uint2* __restrict__ recs, const int64_t* __restrict__ d_n, int64_t cap,
                                                              uint32_t* __restrict__ hist /*[4][RADIX]*/) {
@@ -142,113 +162,228 @@ __global__ void __launch_bounds__(HIST_THREADS) hist4_kernel(const uint2* __rest
     }
 }
 
-struct KnnLayout {
-    size_t bounds, rec_a, rec_b, sorted, zero, zero_bytes, hist, tickets, lookback, cell_lo, cell_hi, total;
-    int64_t tiles, max_cells;
-};
+// ---- the K nearest reference points of arbitrary queries --------------------------------------------------------------
+// Insert (d, j) into the ascending list of the KC best: a fixed sequence of selects over the whole list, so it stays in registers.
+// Strict comparisons keep an earlier-inserted point ahead of a later one at the same distance.
+template <int KC>
+__device__ __forceinline__ void list_insert(float d, int j, float (&bd)[KC], int (&bi)[KC]) {
+#pragma unroll
+    for (int t = KC - 1; t > 0; --t) {
+        const bool shift = d < bd[t - 1], here = !shift && d < bd[t];
+        bi[t] = shift ? bi[t - 1] : (here ? j : bi[t]);
+        bd[t] = shift ? bd[t - 1] : (here ? d : bd[t]);
+    }
+    const bool first = d < bd[0];
+    bi[0] = first ? j : bi[0];
+    bd[0] = first ? d : bd[0];
+}
 
-constexpr int KNN_IPT = 8;
+// One thread per query: the list holds the KC >= k best (KC a power of two), the search stops once the k-th best is no larger than
+// the distance to every unsearched cell.  A query outside the grid's box is clamped to its edge cell; every cell at Chebyshev index
+// distance > r from that cell still lies more than r cells away from the query along some axis, so the bound holds there too.  The
+// bound is shrunk by 2^-10 of a cell, which covers the rounding of the cell coordinates.
+template <int KC>
+__global__ void __launch_bounds__(128) knn_query_kernel(int64_t s, const float* __restrict__ queries, int k, const float4* __restrict__ sorted,
+                                                        const int* __restrict__ cell_lo, const int* __restrict__ cell_hi,
+                                                        const KnnGrid* __restrict__ grid, const float* __restrict__ points,
+                                                        float* __restrict__ dists, int64_t* __restrict__ idx) {
+    const int64_t q = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (q >= s) return;
+    const KnnGrid g = *grid;
+    const float px = queries[3 * q], py = queries[3 * q + 1], pz = queries[3 * q + 2];
+    const int cx = cell_coord(px, g.lox, g.inv_cs, g.gx), cy = cell_coord(py, g.loy, g.inv_cs, g.gy), cz = cell_coord(pz, g.loz, g.inv_cs, g.gz);
+    float bd[KC];
+    int bi[KC];
+#pragma unroll
+    for (int t = 0; t < KC; ++t) { bd[t] = FLT_MAX; bi[t] = -1; }
+    const int rmax = max(g.gx, max(g.gy, g.gz));
+    for (int r = 0; r <= rmax; ++r) {
+        for (int dz = -r; dz <= r; ++dz) {
+            const int z = cz + dz;
+            if (z < 0 || z >= g.gz) continue;
+            for (int dy = -r; dy <= r; ++dy) {
+                const int y = cy + dy;
+                if (y < 0 || y >= g.gy) continue;
+                const bool face = (abs(dz) == r) || (abs(dy) == r);
+                for (int dx = -r; dx <= r; dx += (face ? 1 : max(1, 2 * r))) {
+                    const int x = cx + dx;
+                    if (x < 0 || x >= g.gx) continue;
+                    const int c = (z * g.gy + y) * g.gx + x;
+                    const int lo = cell_lo[c], hi = cell_hi[c];
+                    for (int j = lo; j < hi; ++j) {
+                        const float4 p = sorted[j];
+                        const float ex = p.x - px, ey = p.y - py, ez = p.z - pz;
+                        const float d = ex * ex + ey * ey + ez * ez;
+                        if (d < bd[KC - 1]) list_insert<KC>(d, __float_as_int(p.w), bd, bi);
+                    }
+                }
+            }
+        }
+        float kth = bd[0];
+#pragma unroll
+        for (int t = 1; t < KC; ++t) kth = (t == k - 1) ? bd[t] : kth;
+        const float reach = float(r) * g.cs * (1.f - 1.f / 1024.f);
+        if (kth <= reach * reach) break;
+    }
+    // Fewer than k points at a finite distance below FLT_MAX (a query with a NaN or infinite coordinate, or non-finite reference
+    // points): the empty slots take the lowest indices not in the list, as pytorch3d keeps its first candidates when no distance
+    // compares smaller, with their distances as computed (NaN or inf).  Every index written is in [0, n).
+    bool short_list = false;
+#pragma unroll
+    for (int t = 0; t < KC; ++t) short_list = short_list || (t < k && bi[t] < 0);
+    if (short_list) {
+        int next = 0;
+#pragma unroll
+        for (int t = 0; t < KC; ++t) {
+            if (t < k && bi[t] < 0) {
+                for (bool taken = true; taken;) {
+                    taken = false;
+#pragma unroll
+                    for (int u = 0; u < KC; ++u) taken = taken || bi[u] == next;
+                    if (taken) ++next;
+                }
+                const float ex = points[3 * (int64_t)next] - px, ey = points[3 * (int64_t)next + 1] - py, ez = points[3 * (int64_t)next + 2] - pz;
+                bi[t] = next++;
+                bd[t] = ex * ex + ey * ey + ez * ez;
+            }
+        }
+    }
+#pragma unroll
+    for (int t = 0; t < KC; ++t) {
+        if (t < k) {
+            dists[q * k + t] = bd[t];
+            idx[q * k + t] = bi[t];
+        }
+    }
+}
+
+struct KnnLayout {
+    size_t grid, sorted, rec_a, rec_b, zero, bounds, sort_scratch, cell_lo, cell_hi, zero_bytes, total;
+    int64_t max_cells;
+};
 
 KnnLayout knn_layout(int64_t n) {
     KnnLayout L{};
     size_t off = 0;
     auto take = [&off](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
     const size_t nn = (size_t)(n > 0 ? n : 1);
-    L.tiles = div_up64((int64_t)nn, sweep::PASS_THREADS * KNN_IPT);
     L.max_cells = (int64_t)(4 * nn + 64);
-    L.bounds = take(6 * 4);
+    L.grid = take(sizeof(KnnGrid));
+    L.sorted = take(nn * 16);
     L.rec_a = take(nn * 8);
     L.rec_b = take(nn * 8);
-    L.sorted = take(nn * 16);
-    L.zero = take(0);
-    L.hist = take(4 * sweep::RADIX * 4);
-    L.tickets = take(16 * 4);
-    L.lookback = take((size_t)4 * L.tiles * sweep::RADIX * 4);
-    L.cell_hi = take((size_t)L.max_cells * 4);      // zero-initialised with the region: empty cells have lo = hi = 0
+    L.zero = off;                                    // one memset clears the bounds, the sort's counters and the cell table
+    L.bounds = take(6 * 4);
+    L.sort_scratch = take(record_sort_scratch_bytes((int64_t)nn));
+    L.cell_hi = take((size_t)L.max_cells * 4);      // empty cells have lo = hi = 0
     L.cell_lo = take((size_t)L.max_cells * 4);
     L.zero_bytes = off - L.zero;
     L.total = off;
     return L;
 }
 
-}  // namespace
+// bounds -> grid -> cell keys -> sort by cell -> sorted points and the cell table
+int build_grid(int64_t n, const float* points, const KnnLayout& L, char* w, cudaStream_t s) {
+    uint32_t* bounds = (uint32_t*)(w + L.bounds);
+    KnnGrid* grid = (KnnGrid*)(w + L.grid);
+    uint2* rec_a = (uint2*)(w + L.rec_a);
+    uint2* rec_b = (uint2*)(w + L.rec_b);
+    B200GS_CUDA(cudaMemsetAsync(w + L.zero, 0, L.zero_bytes, s));
+    knn_bounds_kernel<<<(unsigned)min((int64_t)1184, div_up64(n, 256)), 256, 0, s>>>(n, points, bounds);
+    B200GS_LAUNCH_CHECK();
+    knn_grid_kernel<<<1, 1, 0, s>>>(n, bounds, L.max_cells, grid);
+    B200GS_LAUNCH_CHECK();
+    const unsigned blocks = (unsigned)div_up64(n, 256);
+    knn_keys_kernel<<<blocks, 256, 0, s>>>(n, points, grid, rec_a);
+    B200GS_LAUNCH_CHECK();
+    const uint2* sorted_rec = nullptr;
+    if (int rc = launch_record_sort(n, record_key_bits(L.max_cells - 1), rec_a, rec_b, w + L.sort_scratch, s, &sorted_rec)) return rc;
+    knn_gather_kernel<<<blocks, 256, 0, s>>>(n, points, sorted_rec, (float4*)(w + L.sorted), (int*)(w + L.cell_lo), (int*)(w + L.cell_hi));
+    B200GS_LAUNCH_CHECK();
+    return B200GS_OK;
+}
 
-size_t knn_workspace_bytes(int64_t n) { return knn_layout(n).total; }
-
-int launch_knn_mean_dist2(int64_t n, const float* points, float* out, void* ws, size_t ws_bytes, cudaStream_t s) {
-    if (n == 0) return B200GS_OK;
-    const KnnLayout L = knn_layout(n);
-    if (ws_bytes < L.total) {
-        set_error("knn: workspace too small (%zu < %zu)", ws_bytes, L.total);
+int check_knn_workspace(int64_t n, size_t ws_bytes) {
+    const size_t need = knn_layout(n).total;
+    if (ws_bytes < need) {
+        set_error("knn: workspace too small (%zu < %zu)", ws_bytes, need);
         return B200GS_ENOSPACE;
     }
     if (n >= (int64_t(1) << 30)) {
         set_error("knn: %lld points exceed 2^30", (long long)n);
         return B200GS_ENOSPACE;
     }
-    char* w = (char*)ws;
-    float* bounds = (float*)(w + L.bounds);
-    // bounding box (the one host round trip of this init-only routine: the grid is sized on the host)
-    const int init[6] = {0x7f7fffff, 0x7f7fffff, 0x7f7fffff, (int)0x80800001u, (int)0x80800001u, (int)0x80800001u};   // +FLT_MAX / -FLT_MAX in the ordered int view
-    B200GS_CUDA(cudaMemcpyAsync(bounds, init, sizeof(init), cudaMemcpyHostToDevice, s));
-    knn_bounds_kernel<<<(unsigned)min((int64_t)1184, div_up64(n, 256)), 256, 0, s>>>(n, points, bounds);
-    B200GS_LAUNCH_CHECK();
-    int hb[6];
-    B200GS_CUDA(cudaMemcpyAsync(hb, bounds, sizeof(hb), cudaMemcpyDeviceToHost, s));
-    B200GS_CUDA(cudaStreamSynchronize(s));
-    float b[6];
-    for (int a = 0; a < 6; ++a) {
-        const int v = hb[a];
-        const unsigned u = v >= 0 ? (unsigned)v : (0x80000000u - (unsigned)v);
-        memcpy(&b[a], &u, 4);
-    }
-    const float ex = fmaxf(b[3] - b[0], 0.f), ey = fmaxf(b[4] - b[1], 0.f), ez = fmaxf(b[5] - b[2], 0.f);
-    const float emax = fmaxf(ex, fmaxf(ey, ez));
-    KnnGrid g{};
-    g.lox = b[0]; g.loy = b[1]; g.loz = b[2];
-    // about two points per OCCUPIED-volume cell; flat or linear point sets fall back to their largest extent
-    double vol = (double)fmaxf(ex, 1e-3f * emax) * fmaxf(ey, 1e-3f * emax) * fmaxf(ez, 1e-3f * emax);
-    float cs = emax > 0.f ? (float)cbrt(vol / (0.5 * (double)n)) : 1.0f;
-    if (!(cs > 0.f)) cs = 1.0f;
-    for (;;) {   // at most 1024 cells per axis and max_cells in total
-        g.gx = (int)fminf(1024.f, floorf(ex / cs) + 1.f);
-        g.gy = (int)fminf(1024.f, floorf(ey / cs) + 1.f);
-        g.gz = (int)fminf(1024.f, floorf(ez / cs) + 1.f);
-        if ((int64_t)g.gx * g.gy * g.gz <= L.max_cells && ex / cs < 1024.f && ey / cs < 1024.f && ez / cs < 1024.f) break;
-        cs *= 1.26f;
-    }
-    g.cs = cs;
-    g.inv_cs = 1.0f / cs;
-    const int64_t n_cells = (int64_t)g.gx * g.gy * g.gz;
+    return B200GS_OK;
+}
 
-    uint2* rec_a = (uint2*)(w + L.rec_a);
-    uint2* rec_b = (uint2*)(w + L.rec_b);
-    float4* sorted = (float4*)(w + L.sorted);
-    uint32_t* hist = (uint32_t*)(w + L.hist);
-    uint32_t* tickets = (uint32_t*)(w + L.tickets);
-    uint32_t* lookback = (uint32_t*)(w + L.lookback);
-    int* cell_lo = (int*)(w + L.cell_lo);
-    int* cell_hi = (int*)(w + L.cell_hi);
-    B200GS_CUDA(cudaMemsetAsync(w + L.zero, 0, L.zero_bytes, s));
-    const unsigned blocks = (unsigned)div_up64(n, 256);
-    knn_keys_kernel<<<blocks, 256, 0, s>>>(n, points, g, rec_a);
-    B200GS_LAUNCH_CHECK();
-    hist4_kernel<<<(unsigned)min((int64_t)592, (int64_t)blocks), HIST_THREADS, 0, s>>>(rec_a, nullptr, n, hist);
-    B200GS_LAUNCH_CHECK();
+size_t sort_counters_bytes() { return align_up(4 * sweep::RADIX * 4 + 16 * 4, 256); }
+
+}  // namespace
+
+int record_key_bits(int64_t max_key) {
     int bits = 1;
-    while ((int64_t(1) << bits) < n_cells) ++bits;
-    const int passes = (bits + 7) / 8;
-    uint2* src = rec_a;
-    uint2* dst = rec_b;
-    for (int pass = 0; pass < passes; ++pass) {
-        sweep::onesweep_pass_kernel<uint2, KNN_IPT><<<(unsigned)L.tiles, sweep::PASS_THREADS, 0, s>>>(src, dst, nullptr, n, 8 * pass, hist + pass * sweep::RADIX,
-                                                                                            lookback + (size_t)pass * L.tiles * sweep::RADIX, tickets + pass);
+    while (bits < 32 && (int64_t(1) << bits) <= max_key) ++bits;
+    return bits;
+}
+
+size_t record_sort_scratch_bytes(int64_t n) {
+    const int64_t tiles = div_up64(n > 0 ? n : 1, sweep::PASS_THREADS * SORT_IPT);
+    return sort_counters_bytes() + (size_t)4 * tiles * sweep::RADIX * 4;
+}
+
+int launch_record_sort(int64_t n, int bits, uint2* a, uint2* b, void* scratch, cudaStream_t s, const uint2** out) {
+    *out = a;
+    if (n == 0) return B200GS_OK;
+    const int64_t tiles = div_up64(n, sweep::PASS_THREADS * SORT_IPT);
+    uint32_t* hist = (uint32_t*)scratch;
+    uint32_t* tickets = hist + 4 * sweep::RADIX;
+    uint32_t* lookback = (uint32_t*)((char*)scratch + sort_counters_bytes());
+    hist4_kernel<<<(unsigned)min((int64_t)592, div_up64(n, 256)), HIST_THREADS, 0, s>>>(a, nullptr, n, hist);
+    B200GS_LAUNCH_CHECK();
+    uint2* src = a;
+    uint2* dst = b;
+    for (int pass = 0; pass < (bits + 7) / 8; ++pass) {
+        sweep::onesweep_pass_kernel<uint2, SORT_IPT><<<(unsigned)tiles, sweep::PASS_THREADS, 0, s>>>(src, dst, nullptr, n, 8 * pass, hist + pass * sweep::RADIX,
+                                                                                          lookback + (size_t)pass * tiles * sweep::RADIX, tickets + pass);
         B200GS_LAUNCH_CHECK();
         uint2* t = src; src = dst; dst = t;
     }
-    knn_gather_kernel<<<blocks, 256, 0, s>>>(n, points, src, sorted, cell_lo, cell_hi);
+    *out = src;
+    return B200GS_OK;
+}
+
+size_t knn_workspace_bytes(int64_t n) { return knn_layout(n).total; }
+
+int launch_knn_mean_dist2(int64_t n, const float* points, float* out, void* ws, size_t ws_bytes, cudaStream_t s) {
+    if (n == 0) return B200GS_OK;
+    if (int rc = check_knn_workspace(n, ws_bytes)) return rc;
+    const KnnLayout L = knn_layout(n);
+    char* w = (char*)ws;
+    if (int rc = build_grid(n, points, L, w, s)) return rc;
+    knn_search_kernel<<<(unsigned)div_up64(n, 128), 128, 0, s>>>(n, (const float4*)(w + L.sorted), (const int*)(w + L.cell_lo),
+                                                                (const int*)(w + L.cell_hi), (const KnnGrid*)(w + L.grid), out);
     B200GS_LAUNCH_CHECK();
-    knn_search_kernel<<<(unsigned)div_up64(n, 128), 128, 0, s>>>(n, sorted, cell_lo, cell_hi, g, out);
+    return B200GS_OK;
+}
+
+int launch_knn_points(int64_t s_q, const float* queries, int64_t n, const float* points, int k, float* dists, int64_t* idx, void* ws,
+                      size_t ws_bytes, cudaStream_t s) {
+    if (int rc = check_knn_workspace(n, ws_bytes)) return rc;
+    if (s_q == 0) return B200GS_OK;
+    const KnnLayout L = knn_layout(n);
+    char* w = (char*)ws;
+    if (int rc = build_grid(n, points, L, w, s)) return rc;
+    const unsigned blocks = (unsigned)div_up64(s_q, 128);
+    const float4* sorted = (const float4*)(w + L.sorted);
+    const int* lo = (const int*)(w + L.cell_lo);
+    const int* hi = (const int*)(w + L.cell_hi);
+    const KnnGrid* grid = (const KnnGrid*)(w + L.grid);
+    if (k <= 1) knn_query_kernel<1><<<blocks, 128, 0, s>>>(s_q, queries, k, sorted, lo, hi, grid, points, dists, idx);
+    else if (k <= 2) knn_query_kernel<2><<<blocks, 128, 0, s>>>(s_q, queries, k, sorted, lo, hi, grid, points, dists, idx);
+    else if (k <= 4) knn_query_kernel<4><<<blocks, 128, 0, s>>>(s_q, queries, k, sorted, lo, hi, grid, points, dists, idx);
+    else if (k <= 8) knn_query_kernel<8><<<blocks, 128, 0, s>>>(s_q, queries, k, sorted, lo, hi, grid, points, dists, idx);
+    else if (k <= 16) knn_query_kernel<16><<<blocks, 128, 0, s>>>(s_q, queries, k, sorted, lo, hi, grid, points, dists, idx);
+    else knn_query_kernel<32><<<blocks, 128, 0, s>>>(s_q, queries, k, sorted, lo, hi, grid, points, dists, idx);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }

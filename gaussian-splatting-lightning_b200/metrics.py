@@ -17,7 +17,10 @@ progress-bar flags; their per-Gaussian terms are ``gaussian_regularizers``: two 
 ``B200VanillaWithNormalRegMetrics`` has ``VanillaWithNormalRegMetrics``' fields, defaults, ``setup`` mutation, output keys and
 progress-bar flags; its depth-normal term is ``normal_consistency_loss``: two kernel launches forward, one backward.
 ``depth_to_normal`` is gsplat's ``utils.depth_to_normal`` for the reference's call, which ``compat.install()`` registers.
+``B200VanillaMetricsWithSimilarityRegularization`` has ``VanillaMetricsWithSimilarityRegularization``' fields, defaults, backward
+hook and logged key; its k-NN query is ``ops.knn_points`` and its term ``ops.similarity_regularization``.
 """
+import time
 from dataclasses import dataclass, field
 from typing import Literal, Optional
 
@@ -714,4 +717,105 @@ class B200VanillaWithNormalRegMetrics(B200NormalRegMixin, B200VanillaMetrics):
 
 
 class B200VanillaWithNormalRegMetricsModule(B200NormalRegModuleMixin, B200VanillaMetricsModule):
+    pass
+
+
+# ---- VanillaMetricsWithSimilarityRegularization (internal/metrics/appearance_feature_similarity_regularization_metrics.py) ------------
+class Similarity:
+    """The similarity of ``SimilarityRegularizationConfigMixin.similarity_type``; the term runs on ``ops.similarity_regularization``."""
+
+
+@dataclass
+class Cosine(Similarity):
+    pass
+
+
+@dataclass
+class Euclidean(Similarity):
+    pass
+
+
+def _similarity_kind(similarity_type) -> str:
+    """"cosine" or "euclidean" from the reference's Cosine() / Euclidean() objects, these classes, or {"class_path": "Cosine"}"""
+    if isinstance(similarity_type, dict):
+        name = str(similarity_type.get("class_path", "")).rsplit(".", 1)[-1]
+    else:
+        name = type(similarity_type).__name__
+    if name not in ("Cosine", "Euclidean"):
+        raise NotImplementedError(f"similarity_type {similarity_type!r}: only Cosine and Euclidean are provided")
+    return name.lower()
+
+
+@dataclass
+class B200SimilarityRegularizationConfigMixin:
+    n_appearance_samples: int = 20_480
+
+    n_appearance_nn: int = 16
+
+    distance_weight_decay: float = 200.
+    """
+    Used to decrease the weights with increasing distance.
+    The value should be higher for smaller scenes.
+    """
+
+    similarity_reg_from: int = 0
+
+    similarity_reg_lambda: float = 0.2
+
+    similarity_reg_interval: int = 50
+
+    similarity_type: Similarity = field(default_factory=lambda: {"class_path": "Cosine"})
+
+
+class B200SimilarityRegularizationMixin:
+    """Every ``similarity_reg_interval`` steps from ``similarity_reg_from`` on, after the main backward: ``n_appearance_samples``
+    Gaussians drawn by ``torch.randperm``, their ``n_appearance_nn`` nearest Gaussians by ``ops.knn_points`` and the weighted
+    similarity term by ``ops.similarity_regularization``, back-propagated into the appearance features with ``manual_backward``
+    and logged as ``train/as_r``.  No host synchronisation on the way."""
+
+    def get_similarity_metric(self, gaussian_model):
+        """(loss, meta, knn_time) as the reference returns them.  meta has the reference's nine slots in its order: sample_indices,
+        the KNN result ([1,S,K] dists and idx), None, distance_based_weight [S,K], None, None, triu_mask [K,K], None and the unscaled
+        mean; the [S,K,K] intermediates are never formed.  knn_time is the host time of the k-NN call (the reference's time.time()
+        difference, which does not wait for the device either)."""
+        from .compat import KNN
+        kind = _similarity_kind(self.config.similarity_type)
+        started_at = time.time()
+        with torch.no_grad():
+            means = gaussian_model.get_means()
+            sample_indices = torch.randperm(means.shape[0], device=means.device)[:self.config.n_appearance_samples]
+            dists, idx = ops.knn_points(means[sample_indices], means, self.config.n_appearance_nn)
+            knn_consumed_time = time.time() - started_at
+        loss, mean, weights = ops.similarity_regularization(gaussian_model.get_appearance_features(), idx, dists,
+                                                            decay=self.config.distance_weight_decay,
+                                                            weight=self.config.similarity_reg_lambda, kind=kind)
+        k = idx.shape[1]
+        triu_mask = torch.triu(torch.ones((k, k), dtype=torch.bool, device=means.device), diagonal=1)
+        return loss, (sample_indices, KNN(dists[None], idx[None], None), None, weights, None, None, triu_mask, None, mean), \
+            knn_consumed_time
+
+    def similarity_metric_backward_hook(self, outputs, batch, gaussian_model, step, pl_module):
+        if step < self.config.similarity_reg_from:
+            return
+        if step % self.config.similarity_reg_interval != 0:
+            return
+
+        similarities_reg, meta, _ = self.get_similarity_metric(gaussian_model)
+        pl_module.manual_backward(similarities_reg)
+        pl_module.log("train/as_r", meta[-1], prog_bar=True, on_step=False, on_epoch=True, batch_size=pl_module.batch_size)
+
+    def training_setup(self, pl_module):
+        pl_module.on_after_backward_hooks.append(self.similarity_metric_backward_hook)
+        return super().training_setup(pl_module)
+
+
+@dataclass
+class B200VanillaMetricsWithSimilarityRegularization(B200SimilarityRegularizationConfigMixin, B200VanillaMetrics):
+    def instantiate(self, *args, **kwargs) -> "B200VanillaMetricsWithSimilarityRegularizationModule":
+        self._check()
+        _similarity_kind(self.similarity_type)
+        return B200VanillaMetricsWithSimilarityRegularizationModule(self)
+
+
+class B200VanillaMetricsWithSimilarityRegularizationModule(B200SimilarityRegularizationMixin, B200VanillaMetricsModule):
     pass

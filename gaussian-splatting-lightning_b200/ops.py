@@ -888,6 +888,110 @@ def knn_mean_dist2(points: torch.Tensor) -> torch.Tensor:
     return out
 
 
+KNN_MAX_K = 32
+
+
+def knn_launches(n: int) -> int:
+    """library launches of one knn_points or knn_mean_dist2 call over n points: bounds, grid, cell keys, histogram, the radix passes
+    over the cell keys (< 4n + 64 cells), gather, search"""
+    bits = max(1, (4 * max(n, 1) + 63).bit_length())
+    return 6 + (bits + 7) // 8
+
+
+def knn_points(queries: torch.Tensor, points: torch.Tensor, K: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The K nearest of ``points`` [N,3] for every query of ``queries`` [S,3] (float32 CUDA, one device), a query that is itself one
+    of the points included: (dists [S,K] squared distances, idx [S,K] int64), ascending.  pytorch3d's ``knn_points`` for one batch
+    entry with norm 2.  Exact up to ties.  No host synchronisation; not differentiable (both reference callers run it under
+    ``no_grad``).  1 <= K <= min(32, N)."""
+    q, pts = _f32c(queries, "queries"), _f32c(points, "points")
+    if q.dim() != 2 or q.shape[1] != 3 or pts.dim() != 2 or pts.shape[1] != 3:
+        raise ValueError(f"queries and points must be [S, 3] and [N, 3], got {tuple(q.shape)} and {tuple(pts.shape)}")
+    if q.device != pts.device:
+        raise ValueError("queries and points must be on one device")
+    K = int(K)
+    if not 1 <= K <= KNN_MAX_K or K > pts.shape[0]:
+        raise ValueError(f"K must be 1..{KNN_MAX_K} and at most the number of points ({pts.shape[0]}), got {K}")
+    L = lib()
+    s, n = q.shape[0], pts.shape[0]
+    dists = torch.empty((s, K), dtype=torch.float32, device=q.device)
+    idx = torch.empty((s, K), dtype=torch.int64, device=q.device)
+    ws = torch.empty(max(int(L.b200gs_knn_workspace_bytes(n)), 256), dtype=torch.uint8, device=q.device)
+    check(L.b200gs_knn_points(s, ptr(q), n, ptr(pts), K, ptr(dists), ptr(idx), ptr(ws), ws.numel(), _stream()), "b200gs_knn_points")
+    return dists, idx
+
+
+SIMILARITY_KINDS = {"cosine": 0, "euclidean": 1}
+SIMILARITY_FWD_LAUNCHES = 2     # library launches of one similarity_regularization forward: per-sample sums, reduce
+
+
+def similarity_bwd_launches(n: int) -> int:
+    """library launches of one similarity_regularization backward over n Gaussians: entries, histogram, radix passes, run table,
+    sums"""
+    bits = max(1, (n - 1).bit_length())
+    return 4 + (bits + 7) // 8
+
+
+class _SimilarityRegularization(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, features, idx, dists, decay, weight, kind):
+        n, d = features.shape
+        s, k = idx.shape
+        L = lib()
+        nbytes = int(L.b200gs_similarity_reg_workspace_bytes(n, s, k, d, 0))          # the per-sample sums only
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=features.device)
+        out = torch.empty(2, dtype=torch.float32, device=features.device)
+        weights = torch.empty((s, k), dtype=torch.float32, device=features.device)
+        check(L.b200gs_similarity_reg_fwd(n, d, ptr(features), s, k, ptr(idx), ptr(dists), kind, decay, weight, ptr(ws), nbytes, ptr(out),
+                                          ptr(weights), _stream()), "b200gs_similarity_reg_fwd")
+        ctx.save_for_backward(features, idx, dists)
+        ctx.args = (decay, weight, kind)
+        mean = out[1]
+        ctx.mark_non_differentiable(mean, weights)
+        return out[0], mean, weights
+
+    @staticmethod
+    def backward(ctx, v_loss, _v_mean, _v_weights):
+        features, idx, dists = ctx.saved_tensors
+        decay, weight, kind = ctx.args
+        n, d = features.shape
+        s, k = idx.shape
+        L = lib()
+        nbytes = int(L.b200gs_similarity_reg_workspace_bytes(n, s, k, d, 1))
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=features.device)
+        v = v_loss.reshape(1).to(torch.float32).contiguous()
+        v_features = torch.empty_like(features)
+        check(L.b200gs_similarity_reg_bwd(n, d, ptr(features), s, k, ptr(idx), ptr(dists), kind, decay, weight, ptr(ws), nbytes,
+                                              ptr(v), ptr(v_features), _stream()), "b200gs_similarity_reg_bwd")
+        return v_features, None, None, None, None, None
+
+
+def similarity_regularization(features: torch.Tensor, idx: torch.Tensor, dists: torch.Tensor, *, decay: float, weight: float,
+                              kind: str = "cosine"):
+    """``SimilarityRegularizationMixin.get_similarity_metric``'s term after ``knn_points`` (K43/K44, backward K45, the onesweep sort
+    and K46), without its [S,K,K,D] broadcast:
+        m = mean_{s, i<j} r_sij exp(-decay dists[s,j]),   loss = weight m,
+        "cosine": r = -n_i . n_j with n = F.normalize(f),   "euclidean": r = |f_i - f_j|,   f_i = features[idx[s,i]].
+    The forward allocates only the S per-sample sums; the backward its own S K (4 D + 16) + 8 N bytes.
+    features float32 CUDA [N,D] (D <= 256), idx int64 [S,K] (2 <= K <= 32, values in [0, N)), dists float32 [S,K].  Returns
+    (loss, m, w): device scalars and the weights [S,K]; the gradient goes to ``features`` only, densely and deterministically.  No
+    host synchronisation."""
+    if kind not in SIMILARITY_KINDS:
+        raise NotImplementedError(f"similarity kind {kind!r}: only {sorted(SIMILARITY_KINDS)} are provided")
+    if features.dim() != 2 or idx.dim() != 2 or tuple(dists.shape) != tuple(idx.shape):
+        raise ValueError(f"features must be [N, D] and idx, dists [S, K], got {tuple(features.shape)}, {tuple(idx.shape)}, "
+                         f"{tuple(dists.shape)}")
+    n, d = features.shape
+    s, k = idx.shape
+    if not 1 <= d <= 256 or not 2 <= k <= KNN_MAX_K or s < 1 or n < 1:
+        raise ValueError(f"need 1 <= D <= 256, 2 <= K <= {KNN_MAX_K}, S >= 1 and N >= 1, got D={d}, K={k}, S={s}, N={n}")
+    if features.dtype != torch.float32 or dists.dtype != torch.float32 or idx.dtype != torch.int64:
+        raise ValueError("features and dists must be float32 and idx int64")
+    if not (features.is_cuda and idx.device == features.device and dists.device == features.device):
+        raise ValueError("features, idx and dists must be CUDA tensors on one device")
+    return _SimilarityRegularization.apply(features.contiguous(), idx.detach().contiguous(), dists.detach().contiguous(), float(decay),
+                                           float(weight), SIMILARITY_KINDS[kind])
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 # fused L1 + SSIM loss (csrc/loss.cu; the metric the reference computes right after the renderer, vanilla_metrics.py:57-80)
 # ----------------------------------------------------------------------------------------------------------------------

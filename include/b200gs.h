@@ -391,11 +391,47 @@ B200GS_API int b200gs_normal_reg_bwd(int32_t height, int32_t width, const float*
 B200GS_API int b200gs_depth_to_normal(int32_t height, int32_t width, const float* depth, const float* c2w, int64_t c2w_s0, int64_t c2w_s1,
                                       const float* K, int64_t K_s0, int64_t K_s1, float* normals, void* stream);
 
-/* b200gs_knn_mean_dist2: simple_knn's distCUDA2 (vanilla_gaussian.py:122-125, the scale initialiser): mean_dist2[i] = mean of the squared
- *     distances from points[i] (float[n,3]) to its 3 nearest neighbours (exact).  Synchronises the stream once (the hash grid is sized
- *     on the host from the bounding box); init-time only. */
+/* ---- k nearest neighbours on a hash grid over the reference points (no host synchronisation: the grid is sized on the device) ----
+ * b200gs_knn_mean_dist2: simple_knn's distCUDA2 (vanilla_gaussian.py:122-125, the scale initialiser): mean_dist2[i] = mean of the squared
+ *     distances from points[i] (float[n,3]) to its 3 nearest neighbours (exact).
+ * b200gs_knn_points: pytorch3d.ops.knn_points for one batch entry with norm 2 and sorted output (appearance_feature_similarity_
+ *     regularization_metrics.py:70-74, segany_splatting.py:276-280): for every query (float[s,3]; inside or outside the reference set's
+ *     bounding box) the k nearest of the n reference points (float[n,3]), a query that is itself a reference point included, in
+ *     ascending order: dists float[s,k] squared fp32 distances, idx int64[s,k].  Exact up to ties: points at the same distance keep the
+ *     grid's order.  Points with a non-finite coordinate are left out of the grid's bounding box; a query with fewer than k points at
+ *     a finite distance (a NaN or infinite query, non-finite points) fills its remaining slots with the lowest unused indices and
+ *     their distances as computed, so every index is in [0, n).  The grid sizing runs a bounded number of steps on any box.  B200GS_EINVAL for k outside 1..32 or k > n, B200GS_ENOSPACE for n >= 2^30 or a short workspace.
+ * b200gs_knn_workspace_bytes: the workspace of both for n reference points.
+ * Launches: 6 + ceil(log2(4n + 64) / 8) (bounds, grid, cell keys, histogram, the radix passes, gather, search).  No float atomics. */
 B200GS_API size_t b200gs_knn_workspace_bytes(int64_t n);
 B200GS_API int b200gs_knn_mean_dist2(int64_t n, const float* points, float* mean_dist2, void* workspace, size_t workspace_bytes, void* stream);
+B200GS_API int b200gs_knn_points(int64_t s, const float* queries, int64_t n, const float* points, int32_t k, float* dists, int64_t* idx,
+                                 void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- Appearance-feature similarity regulariser (appearance_feature_similarity_regularization_metrics.py:63-102,
+ *      SimilarityRegularizationMixin.get_similarity_metric after knn_points, and its autograd backward) ------------------------------
+ * out float[2] <- [lambda m, m],  m = mean_{s, i<j} r_sij w_sj  over the S K (K - 1) / 2 pairs,  w_sj = exp(-decay dists[s,j]);
+ *     kind 0 (Cosine): r_sij = -n_i . n_j with n = f / max(|f|, 1e-12) (F.normalize); kind 1 (Euclidean): r_sij = |f_i - f_j|;
+ *     f_i = features[idx[s,i]] (features float[n,d] contiguous, idx int64[s,k] with values in [0, n), dists float[s,k]); an index
+ *     outside [0, n) is clamped into it, so it reads a real row (memory-safe, not meaningful).
+ *     weights float[s,k] <- w when not NULL.
+ * b200gs_similarity_reg_bwd: v_features float[n,d] (every row written, 0 where no sample reached) <- d (v_loss[0] out[0]) / d features,
+ *     v_loss read on the device; dists get no gradient.  Zero-norm rows take F.normalize's 1/eps branch, zero distances torch's zero
+ *     norm gradient.  Per-entry rows are sorted by idx (onesweep) and summed per Gaussian in entry order: no float atomics, repeats
+ *     are bit-identical.
+ * Sizes: 1 <= d <= 256, 2 <= k <= 32, s >= 1, n >= 1, n < 2^30, s k < 2^30; kind 0 or 1; B200GS_EINVAL otherwise, before any CUDA call.
+ * b200gs_similarity_reg_workspace_bytes: scratch of the forward (backward 0: the s per-sample sums) or of the backward (backward 1:
+ *     s k (4 d + 16) bytes of entry rows and records, n 8 bytes of run table and the sort's counters); 0 for sizes not accepted.
+ *     The two calls need not share a workspace: the backward reads nothing the forward wrote.
+ * Launches: forward 2 (per-sample sums, reduce); backward 4 + ceil(log2(n) / 8) (entries, histogram, radix passes, run table,
+ *     per-Gaussian sums). */
+B200GS_API size_t b200gs_similarity_reg_workspace_bytes(int64_t n, int64_t s, int32_t k, int32_t d, int32_t backward);
+B200GS_API int b200gs_similarity_reg_fwd(int64_t n, int32_t d, const float* features, int64_t s, int32_t k, const int64_t* idx,
+                                         const float* dists, int32_t kind, float decay, float lambda, void* workspace,
+                                         size_t workspace_bytes, float* out, float* weights, void* stream);
+B200GS_API int b200gs_similarity_reg_bwd(int64_t n, int32_t d, const float* features, int64_t s, int32_t k, const int64_t* idx,
+                                         const float* dists, int32_t kind, float decay, float lambda, void* workspace,
+                                         size_t workspace_bytes, const float* v_loss, float* v_features, void* stream);
 
 /* ---- standalone SH (gsplat.sh.spherical_harmonics; gsplat_renderer.py:105) -------------------------------------------
  * dirs[n,3] need not be unit (normalised inside, as gsplat does).  out rgb[n,3] = SH (no +0.5, no clamp).
