@@ -96,6 +96,8 @@ _SIGNATURES = {
     "b200gs_similarity_reg_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int32, c_int32, c_int32]),
     "b200gs_similarity_reg_fwd": (c_int32, [c_int64, c_int32, _P, c_int64, c_int32, _P, _P, c_int32, c_float, c_float, _P, c_size_t, _P, _P, _P]),
     "b200gs_similarity_reg_bwd": (c_int32, [c_int64, c_int32, _P, c_int64, c_int32, _P, _P, c_int32, c_float, c_float, _P, c_size_t, _P, _P, _P]),
+    "b200gs_glossy_sh_fwd": (c_int32, [c_int32, c_int64, _P, _P, _P, _P, c_int32, _P, _P, c_int32, c_int32, _P, _P, _P, _P, _P]),
+    "b200gs_glossy_sh_bwd": (c_int32, [c_int32, c_int64, _P, _P, c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, _P, _P, _P]),
     "b200gs_sh_fwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P]),
     "b200gs_sh_bwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P, _P, _P]),
     "b200gs_sh_split_fwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P, _P, _P]),

@@ -42,7 +42,7 @@ using namespace b200gs;
 extern "C" {
 
 const char* b200gs_last_error(void) { return g_error; }
-int b200gs_version(void) { return 233; }
+int b200gs_version(void) { return 234; }
 int64_t b200gs_launch_count(void) { return (int64_t)g_launches.load(std::memory_order_relaxed); }
 
 int b200gs_project_fwd(const B200gsView* view, int64_t n, const float* means, const float* scales, const float* quats,
@@ -793,6 +793,39 @@ int b200gs_sh_split_bwd(int32_t degree, int32_t k_rest, int64_t n, const float* 
     B200GS_CHECK_ARG(n >= 0, "n < 0");
     B200GS_CHECK_ARG(n == 0 || (dirs && dc && v_rgb && v_dc && (k_rest == 0 || (rest && v_rest))), "NULL pointer");
     return launch_sh_bwd(degree, k_rest + 1, n, dirs, dc, v_rgb, v_dc, v_dirs, (cudaStream_t)stream, true, rest, mask, v_rest);
+}
+
+// shared by the Glossy-Gaussian entry points: the degree, the opacity rest width and, when the colour is on, its layout
+static int check_glossy(const char* fn, int32_t degree, int64_t n, const float* means, const float* campos, int32_t op_k_rest,
+                        bool colour, int32_t sh_stride, int32_t sh_split) {
+    auto fail = [&](const char* msg) { set_error("%s: %s", fn, msg); return B200GS_EINVAL; };
+    if (degree < 0 || degree > 4) return fail("degree must be 0..4");
+    if (n < 0) return fail("n < 0");
+    if (op_k_rest < 0 || op_k_rest + 1 < (degree + 1) * (degree + 1)) return fail("1 + op_k_rest < (degree+1)^2");
+    if (n > 0 && !(means && campos)) return fail("NULL pointer");
+    if (colour && sh_split != 0 && sh_split != 1) return fail("sh_split must be 0 or 1");
+    if (colour && sh_stride < (degree + 1) * (degree + 1)) return fail("sh_stride < (degree+1)^2");
+    return 0;
+}
+
+int b200gs_glossy_sh_fwd(int32_t degree, int64_t n, const float* means, const float* campos, const float* op_dc, const float* op_rest,
+                         int32_t op_k_rest, const float* shs, const float* shs_rest, int32_t sh_stride, int32_t sh_split,
+                         const uint8_t* mask, float* opacity, float* rgb, uint8_t* clamped, void* stream) {
+    if (int rc = check_glossy(__func__, degree, n, means, campos, op_k_rest, rgb != nullptr, sh_stride, sh_split)) return rc;
+    B200GS_CHECK_ARG(n == 0 || (op_dc && opacity && clamped && (op_k_rest == 0 || op_rest)), "NULL pointer");
+    B200GS_CHECK_ARG(n == 0 || !rgb || (shs && (!sh_split || sh_stride == 1 || shs_rest)), "NULL pointer");
+    return launch_glossy_sh_fwd(degree, n, means, campos, op_dc, op_rest, op_k_rest, shs, shs_rest, sh_stride, sh_split != 0, mask, opacity,
+                                rgb, clamped, (cudaStream_t)stream);
+}
+
+int b200gs_glossy_sh_bwd(int32_t degree, int64_t n, const float* means, const float* campos, int32_t op_k_rest, int32_t sh_stride,
+                         int32_t sh_split, const uint8_t* clamped, const float* v_opacity, const float* v_rgb, float* v_op_dc,
+                         float* v_op_rest, float* v_shs, float* v_shs_rest, void* stream) {
+    if (int rc = check_glossy(__func__, degree, n, means, campos, op_k_rest, v_rgb != nullptr, sh_stride, sh_split)) return rc;
+    B200GS_CHECK_ARG(n == 0 || (clamped && v_opacity && v_op_dc && (op_k_rest == 0 || v_op_rest)), "NULL pointer");
+    B200GS_CHECK_ARG(n == 0 || !v_rgb || (v_shs && (!sh_split || sh_stride == 1 || v_shs_rest)), "NULL pointer");
+    return launch_glossy_sh_bwd(degree, n, means, campos, op_k_rest, sh_stride, sh_split != 0, clamped, v_opacity, v_rgb, v_op_dc, v_op_rest,
+                                v_shs, v_shs_rest, (cudaStream_t)stream);
 }
 
 int b200gs_isect_keys(int32_t n_tiles, const int32_t* tile_ranges, const int32_t* sorted_ids, int64_t n_pairs, const float* depth,

@@ -255,6 +255,12 @@ int launch_record_sort(int64_t n, int bits, uint2* a, uint2* b, void* scratch, c
 
 // similarity regulariser (similarity_reg.cu): features [N,D] contiguous, idx [S,K] int64, dists [S,K]; kind 0 Cosine, 1 Euclidean
 size_t similarity_reg_workspace_bytes(int64_t n, int64_t s, int k, int d, bool backward);
+int launch_glossy_sh_fwd(int degree, int64_t n, const float* means, const float* campos, const float* op_dc, const float* op_rest,
+                         int op_k_rest, const float* shs, const float* shs_rest, int sh_stride, bool split, const uint8_t* mask,
+                         float* opacity, float* rgb, uint8_t* clamped, cudaStream_t s);
+int launch_glossy_sh_bwd(int degree, int64_t n, const float* means, const float* campos, int op_k_rest, int sh_stride, bool split,
+                         const uint8_t* clamped, const float* v_opacity, const float* v_rgb, float* v_op_dc, float* v_op_rest,
+                         float* v_shs, float* v_shs_rest, cudaStream_t s);
 int launch_similarity_reg_fwd(int64_t n, int d, const float* features, int64_t s, int k, const int64_t* idx, const float* dists, int kind,
                               float decay, float lambda, float* ws, float* out, float* weights, cudaStream_t st);
 int launch_similarity_reg_bwd(int64_t n, int d, const float* features, int64_t s, int k, const int64_t* idx, const float* dists, int kind,

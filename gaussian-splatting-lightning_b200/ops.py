@@ -11,6 +11,7 @@ Functions
   rasterize_gaussians(...)    gsplat v0 ``rasterize_gaussians``        (gsplat_renderer.py:86-99)
   spherical_harmonics_decomposed(...)  gsplat ``sh_decomposed``   (gsplat_v1_renderer.py:124)
   isect_keys / isect_offsets  gsplat v1 ``isect_tiles`` keys / ``isect_offset_encode``   (gsplat_v1_renderer.py:446,458)
+  glossy_sh(...)              Glossy-Gaussian view-dependent opacity + SH colour   (glossy_renderer.py get_opacities / get_rgbs)
 """
 import ctypes
 import os
@@ -701,6 +702,107 @@ def spherical_harmonics_decomposed(degrees_to_use: int, dirs: torch.Tensor, dc: 
             raise ValueError("masks must be [N] on the device of the coefficients")
         mask = (masks if masks.dtype == torch.bool else masks != 0).contiguous().view(torch.uint8)
     return _SphericalHarmonicsSplit.apply(degrees_to_use, dirs, dc, coeffs, mask)
+
+
+# ---- Glossy-Gaussian view-dependent opacity and colour (csrc/glossy.cu) -------------------------------------------------------
+GLOSSY_FWD_LAUNCHES = 1     # K47
+GLOSSY_BWD_LAUNCHES = 1     # K48
+
+
+def _f32_in_place(t: torch.Tensor, name: str) -> torch.Tensor:
+    """A float32 CUDA tensor the kernels read in place: refused, never copied, when it is not contiguous."""
+    _f32c(t, name)
+    if not t.is_contiguous():
+        raise ValueError(f"{name} must be contiguous (read in place)")
+    return t
+
+
+class _GlossySH(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, degree, split, mask, means, campos, op_dc, op_rest, shs, shs_rest):
+        n, dev = means.shape[0], means.device
+        colour = shs is not None
+        stride = (shs.shape[1] + (shs_rest.shape[1] if split else 0)) if colour else 0
+        opacity = torch.empty(n, dtype=torch.float32, device=dev)
+        rgb = torch.empty(n, 3, dtype=torch.float32, device=dev) if colour else None
+        clamped = torch.empty(n, dtype=torch.uint8, device=dev)
+        check(lib().b200gs_glossy_sh_fwd(degree, n, ptr(means), ptr(campos), ptr(op_dc), ptr(op_rest), op_rest.shape[1], ptr(shs),
+                                         ptr(shs_rest), stride, int(split), ptr(mask), ptr(opacity), ptr(rgb), ptr(clamped), _stream()),
+              "b200gs_glossy_sh_fwd")
+        ctx.degree, ctx.split, ctx.stride, ctx.colour = degree, split, stride, colour
+        ctx.shapes = (op_dc.shape, op_rest.shape, shs.shape if colour else None, shs_rest.shape if colour and split else None)
+        ctx.save_for_backward(means, campos, clamped)
+        return rgb, opacity
+
+    @staticmethod
+    def backward(ctx, v_rgb, v_opacity):
+        means, campos, clamped = ctx.saved_tensors
+        n, dev = means.shape[0], means.device
+        dc_shape, rest_shape, shs_shape, shs_rest_shape = ctx.shapes
+        v_opacity = _f32c(v_opacity, "grad") if v_opacity is not None else torch.zeros(n, dtype=torch.float32, device=dev)
+        colour = ctx.colour and v_rgb is not None
+        v_rgb = _f32c(v_rgb, "grad") if colour else None
+        v_op_dc = torch.empty(dc_shape, dtype=torch.float32, device=dev)
+        v_op_rest = torch.empty(rest_shape, dtype=torch.float32, device=dev)
+        v_shs = torch.empty(shs_shape, dtype=torch.float32, device=dev) if colour else None
+        v_shs_rest = torch.empty(shs_rest_shape, dtype=torch.float32, device=dev) if colour and ctx.split else None
+        check(lib().b200gs_glossy_sh_bwd(ctx.degree, n, ptr(means), ptr(campos), rest_shape[1], ctx.stride, int(ctx.split), ptr(clamped),
+                                         ptr(v_opacity), ptr(v_rgb), ptr(v_op_dc), ptr(v_op_rest), ptr(v_shs), ptr(v_shs_rest), _stream()),
+              "b200gs_glossy_sh_bwd")
+        return None, None, None, None, None, v_op_dc, v_op_rest, v_shs, v_shs_rest
+
+
+def glossy_sh(degree: int, means: torch.Tensor, campos: torch.Tensor, op_dc: torch.Tensor, op_rest: torch.Tensor, *,
+              shs_dc: Optional[torch.Tensor] = None, shs_rest: Optional[torch.Tensor] = None, features: Optional[torch.Tensor] = None,
+              mask: Optional[torch.Tensor] = None) -> Tuple[Optional[torch.Tensor], torch.Tensor]:
+    """Glossy-Gaussian view-dependent opacity and SH colour on one kernel each way: returns ``(rgb, opacity)``.
+
+    The view direction of Gaussian i is ``F.normalize(means[i] - campos)``, detached (no gradient reaches ``means``); ``campos`` is
+    the camera centre, 3 floats on the device.  ``opacity`` [N] = ``clamp(SH_degree(op_dc | op_rest) + 0.5, 0, 1)`` for every row,
+    from the model's ``[N,1,1]`` dc and ``[N,R,1]`` rest, R >= (degree+1)^2 - 1.  ``rgb`` [N,3] = ``clamp(SH_degree(colour) + 0.5,
+    min=0)`` on the rows where ``mask`` ([N] bool, None: all) is set and 0.5 on the others; the colour is ``shs_dc`` [N,1,3] with
+    ``shs_rest`` [N,K-1,3], or ``features`` [N,K,3], K >= (degree+1)^2; without either, no colour is computed and rgb is None.
+    Every tensor is read in place: non-float32, non-CUDA or non-contiguous inputs are refused with a ValueError."""
+    degree = int(degree)
+    if not 0 <= degree <= 4:
+        raise ValueError(f"degree must be 0..4, got {degree}")
+    n, need = means.shape[0], (degree + 1) ** 2
+    if means.shape != (n, 3):
+        raise ValueError("means must be [N, 3]")
+    if op_dc.shape != (n, 1, 1) or op_rest.dim() != 3 or op_rest.shape[0] != n or op_rest.shape[2] != 1:
+        raise ValueError("expected op_dc [N,1,1] and op_rest [N,R,1]")
+    if op_rest.shape[1] + 1 < need:
+        raise ValueError(f"op_rest has {op_rest.shape[1]} rows, degree {degree} needs {need - 1}")
+    if features is not None and (shs_dc is not None or shs_rest is not None):
+        raise ValueError("pass either features or shs_dc and shs_rest, not both")
+    if (shs_dc is None) != (shs_rest is None):
+        raise ValueError("shs_dc and shs_rest go together")
+    split = shs_dc is not None
+    shs = shs_dc if split else features
+    if split:
+        if shs_dc.shape != (n, 1, 3) or shs_rest.dim() != 3 or shs_rest.shape[0] != n or shs_rest.shape[2] != 3:
+            raise ValueError("expected shs_dc [N,1,3] and shs_rest [N,K-1,3]")
+        if shs_rest.shape[1] + 1 < need:
+            raise ValueError(f"shs_rest has {shs_rest.shape[1]} rows, degree {degree} needs {need - 1}")
+    elif features is not None:
+        if features.dim() != 3 or features.shape[0] != n or features.shape[2] != 3:
+            raise ValueError("expected features [N,K,3]")
+        if features.shape[1] < need:
+            raise ValueError(f"features has {features.shape[1]} coefficients, degree {degree} needs {need}")
+    means = _f32_in_place(means.detach(), "means")
+    op_dc, op_rest = _f32_in_place(op_dc, "op_dc"), _f32_in_place(op_rest, "op_rest")
+    if shs is not None:
+        shs = _f32_in_place(shs, "shs_dc" if split else "features")
+        shs_rest = _f32_in_place(shs_rest, "shs_rest") if split else None
+    campos = _f32c(campos, "campos").reshape(-1)
+    if campos.numel() != 3 or campos.device != means.device:
+        raise ValueError("campos must be 3 floats on the device of means")
+    m = None
+    if mask is not None and shs is not None:
+        if mask.shape != (n,) or mask.device != means.device:
+            raise ValueError("mask must be [N] on the device of means")
+        m = (mask if mask.dtype == torch.bool else mask != 0).contiguous().view(torch.uint8)
+    return _GlossySH.apply(degree, split, m, means, campos, op_dc, op_rest, shs, shs_rest)
 
 
 class _RasterizeGaussians(torch.autograd.Function):

@@ -453,6 +453,29 @@ B200GS_API int b200gs_sh_split_fwd(int32_t degree, int32_t k_rest, int64_t n, co
 B200GS_API int b200gs_sh_split_bwd(int32_t degree, int32_t k_rest, int64_t n, const float* dirs, const float* dc, const float* rest,
                                    const uint8_t* mask, const float* v_rgb, float* v_dc, float* v_rest, float* v_dirs, void* stream);
 
+/* ---- K47 / K48: Glossy-Gaussian view-dependent opacity and SH colour (glossy_renderer.py get_opacities / get_rgbs with
+ *      GlossyGaussianModel.get_view_dep_opacities, glossy_gaussian.py:66-79) --------------------------------------------------
+ * dir_i = (means[i] - campos) / max(|means[i] - campos|, 1e-12) (F.normalize; a Gaussian at the camera centre gets the zero
+ *     direction); means float[n,3], campos float[3] on the device (never read on the host).
+ * opacity[i] = clamp(SH_degree(op_dc[i] | op_rest[i]; dir_i) + 0.5, 0, 1) for EVERY row: op_dc float[n] (the [n,1,1] property),
+ *     op_rest float[n,op_k_rest] (the [n,R,1] property), op_k_rest + 1 >= (degree+1)^2; rows at or beyond the degree are not read.
+ * rgb[i,3] (nullable: no colour) = clamp(SH_degree(colour; dir_i) + 0.5, min=0) where mask[i] != 0 (mask uint8[n], nullable = all),
+ *     0.5 elsewhere, reading no colour coefficient.  Colour: sh_split = 1: shs = dc [n,1,3], shs_rest = rest [n,sh_stride-1,3];
+ *     sh_split = 0: shs = [n,sh_stride,3]; sh_stride >= (degree+1)^2.
+ * clamped uint8[n] <- the clamp decisions the backward needs (bit c: colour channel c clamped or the row masked; bit 3: opacity
+ *     clamped).  Bounds are inclusive as in torch.clamp: a value exactly on a bound passes its gradient.
+ * bwd: v_op_dc float[n], v_op_rest float[n,op_k_rest] and, when v_rgb (float[n,3]) is not NULL, v_shs / v_shs_rest in the forward's
+ *     colour layout, every row written in full: zeros at or beyond the degree, on masked rows and for clamped outputs.  No means or
+ *     direction gradient (the reference detaches the direction), no coefficient read, no atomics: repeats are bit-identical.
+ * degree 0..4, n >= 0; B200GS_EINVAL before any CUDA call otherwise.  Launches: one each way, no host synchronisation.
+ * Algorithmic bytes per Gaussian at degree 3 (16-coefficient storage): fwd 269 in, 17 out; bwd 29 in, 256 out. */
+B200GS_API int b200gs_glossy_sh_fwd(int32_t degree, int64_t n, const float* means, const float* campos, const float* op_dc,
+                                    const float* op_rest, int32_t op_k_rest, const float* shs, const float* shs_rest, int32_t sh_stride,
+                                    int32_t sh_split, const uint8_t* mask, float* opacity, float* rgb, uint8_t* clamped, void* stream);
+B200GS_API int b200gs_glossy_sh_bwd(int32_t degree, int64_t n, const float* means, const float* campos, int32_t op_k_rest,
+                                    int32_t sh_stride, int32_t sh_split, const uint8_t* clamped, const float* v_opacity,
+                                    const float* v_rgb, float* v_op_dc, float* v_op_rest, float* v_shs, float* v_shs_rest, void* stream);
+
 /* ---- K2-K5: tile binning ------------------------------------------------------------------------------------------
  * replaces dgr InclusiveSum + duplicateWithKeys + SortPairs + identifyTileRanges / gsplat isect_tiles + isect_offset_encode.
  * Result order is exactly that of a stable sort of (tile_id << 32 | float_bits(depth)) keys emitted Gaussian-major:
