@@ -112,8 +112,7 @@ _SIGNATURES = {
     "b200gs_loss_fwd": (c_int32, [c_int32, c_int32, c_int32, _P, _P, _P, _P, _P]),
     "b200gs_loss_bwd": (c_int32, [c_int32, c_int32, c_int32, _P, _P, _P, ctypes.c_float, _P, _P, _P]),
     "b200gs_publish_i64": (c_int32, [_P, _P, c_int32, _P]),
-    "b200gs_blend_fwd": (c_int32, [c_int32] * 4 + [_P] * 7 + [_P, c_int64, c_int64, _P, _P, _P, _P]),
-    "b200gs_blend_fwd_hits": (c_int32, [c_int32] * 4 + [_P] * 7 + [_P, c_int64, c_int64, _P, _P, _P, _P, _P]),
+    "b200gs_blend_fwd": (c_int32, [c_int32] * 4 + [_P] * 7 + [_P, c_int64, c_int64, _P, _P, _P, _P, _P]),
     "b200gs_blend_bwd": (c_int32, [c_int32] * 4 + [_P] * 7 + [_P, _P, _P, c_int64, c_int64, _P, c_float, c_float]
                          + [_P] * 5 + [_P]),
     "b200gs_blend_feat_fwd": (c_int32, [c_int32] * 3 + [_P] * 7 + [_P] * 4 + [_P]),

@@ -42,7 +42,7 @@ using namespace b200gs;
 extern "C" {
 
 const char* b200gs_last_error(void) { return g_error; }
-int b200gs_version(void) { return 234; }
+int b200gs_version(void) { return 235; }
 int64_t b200gs_launch_count(void) { return (int64_t)g_launches.load(std::memory_order_relaxed); }
 
 int b200gs_project_fwd(const B200gsView* view, int64_t n, const float* means, const float* scales, const float* quats,
@@ -879,21 +879,10 @@ int b200gs_bin_sort(int32_t mode, int32_t width, int32_t height, int64_t n, int3
 int b200gs_blend_fwd(int32_t mode, int32_t width, int32_t height, int32_t channels, const int32_t* tile_ranges,
                      const int32_t* sorted_ids, const float* xy, const float* conic, const float* opacity,
                      const float* colors, const float* bg, float* image, int64_t pix_stride, int64_t ch_stride,
-                     float* final_T, int32_t* n_contrib, float* alpha, void* stream) {
+                     float* final_T, int32_t* n_contrib, float* alpha, uint8_t* hit_any, void* stream) {
     B200GS_CHECK_ARG(mode == B200GS_MODE_VANILLA || mode == B200GS_MODE_GSPLAT, "bad mode");
     B200GS_CHECK_ARG(width > 0 && height > 0, "bad size");
     B200GS_CHECK_ARG(tile_ranges && image && final_T && n_contrib, "NULL output/range pointer");
-    return launch_blend_fwd(mode, width, height, channels, tile_ranges, sorted_ids, false, xy, conic, opacity, colors, bg, image,
-                            pix_stride, ch_stride, final_T, n_contrib, alpha, (cudaStream_t)stream);
-}
-
-int b200gs_blend_fwd_hits(int32_t mode, int32_t width, int32_t height, int32_t channels, const int32_t* tile_ranges,
-                          const int32_t* sorted_ids, const float* xy, const float* conic, const float* opacity,
-                          const float* colors, const float* bg, float* image, int64_t pix_stride, int64_t ch_stride,
-                          float* final_T, int32_t* n_contrib, float* alpha, uint8_t* hit_any, void* stream) {
-    B200GS_CHECK_ARG(mode == B200GS_MODE_VANILLA || mode == B200GS_MODE_GSPLAT, "bad mode");
-    B200GS_CHECK_ARG(width > 0 && height > 0, "bad size");
-    B200GS_CHECK_ARG(tile_ranges && image && final_T && n_contrib && hit_any, "NULL output/range pointer");
     return launch_blend_fwd(mode, width, height, channels, tile_ranges, sorted_ids, false, xy, conic, opacity, colors, bg, image,
                             pix_stride, ch_stride, final_T, n_contrib, alpha, (cudaStream_t)stream, hit_any);
 }

@@ -302,12 +302,6 @@ def bin_and_blend_rows(mode, width, height, rows, bg, cull=True, planar=False, b
                            lambda binning: blend_forward_rows(mode, width, height, binning, rows, bg, planar))
 
 
-def bin_and_blend(mode, width, height, xy, depth, radii, conic, opacity, colors, bg, planar, want_alpha):
-    """Forward binning + blend with the lazy (sync-free) pair count; falls back to an exact re-run on overflow."""
-    return _bin_then_blend(lambda lazy: bin_gaussians(mode, width, height, xy, depth, radii, conic, opacity, lazy=lazy),
-                           lambda binning: blend_forward(mode, width, height, binning, xy, conic, opacity, colors, bg, planar, want_alpha))
-
-
 # ----------------------------------------------------------------------------------------------------------------------
 # raw stage calls (no autograd) — also used directly by tests
 # ----------------------------------------------------------------------------------------------------------------------
@@ -350,7 +344,7 @@ def project_backward(view: B200gsView, means, scales, quats, shs, radii, clamped
 
 def blend_forward(mode, width, height, binning: Binning, xy, conic, opacity, colors, bg, planar: bool, want_alpha: bool, hit_any=None):
     """planar=True -> image [C,H,W] (vanilla); else [H,W,C] (gsplat).  hit_any: zero-filled uint8 [N] that receives 1 for every splat
-    that contributed to a pixel (b200gs_blend_fwd_hits)."""
+    that contributed to a pixel."""
     L = lib()
     ch = colors.shape[1]
     dev = xy.device
@@ -364,14 +358,9 @@ def blend_forward(mode, width, height, binning: Binning, xy, conic, opacity, col
     n_contrib = torch.empty(height, width, dtype=torch.int32, device=dev)
     alpha = torch.empty(height, width, dtype=torch.float32, device=dev) if want_alpha else None
     with _stage("blend_fwd"):
-        if hit_any is None:
-            check(L.b200gs_blend_fwd(mode, width, height, ch, ptr(binning.tile_ranges), ptr(binning.sorted_ids), ptr(xy), ptr(conic),
-                                     ptr(opacity), ptr(colors), ptr(bg), ptr(image), ps, cs, ptr(final_T), ptr(n_contrib), ptr(alpha),
-                                     _stream()), "b200gs_blend_fwd")
-        else:
-            check(L.b200gs_blend_fwd_hits(mode, width, height, ch, ptr(binning.tile_ranges), ptr(binning.sorted_ids), ptr(xy), ptr(conic),
-                                          ptr(opacity), ptr(colors), ptr(bg), ptr(image), ps, cs, ptr(final_T), ptr(n_contrib), ptr(alpha),
-                                          ptr(hit_any), _stream()), "b200gs_blend_fwd_hits")
+        check(L.b200gs_blend_fwd(mode, width, height, ch, ptr(binning.tile_ranges), ptr(binning.sorted_ids), ptr(xy), ptr(conic),
+                                 ptr(opacity), ptr(colors), ptr(bg), ptr(image), ps, cs, ptr(final_T), ptr(n_contrib), ptr(alpha),
+                                 ptr(hit_any), _stream()), "b200gs_blend_fwd")
     return image, final_T, n_contrib, alpha
 
 
@@ -460,7 +449,9 @@ class _RasterizeVanilla(torch.autograd.Function):
         W, H = view.width, view.height
         xy, depth, radii, conic, _, tiles, _, rgb, clamped = project_forward(view, means3D, scales, rotations, shs if use_sh else None)
         colors = rgb if use_sh else colors_precomp
-        binning, (image, final_T, n_contrib, _) = bin_and_blend(MODE_VANILLA, W, H, xy, depth, radii, conic, opac, colors, bg, True, False)
+        binning, (image, final_T, n_contrib, _) = _bin_then_blend(
+            lambda lazy: bin_gaussians(MODE_VANILLA, W, H, xy, depth, radii, conic, opac, lazy=lazy),
+            lambda binning: blend_forward(MODE_VANILLA, W, H, binning, xy, conic, opac, colors, bg, True, False))
         ctx.view = view
         ctx.use_sh = use_sh
         ctx.binning = binning
@@ -805,77 +796,73 @@ def glossy_sh(degree: int, means: torch.Tensor, campos: torch.Tensor, op_dc: tor
     return _GlossySH.apply(degree, split, m, means, campos, op_dc, op_rest, shs, shs_rest)
 
 
-class _RasterizeGaussians(torch.autograd.Function):
+def _check_channels(colors, background):
+    if colors.dim() != 2 or colors.shape[1] < 1:
+        raise ValueError("colors must be [N, D] with D >= 1")
+    if background is not None and background.shape[0] != colors.shape[1]:
+        raise ValueError("background must have one entry per colour channel")
+
+
+class _RasterizeGsplat(torch.autograd.Function):
+    """The gsplat-mode blend of [N, D] colours behind rasterize_gaussians and rasterize_binned.
+
+    binning: a Binning computed beforehand, or None to bin here from depths / radii with the lazy protocol (_bin_then_blend).
+    D <= 4 runs K6 / K7; wider D the D-channel kernels, whose backward skips the geometry gradients when none of xys, conics and
+    opacity needs one.  want_hits (K6 only): also return uint8 [N] has-hit flags.  absgrad: after the backward, `xys.absgrad`
+    holds this blend's value, or with sum_absgrad, that value added to the one it already holds (so the channel groups and the
+    passes of one render accumulate)."""
+
     @staticmethod
-    def forward(ctx, xys, depths, radii, conics, colors, opacity, img_height, img_width, background, return_alpha, absgrad):
+    def forward(ctx, xys, conics, colors, opacity, background, depths, radii, binning, hw, absgrad, sum_absgrad, want_hits):
         xys = _f32c(xys, "xys")
-        depths = _f32c(depths, "depths")
         conics = _f32c(conics, "conics")
         colors = _f32c(colors, "colors")
         opac = _f32c(opacity, "opacity").reshape(-1)
-        radii = radii.contiguous()
         bg = _f32c(background, "background") if background is not None else None
-        H, W = int(img_height), int(img_width)
-        binning, (image, final_T, n_contrib, alpha) = bin_and_blend(MODE_GSPLAT, W, H, xys, depths, radii, conics, opac, colors, bg, False, True)
-        ctx.binning = binning
-        ctx.hw = (H, W)
-        ctx.absgrad = absgrad
-        ctx.opac_shape = tuple(opacity.shape)
+        H, W = hw
+        features = colors.shape[1] > 4
+
+        def blend(binning):
+            if features:
+                return (*blend_features_forward(W, H, binning, xys, conics, opac, colors, bg), None)
+            hits = torch.zeros(xys.shape[0], dtype=torch.uint8, device=xys.device) if want_hits else None
+            return (*blend_forward(MODE_GSPLAT, W, H, binning, xys, conics, opac, colors, bg, False, True, hits), hits)
+
+        if binning is None:
+            depths, radii = _f32c(depths, "depths"), radii.contiguous()
+            binning, out = _bin_then_blend(lambda lazy: bin_gaussians(MODE_GSPLAT, W, H, xys, depths, radii, conics, opac, lazy=lazy), blend)
+        else:
+            out = blend(binning)
+        image, final_T, n_contrib, alpha, hits = out
+        ctx.binning, ctx.hw, ctx.features, ctx.opac_shape = binning, hw, features, tuple(opacity.shape)
+        ctx.absgrad, ctx.sum_absgrad = absgrad, sum_absgrad
         ctx.save_for_backward(xys, conics, colors, opac, bg, final_T, n_contrib)
         ctx.xys_ref = xys
-        return image, alpha
+        if hits is None:
+            return image, alpha
+        ctx.mark_non_differentiable(hits)
+        return image, alpha, hits
 
     @staticmethod
-    def backward(ctx, v_image, v_alpha):
-        xys, conics, colors, opac, bg, final_T, n_contrib = ctx.saved_tensors
-        H, W = ctx.hw
-        v_image = _f32c(v_image, "grad_image")
-        v_alpha = _f32c(v_alpha, "grad_alpha") if v_alpha is not None else None
-        v_xy, v_conic, v_opacity, v_colors, v_abs = blend_backward(MODE_GSPLAT, W, H, ctx.binning, xys, conics, opac, colors, bg,
-                                                                   final_T, n_contrib, v_image, v_alpha, False, (1.0, 1.0),
-                                                                   ctx.absgrad)
-        if ctx.absgrad:
-            ctx.xys_ref.absgrad = v_abs
-        return v_xy, None, None, v_conic, v_colors, v_opacity.reshape(ctx.opac_shape), None, None, None, None, None
-
-
-class _RasterizeFeatures(torch.autograd.Function):
-    """rasterize_gaussians for D > 4 channels (the reference's feature renderers: 32-channel features, often with the geometry
-    frozen).  One binning, the D-channel blend kernels; the backward runs the features-only kernels when none of xys, conics and
-    opacity needs a gradient."""
-
-    @staticmethod
-    def forward(ctx, xys, depths, radii, conics, colors, opacity, img_height, img_width, background, absgrad):
-        xys = _f32c(xys, "xys")
-        depths = _f32c(depths, "depths")
-        conics = _f32c(conics, "conics")
-        colors = _f32c(colors, "colors")
-        opac = _f32c(opacity, "opacity").reshape(-1)
-        radii = radii.contiguous()
-        bg = _f32c(background, "background") if background is not None else None
-        H, W = int(img_height), int(img_width)
-        binning, (image, final_T, n_contrib, alpha) = _bin_then_blend(
-            lambda lazy: bin_gaussians(MODE_GSPLAT, W, H, xys, depths, radii, conics, opac, lazy=lazy),
-            lambda binning: blend_features_forward(W, H, binning, xys, conics, opac, colors, bg))
-        ctx.binning, ctx.hw, ctx.absgrad, ctx.opac_shape = binning, (H, W), bool(absgrad), tuple(opacity.shape)
-        ctx.save_for_backward(xys, conics, colors, opac, bg, final_T, n_contrib)
-        ctx.xys_ref = xys
-        return image, alpha
-
-    @staticmethod
-    def backward(ctx, v_image, v_alpha):
+    def backward(ctx, v_image, v_alpha, *_):
         xys, conics, colors, opac, bg, final_T, n_contrib = ctx.saved_tensors
         H, W = ctx.hw
         need = ctx.needs_input_grad
-        geometry = need[0] or need[3] or need[5]
         v_image = _f32c(v_image, "grad_image")
         v_alpha = _f32c(v_alpha, "grad_alpha") if v_alpha is not None else None
-        v_xy, v_conic, v_opacity, v_colors, v_abs = blend_features_backward(W, H, ctx.binning, xys, conics, opac, colors, bg, final_T,
-                                                                            n_contrib, v_image, v_alpha, geometry, geometry and ctx.absgrad)
+        if ctx.features:
+            geometry = need[0] or need[1] or need[3]
+            grads = blend_features_backward(W, H, ctx.binning, xys, conics, opac, colors, bg, final_T, n_contrib, v_image, v_alpha,
+                                            geometry, geometry and ctx.absgrad)
+        else:
+            grads = blend_backward(MODE_GSPLAT, W, H, ctx.binning, xys, conics, opac, colors, bg, final_T, n_contrib, v_image, v_alpha,
+                                   False, (1.0, 1.0), ctx.absgrad)
+        v_xy, v_conic, v_opacity, v_colors, v_abs = grads
         if v_abs is not None:
-            ctx.xys_ref.absgrad = v_abs
-        return (v_xy, None, None, v_conic, v_colors if need[4] else None, v_opacity.reshape(ctx.opac_shape) if geometry else None,
-                None, None, None, None)
+            prev = getattr(ctx.xys_ref, "absgrad", None) if ctx.sum_absgrad else None
+            ctx.xys_ref.absgrad = v_abs if prev is None else prev + v_abs
+        return (v_xy if need[0] else None, v_conic if need[1] else None, v_colors if need[2] else None,
+                v_opacity.reshape(ctx.opac_shape) if need[3] else None) + (None,) * 8
 
 
 def rasterize_gaussians(xys, depths, radii, conics, num_tiles_hit, colors, opacity, img_height, img_width, block_width=16,
@@ -885,66 +872,27 @@ def rasterize_gaussians(xys, depths, radii, conics, num_tiles_hit, colors, opaci
     it is the sum of each 32-channel chunk's value (an upper bound of gsplat's all-channel value)."""
     if block_width != TILE:
         raise ValueError(f"b200gs supports block_width {TILE} only")
-    if colors.dim() != 2 or colors.shape[1] < 1:
-        raise ValueError("colors must be [N, D] with D >= 1")
-    if background is not None and background.shape[0] != colors.shape[1]:
-        raise ValueError("background must have one entry per colour channel")
-    if colors.shape[1] <= 4:
-        image, alpha = _RasterizeGaussians.apply(xys, depths, radii, conics, colors, opacity, img_height, img_width, background,
-                                                 return_alpha, absgrad)
-    else:
-        image, alpha = _RasterizeFeatures.apply(xys, depths, radii, conics, colors, opacity, img_height, img_width, background, absgrad)
+    _check_channels(colors, background)
+    image, alpha = _RasterizeGsplat.apply(xys, conics, colors, opacity, background, depths, radii, None, (int(img_height), int(img_width)),
+                                          bool(absgrad), False, False)
     return (image, alpha) if return_alpha else image
-
-
-class _RasterizeBinned(torch.autograd.Function):
-    """K6 / K7 on a binning computed beforehand (gsplat v1: isect_tiles + isect_offset_encode once, rasterize_to_pixels several
-    times with different colour sets — gsplat_v1_renderer.py:176-196,326-352).  <= 4 channels per call."""
-
-    @staticmethod
-    def forward(ctx, xys, conics, colors, opacity, background, binning, hw, absgrad, want_hits):
-        xys = _f32c(xys, "means2d")
-        conics = _f32c(conics, "conics")
-        colors = _f32c(colors, "colors")
-        opac = _f32c(opacity, "opacities").reshape(-1)
-        bg = _f32c(background, "background") if background is not None else None
-        H, W = hw
-        hits = torch.zeros(xys.shape[0], dtype=torch.uint8, device=xys.device) if want_hits else None
-        image, final_T, n_contrib, alpha = blend_forward(MODE_GSPLAT, W, H, binning, xys, conics, opac, colors, bg, False, True, hits)
-        ctx.binning, ctx.hw, ctx.absgrad, ctx.opac_shape = binning, hw, bool(absgrad), tuple(opacity.shape)
-        ctx.save_for_backward(xys, conics, colors, opac, bg, final_T, n_contrib)
-        ctx.xys_ref = xys
-        ctx.mark_non_differentiable(*([hits] if hits is not None else []))
-        return (image, alpha, hits) if hits is not None else (image, alpha)
-
-    @staticmethod
-    def backward(ctx, v_image, v_alpha, *_):
-        xys, conics, colors, opac, bg, final_T, n_contrib = ctx.saved_tensors
-        H, W = ctx.hw
-        v_image = _f32c(v_image, "grad_image")
-        v_alpha = _f32c(v_alpha, "grad_alpha") if v_alpha is not None else None
-        v_xy, v_conic, v_opacity, v_colors, v_abs = blend_backward(MODE_GSPLAT, W, H, ctx.binning, xys, conics, opac, colors, bg, final_T,
-                                                                   n_contrib, v_image, v_alpha, False, (1.0, 1.0), ctx.absgrad)
-        if ctx.absgrad:   # channel groups of one render accumulate (|.| per group: an upper bound of gsplat's all-channel value when D > 4)
-            prev = getattr(ctx.xys_ref, "absgrad", None)
-            ctx.xys_ref.absgrad = v_abs if prev is None else prev + v_abs
-        return v_xy, v_conic, v_colors, v_opacity.reshape(ctx.opac_shape), None, None, None, None, None
 
 
 def rasterize_binned(means2d, conics, colors, opacities, binning: Binning, img_height: int, img_width: int, background=None,
                      absgrad: bool = False, want_hits: bool = False):
-    """-> (image [H,W,D], alpha [H,W], hits uint8 [N] or None) for any D >= 1: the channels are composited in groups of <= 4 over the
-    same per-tile lists (alpha / hits come from the first group; `means2d.absgrad`, when requested, accumulates every group's)."""
-    if colors.dim() != 2 or colors.shape[1] < 1:
-        raise ValueError("colors must be [N, D] with D >= 1")
-    if background is not None and background.shape[0] != colors.shape[1]:
-        raise ValueError("background must have one entry per colour channel")
+    """K6 / K7 on a binning computed beforehand (gsplat v1: isect_tiles + isect_offset_encode once, rasterize_to_pixels several
+    times with different colour sets — gsplat_v1_renderer.py:176-196,326-352).
+    -> (image [H,W,D], alpha [H,W], hits uint8 [N] or None) for any D >= 1: the channels are composited in groups of <= 4 over the
+    same per-tile lists (alpha / hits come from the first group; `means2d.absgrad`, when requested, accumulates every group's: |.|
+    per group, an upper bound of gsplat's all-channel value when D > 4).  The groups stay on K6 / K7 even when D > 4: only K6
+    writes hits, and with a background the D-channel kernels round the background term differently (see csrc/blend.cu)."""
+    _check_channels(colors, background)
     D = colors.shape[1]
-    images, alpha, hits, abs_total = [], None, None, None
+    images, alpha, hits = [], None, None
     for c0 in range(0, D, 4):
         c1 = min(D, c0 + 4)
-        out = _RasterizeBinned.apply(means2d, conics, colors[:, c0:c1], opacities, None if background is None else background[c0:c1], binning,
-                                     (int(img_height), int(img_width)), absgrad, want_hits and c0 == 0)
+        out = _RasterizeGsplat.apply(means2d, conics, colors[:, c0:c1], opacities, None if background is None else background[c0:c1], None,
+                                     None, binning, (int(img_height), int(img_width)), bool(absgrad), True, want_hits and c0 == 0)
         images.append(out[0])
         if c0 == 0:
             alpha = out[1]

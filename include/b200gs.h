@@ -545,14 +545,10 @@ B200GS_API int b200gs_publish_i64(const int64_t* d_values, int64_t* host_values,
  * in : xy[n,2] conic[n,3] opacity[n] colors[n,channels]; bg[channels] or NULL.
  * out: image, addressed as image[pixel*pix_stride + channel*ch_stride] (vanilla [C,H,W]: pix_stride 1, ch_stride H*W;
  *      gsplat [H,W,C]: pix_stride C, ch_stride 1); final_T[H*W]; n_contrib[H*W] (1-based position in the tile's list of
- *      the last contributing splat); alpha[H*W] = 1 - final_T (nullable). */
+ *      the last contributing splat); alpha[H*W] = 1 - final_T (nullable); hit_any[n] (nullable; caller zero-fills): 1 for every
+ *      splat that contributed to at least one pixel, gsplat's `means2d.has_hit_any_pixels` (optimizers.py:39 SelectiveAdam;
+ *      gsplat_v1_renderer.py:287 acc_vis). */
 B200GS_API int b200gs_blend_fwd(int32_t mode, int32_t width, int32_t height, int32_t channels, const int32_t* tile_ranges,
-                     const int32_t* sorted_ids, const float* xy, const float* conic, const float* opacity,
-                     const float* colors, const float* bg, float* image, int64_t pix_stride, int64_t ch_stride,
-                     float* final_T, int32_t* n_contrib, float* alpha, void* stream);
-/* b200gs_blend_fwd_hits: the same, and hit_any[g] = 1 for every splat g that contributed to at least one pixel (caller zero-fills
- *     hit_any[n]): gsplat's `means2d.has_hit_any_pixels` (optimizers.py:39 SelectiveAdam; gsplat_v1_renderer.py:287 acc_vis). */
-B200GS_API int b200gs_blend_fwd_hits(int32_t mode, int32_t width, int32_t height, int32_t channels, const int32_t* tile_ranges,
                      const int32_t* sorted_ids, const float* xy, const float* conic, const float* opacity,
                      const float* colors, const float* bg, float* image, int64_t pix_stride, int64_t ch_stride,
                      float* final_T, int32_t* n_contrib, float* alpha, uint8_t* hit_any, void* stream);

@@ -63,7 +63,7 @@ def test_argument_validation_without_gpu(lib):
     assert L.b200gs_project_fwd(ctypes.byref(v), 5, dummy, dummy, dummy, dummy, *([dummy] * 9), None) == -1
     assert b"sh_stride" in L.b200gs_last_error()
     # unsupported channel count / bad image size in the blend entry points
-    assert L.b200gs_blend_fwd(0, 0, 64, 3, *([None] * 7), None, 1, 1, None, None, None, None) == -1
+    assert L.b200gs_blend_fwd(0, 0, 64, 3, *([None] * 7), None, 1, 1, None, None, None, None, None) == -1
     # [n,12] row buffers that are not 16-byte aligned (every other pointer is a non-NULL dummy)
     d16, d8 = ctypes.c_void_p(16), ctypes.c_void_p(8)
     assert L.b200gs_blend_fwd_rows(0, 64, 64, d16, d16, d8, d16, d16, 3, 1, d16, d16, d16, None) == -1
