@@ -564,22 +564,16 @@ __global__ void appearance_reduce_kernel(const float* __restrict__ partials, int
     out[i] = sum;
 }
 
-}  // namespace
-
-int64_t appearance_mlp_params(int feat_dim, int n_freq, int n_neurons, int n_layers, int n_out) {
-    return AppShape{feat_dim, n_freq, n_neurons, n_layers, n_out}.params();
-}
-
 bool appearance_mlp_fits(int feat_dim, int n_freq, int n_neurons, int n_layers, int n_out) {
     return app_warps(AppShape{feat_dim, n_freq, n_neurons, n_layers, n_out}, true) > 0;
 }
 
 size_t appearance_mlp_workspace_bytes(int feat_dim, int n_freq, int n_neurons, int n_layers, int n_out) {
-    return size_t(APP_MAX_CTAS) * size_t(appearance_mlp_params(feat_dim, n_freq, n_neurons, n_layers, n_out)) * sizeof(float);
+    return size_t(APP_MAX_CTAS) * size_t(AppShape{feat_dim, n_freq, n_neurons, n_layers, n_out}.params()) * sizeof(float);
 }
 
-static AppParams app_params(const B200gsAppearanceMlp& m, int64_t n, const float* features, const uint8_t* mask, const float* base_rgb,
-                            const float* dirs, const float* cam, const float* raw_opacity) {
+AppParams app_params(const B200gsAppearanceMlp& m, int64_t n, const float* features, const uint8_t* mask, const float* base_rgb,
+                     const float* dirs, const float* cam, const float* raw_opacity) {
     AppParams p{};
     p.s = AppShape{m.feat_dim, m.n_freq, m.n_neurons, m.n_layers, m.n_out};
     p.n = n;
@@ -591,7 +585,7 @@ static AppParams app_params(const B200gsAppearanceMlp& m, int64_t n, const float
 }
 
 template <typename K>
-static int app_launch(K kernel, const AppParams& p, bool bwd, int* grid_out, cudaStream_t s) {
+int app_launch(K kernel, const AppParams& p, bool bwd, int* grid_out, cudaStream_t s) {
     const int warps = app_warps(p.s, bwd);
     const AppLayout lay = app_layout(p.s, warps, bwd);
     const int threads = 32 * warps, smem = lay.total * 4;
@@ -603,6 +597,8 @@ static int app_launch(K kernel, const AppParams& p, bool bwd, int* grid_out, cud
     return B200GS_OK;
 }
 
+// The launch path of both networks: the visibility MLP is an appearance MLP with n_freq -1, n_out 1, no normalisation and no
+// epilogue.  The shape of m has been validated.
 int launch_appearance_mlp_fwd(const B200gsAppearanceMlp& m, int64_t n, const float* features, const uint8_t* mask, const float* base_rgb,
                               const float* dirs, const float* cam, const float* raw_opacity, float* out, float* opacity_offsets,
                               float* opacities, cudaStream_t s) {
@@ -628,4 +624,113 @@ int launch_appearance_mlp_bwd(const B200gsAppearanceMlp& m, int64_t n, const flo
     return B200GS_OK;
 }
 
+bool appearance_shape_ok(int32_t feat_dim, int32_t n_freq, int32_t n_neurons, int32_t n_layers, int32_t n_out) {
+    return feat_dim >= 8 && feat_dim % 8 == 0 && feat_dim <= 1024 && n_freq <= 16 && (n_neurons == 64 || n_neurons == 128) && n_layers >= 2 &&
+           n_layers <= B200GS_APPEARANCE_MAX_LAYERS && (n_out == 3 || n_out == 4) &&
+           appearance_mlp_fits(feat_dim, n_freq, n_neurons, n_layers, n_out);
+}
+
+int check_appearance(const char* fn, const B200gsAppearanceMlp* m, int64_t n, const float* features, const float* base_rgb,
+                     const float* dirs, const float* raw_opacity) {
+    if (m == nullptr) return fail(fn, "mlp is NULL");
+    if (m->feat_dim < 8 || m->feat_dim % 8 != 0) return fail(fn, "feat_dim must be a positive multiple of 8");
+    if (m->n_neurons != 64 && m->n_neurons != 128) return fail(fn, "n_neurons must be 64 or 128");
+    if (m->n_layers < 2 || m->n_layers > B200GS_APPEARANCE_MAX_LAYERS) return fail(fn, "n_layers must be 2..4");
+    if (m->n_out != 3 && m->n_out != 4) return fail(fn, "n_out must be 3 or 4");
+    if (!appearance_shape_ok(m->feat_dim, m->n_freq, m->n_neurons, m->n_layers, m->n_out)) return fail(fn, "network does not fit shared memory");
+    const int pe = m->n_freq < 0 ? 0 : 3 * (2 * m->n_freq + 1);
+    if (m->w0_stride < m->feat_dim + pe || m->w0_pe_col < m->feat_dim || m->w0_pe_col + pe > m->w0_stride) return fail(fn, "bad w0_stride / w0_pe_col");
+    if (n < 0 || n > INT32_MAX) return fail(fn, "n out of range");
+    for (int l = 0; l < m->n_layers; ++l)
+        if (!m->weights[l] || !m->biases[l]) return fail(fn, "NULL weight or bias pointer");
+    if (n > 0) {
+        if (!features) return fail(fn, "NULL features");
+        if (m->n_freq >= 0 && !dirs) return fail(fn, "NULL dirs with a view direction");
+        if (m->epilogue && !base_rgb) return fail(fn, "NULL base_rgb");
+        if (m->epilogue && m->n_out == 4 && !raw_opacity) return fail(fn, "NULL raw_opacity");
+    }
+    return B200GS_OK;
+}
+
+bool visibility_shape_ok(int32_t feat_dim, int32_t n_neurons, int32_t n_layers) {
+    return feat_dim >= 8 && feat_dim % 8 == 0 && feat_dim <= 32 && (n_neurons == 64 || n_neurons == 128) && n_layers >= 2 &&
+           n_layers <= B200GS_APPEARANCE_MAX_LAYERS && appearance_mlp_fits(feat_dim, -1, n_neurons, n_layers, 1);
+}
+
+int check_visibility(const char* fn, const B200gsAppearanceMlp* m, int64_t n, const float* enc) {
+    if (m == nullptr) return fail(fn, "mlp is NULL");
+    if (m->n_freq != -1 || m->n_out != 1 || m->normalize || m->normalize_dirs || m->epilogue)
+        return fail(fn, "a visibility network has n_freq -1, n_out 1 and no normalisation or epilogue");
+    if (!visibility_shape_ok(m->feat_dim, m->n_neurons, m->n_layers))
+        return fail(fn, "feat_dim must be 8, 16, 24 or 32, n_neurons 64 or 128, n_layers 2..4");
+    if (m->w0_stride < m->feat_dim || m->w0_pe_col < m->feat_dim || m->w0_pe_col > m->w0_stride) return fail(fn, "bad w0_stride / w0_pe_col");
+    if (n < 0 || n > INT32_MAX) return fail(fn, "n out of range");
+    for (int l = 0; l < m->n_layers; ++l)
+        if (!m->weights[l] || !m->biases[l]) return fail(fn, "NULL weight or bias pointer");
+    if (n > 0 && !enc) return fail(fn, "NULL enc");
+    return B200GS_OK;
+}
+
+}  // namespace
+
 }  // namespace b200gs
+
+using namespace b200gs;
+
+extern "C" {
+
+size_t b200gs_appearance_mlp_workspace_bytes(int32_t feat_dim, int32_t n_freq, int32_t n_neurons, int32_t n_layers, int32_t n_out) {
+    if (!appearance_shape_ok(feat_dim, n_freq, n_neurons, n_layers, n_out)) return 0;
+    return appearance_mlp_workspace_bytes(feat_dim, n_freq, n_neurons, n_layers, n_out);
+}
+
+int b200gs_appearance_mlp_fwd(const B200gsAppearanceMlp* mlp, int64_t n, const float* features, const uint8_t* mask, const float* base_rgb,
+                              const float* dirs, const float* cam, const float* raw_opacity, float* out, float* opacity_offsets,
+                              float* opacities, void* stream) {
+    if (int rc = check_appearance(__func__, mlp, n, features, base_rgb, dirs, raw_opacity)) return rc;
+    B200GS_CHECK_ARG(n == 0 || out, "NULL out");
+    B200GS_CHECK_ARG(n == 0 || !(mlp->epilogue && mlp->n_out == 4) || (opacity_offsets && opacities), "NULL opacity output");
+    return launch_appearance_mlp_fwd(*mlp, n, features, mask, base_rgb, dirs, cam, raw_opacity, out, opacity_offsets, opacities,
+                                     (cudaStream_t)stream);
+}
+
+int b200gs_appearance_mlp_bwd(const B200gsAppearanceMlp* mlp, int64_t n, const float* features, const uint8_t* mask, const float* base_rgb,
+                              const float* dirs, const float* cam, const float* raw_opacity, const float* v_out, const float* v_opacities,
+                              const float* v_opacity_offsets, float* v_base_rgb, float* v_features, float* v_raw_opacity, void* workspace,
+                              size_t workspace_bytes, float* v_params, void* stream) {
+    if (int rc = check_appearance(__func__, mlp, n, features, base_rgb, dirs, raw_opacity)) return rc;
+    B200GS_CHECK_ARG(v_params, "NULL v_params");
+    B200GS_CHECK_ARG(n == 0 || (v_out && workspace), "NULL v_out or workspace");
+    B200GS_CHECK_ARG(n == 0 || !mlp->epilogue || v_base_rgb, "NULL v_base_rgb");
+    B200GS_CHECK_ARG(n == 0 || !(mlp->epilogue && mlp->n_out == 4) || v_raw_opacity, "NULL v_raw_opacity");
+    B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(v_features) & 15u) == 0, "v_features must be 16-byte aligned");
+    if (n > 0 && workspace_bytes < appearance_mlp_workspace_bytes(mlp->feat_dim, mlp->n_freq, mlp->n_neurons, mlp->n_layers, mlp->n_out))
+        return workspace_too_small(__func__);
+    return launch_appearance_mlp_bwd(*mlp, n, features, mask, base_rgb, dirs, cam, raw_opacity, v_out, v_opacities, v_opacity_offsets,
+                                     v_base_rgb, v_features, v_raw_opacity, static_cast<float*>(workspace), v_params, (cudaStream_t)stream);
+}
+
+size_t b200gs_visibility_mlp_workspace_bytes(int32_t feat_dim, int32_t n_neurons, int32_t n_layers) {
+    if (!visibility_shape_ok(feat_dim, n_neurons, n_layers)) return 0;
+    return appearance_mlp_workspace_bytes(feat_dim, -1, n_neurons, n_layers, 1);
+}
+
+int b200gs_visibility_mlp_fwd(const B200gsAppearanceMlp* mlp, int64_t n, const float* enc, float* out, void* stream) {
+    if (int rc = check_visibility(__func__, mlp, n, enc)) return rc;
+    B200GS_CHECK_ARG(n == 0 || out, "NULL out");
+    return launch_appearance_mlp_fwd(*mlp, n, enc, nullptr, nullptr, nullptr, nullptr, nullptr, out, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+int b200gs_visibility_mlp_bwd(const B200gsAppearanceMlp* mlp, int64_t n, const float* enc, const float* v_out, float* v_enc,
+                              void* workspace, size_t workspace_bytes, float* v_params, void* stream) {
+    if (int rc = check_visibility(__func__, mlp, n, enc)) return rc;
+    B200GS_CHECK_ARG(v_params, "NULL v_params");
+    B200GS_CHECK_ARG(n == 0 || (v_out && workspace), "NULL v_out or workspace");
+    B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(v_enc) & 15u) == 0, "v_enc must be 16-byte aligned");
+    if (n > 0 && workspace_bytes < appearance_mlp_workspace_bytes(mlp->feat_dim, -1, mlp->n_neurons, mlp->n_layers, 1))
+        return workspace_too_small(__func__);
+    return launch_appearance_mlp_bwd(*mlp, n, enc, nullptr, nullptr, nullptr, nullptr, nullptr, v_out, nullptr, nullptr, nullptr, v_enc,
+                                     nullptr, static_cast<float*>(workspace), v_params, (cudaStream_t)stream);
+}
+
+}  // extern "C"

@@ -280,49 +280,89 @@ TvWeights tv_weights(int n, int channels, int L, int gh, int gw) {
     return {w(L), w(gh), w(gw)};
 }
 
+// bilateral grid: grids [n_grids,12,L,gh,gw]; xy [batch,height,width,2]; rgb / out / v_out / v_rgb share the element strides
+// (sb, sy, sx, sc); grid_idx int64 [n_idx], n_idx == 1 (broadcast) or batch.  Shared by the slice entry points; returns the error
+// code, or 0 when the arguments are valid
+int check_bilagrid_slice(const char* fn, int32_t n_grids, int32_t grid_l, int32_t grid_h, int32_t grid_w, const float* grids, int32_t batch,
+                         int32_t height, int32_t width, const float* xy, const float* rgb, int64_t sb, int64_t sy, int64_t sx, int64_t sc,
+                         const int64_t* grid_idx, int32_t n_idx, const void* out) {
+    if (n_grids < 1 || grid_l < 1 || grid_h < 1 || grid_w < 1) return fail(fn, "grid sizes must be >= 1");
+    if (int64_t(12) * grid_l * grid_h * grid_w > INT32_MAX) return fail(fn, "grid too large");
+    if (batch < 0 || height < 0 || width < 0) return fail(fn, "negative image size");
+    if (sb < 0 || sy < 0 || sx < 0 || sc < 0) return fail(fn, "negative stride");
+    if (n_idx != 1 && n_idx != batch) return fail(fn, "n_idx must be 1 or batch");
+    if (int64_t(batch) * height * width > 0 && !(grids && xy && rgb && grid_idx && out)) return fail(fn, "NULL pointer");
+    return 0;
+}
+
+int check_bilagrid_tv(const char* fn, int32_t n, int32_t channels, int32_t grid_l, int32_t grid_h, int32_t grid_w, const float* grids,
+                      const void* out) {
+    if (n < 0 || channels < 0 || grid_l < 0 || grid_h < 0 || grid_w < 0) return fail(fn, "negative size");
+    const int64_t total = int64_t(n) * channels * grid_l * grid_h * grid_w;
+    if (total / 256 >= INT32_MAX) return fail(fn, "grids too large");
+    if (total > 0 && !(grids && out)) return fail(fn, "NULL pointer");
+    return 0;
+}
+
 }  // namespace
 
-int launch_bilagrid_slice_fwd(int n_grids, int L, int gh, int gw, const float* grids, int batch, int height, int width, const float* xy,
-                              const float* rgb, int64_t sb, int64_t sy, int64_t sx, int64_t sc, const int64_t* grid_idx, int n_idx,
-                              float* out, cudaStream_t s) {
+}  // namespace b200gs
+
+using namespace b200gs;
+
+extern "C" {
+
+int b200gs_bilagrid_slice_fwd(int32_t n_grids, int32_t L, int32_t gh, int32_t gw, const float* grids, int32_t batch, int32_t height,
+                              int32_t width, const float* xy, const float* rgb, int64_t sb, int64_t sy, int64_t sx, int64_t sc,
+                              const int64_t* grid_idx, int32_t n_idx, float* out, void* stream) {
+    if (int rc = check_bilagrid_slice(__func__, n_grids, L, gh, gw, grids, batch, height, width, xy, rgb, sb, sy, sx, sc, grid_idx, n_idx, out))
+        return rc;
     if (int64_t(batch) * height * width == 0) return B200GS_OK;
-    slice_fwd_kernel<<<dim3(div_up(width, BT), div_up(height, BT), batch), dim3(BT, BT), 0, s>>>(
+    slice_fwd_kernel<<<dim3(div_up(width, BT), div_up(height, BT), batch), dim3(BT, BT), 0, (cudaStream_t)stream>>>(
         n_grids, L, gh, gw, grids, height, width, xy, rgb, sb, sy, sx, sc, grid_idx, n_idx, out);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-int launch_bilagrid_slice_bwd(int n_grids, int L, int gh, int gw, const float* grids, int batch, int height, int width, const float* xy,
-                              const float* rgb, int64_t sb, int64_t sy, int64_t sx, int64_t sc, const int64_t* grid_idx, int n_idx,
-                              const float* v_out, float* v_rgb, float* v_grids, cudaStream_t s) {
+int b200gs_bilagrid_slice_bwd(int32_t n_grids, int32_t L, int32_t gh, int32_t gw, const float* grids, int32_t batch, int32_t height,
+                              int32_t width, const float* xy, const float* rgb, int64_t sb, int64_t sy, int64_t sx, int64_t sc,
+                              const int64_t* grid_idx, int32_t n_idx, const float* v_out, float* v_rgb, float* v_grids, void* stream) {
+    if (int rc = check_bilagrid_slice(__func__, n_grids, L, gh, gw, grids, batch, height, width, xy, rgb, sb, sy, sx, sc, grid_idx, n_idx,
+                                      v_out))
+        return rc;
     if (int64_t(batch) * height * width == 0 || (!v_rgb && !v_grids)) return B200GS_OK;
-    slice_bwd_kernel<<<dim3(div_up(width, BT), div_up(height, BT), batch), dim3(BT, BT), 0, s>>>(
+    slice_bwd_kernel<<<dim3(div_up(width, BT), div_up(height, BT), batch), dim3(BT, BT), 0, (cudaStream_t)stream>>>(
         n_grids, L, gh, gw, grids, height, width, xy, rgb, sb, sy, sx, sc, grid_idx, n_idx, v_out, v_rgb, v_grids);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-int64_t bilagrid_tv_blocks(int n, int channels, int L, int gh, int gw) {
+int64_t b200gs_bilagrid_tv_blocks(int32_t n, int32_t channels, int32_t L, int32_t gh, int32_t gw) {
+    if (n < 0 || channels < 0 || L < 0 || gh < 0 || gw < 0) return 0;
     return div_up64(int64_t(n) * channels * L * gh * gw, TV_THREADS);
 }
 
-int launch_bilagrid_tv_fwd(int n, int channels, int L, int gh, int gw, const float* grids, float* partials, cudaStream_t s) {
+int b200gs_bilagrid_tv_fwd(int32_t n, int32_t channels, int32_t L, int32_t gh, int32_t gw, const float* grids, float* partials,
+                           void* stream) {
+    if (int rc = check_bilagrid_tv(__func__, n, channels, L, gh, gw, grids, partials)) return rc;
     const int64_t total = int64_t(n) * channels * L * gh * gw;
     if (total == 0) return B200GS_OK;
-    tv_fwd_kernel<<<(unsigned)div_up64(total, TV_THREADS), TV_THREADS, 0, s>>>(total, L, gh, gw, tv_weights(n, channels, L, gh, gw),
-                                                                                grids, partials);
+    tv_fwd_kernel<<<(unsigned)div_up64(total, TV_THREADS), TV_THREADS, 0, (cudaStream_t)stream>>>(
+        total, L, gh, gw, tv_weights(n, channels, L, gh, gw), grids, partials);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-int launch_bilagrid_tv_bwd(int n, int channels, int L, int gh, int gw, const float* grids, const float* v_tv, float* v_grids,
-                           cudaStream_t s) {
+int b200gs_bilagrid_tv_bwd(int32_t n, int32_t channels, int32_t L, int32_t gh, int32_t gw, const float* grids, const float* v_tv,
+                           float* v_grids, void* stream) {
+    if (int rc = check_bilagrid_tv(__func__, n, channels, L, gh, gw, grids, v_grids)) return rc;
     const int64_t total = int64_t(n) * channels * L * gh * gw;
+    B200GS_CHECK_ARG(total == 0 || v_tv, "NULL pointer");
     if (total == 0) return B200GS_OK;
-    tv_bwd_kernel<<<(unsigned)div_up64(total, TV_THREADS), TV_THREADS, 0, s>>>(total, L, gh, gw, tv_weights(n, channels, L, gh, gw),
-                                                                                grids, v_tv, v_grids);
+    tv_bwd_kernel<<<(unsigned)div_up64(total, TV_THREADS), TV_THREADS, 0, (cudaStream_t)stream>>>(
+        total, L, gh, gw, tv_weights(n, channels, L, gh, gw), grids, v_tv, v_grids);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-}  // namespace b200gs
+}  // extern "C"

@@ -818,9 +818,6 @@ __global__ void __launch_bounds__(CHUNK) scatter_ids_kernel(int n_cells, int cgr
 
 }  // namespace
 
-size_t bin_count_workspace_bytes(int64_t n) { return carve_a(nullptr, n).bytes; }
-size_t bin_sort_workspace_bytes(int64_t n, int64_t max_coarse, int width, int height) { return carve_b(nullptr, n, max_coarse, width, height).bytes; }
-
 // Counter read-back.  For pinned (mapped) host memory the counters are PUBLISHED by a kernel with system-scope stores
 // instead of a cudaMemcpyAsync: an in-stream D2H copy is serviced by a copy engine, and queues behind whatever bulk
 // transfer the application has in flight on it (e.g. the H2D prefetch of the next training image) — which would stall
@@ -830,7 +827,7 @@ __global__ void publish_i64_kernel(const int64_t* __restrict__ src, volatile int
     __threadfence_system();
 }
 
-int publish_i64(const int64_t* d_values, int64_t* host_values, int n, cudaStream_t s) {
+static int publish_i64(const int64_t* d_values, int64_t* host_values, int n, cudaStream_t s) {
     cudaPointerAttributes attr{};
     const cudaError_t e = cudaPointerGetAttributes(&attr, host_values);
     if (e == cudaSuccess && attr.type == cudaMemoryTypeHost && attr.devicePointer != nullptr) {
@@ -852,9 +849,12 @@ static int publish_counts(const int64_t* d_counts, int64_t* host_counts, int syn
     return B200GS_OK;
 }
 
-int bin_count(int mode, int width, int height, int64_t n, bool rows, const float* xy, const float* depth, const int32_t* radii,
-              const float* conic, const float* opacity, void* ws, size_t ws_bytes, int64_t* d_counts, int64_t* host_counts,
-              int sync_host, cudaStream_t s, const int64_t* block_counts, int64_t block_rows) {
+// The count stage of both entry points.  rows: xy, depth, radii, conic and opacity are columns of one 16-byte aligned [n,12] row
+// buffer (b200gs.h), optionally in blocks of block_rows rows of which the first block_counts[b] are valid; otherwise separate
+// arrays, conic and opacity NULL without culling
+static int bin_count(int mode, int width, int height, int64_t n, bool rows, const float* xy, const float* depth, const int32_t* radii,
+                     const float* conic, const float* opacity, void* ws, size_t ws_bytes, int64_t* d_counts, int64_t* host_counts,
+                     int sync_host, cudaStream_t s, const int64_t* block_counts = nullptr, int64_t block_rows = 0) {
     const WorkspaceA W = carve_a(ws, n);
     if (ws_bytes < W.bytes) {
         set_error("bin_count: workspace too small (%zu < %zu)", ws_bytes, W.bytes);
@@ -888,73 +888,6 @@ int bin_count(int mode, int width, int height, int64_t n, bool rows, const float
         }
         // 4 passes: the sorted records are back in rec_a
     }
-    return publish_counts(d_counts, host_counts, sync_host, s);
-}
-
-int bin_sort(int mode, int width, int height, int64_t n, int cull, int64_t max_coarse, int64_t max_pairs, int64_t* d_counts,
-             const void* ws_a, void* ws_b, size_t ws_bytes, int32_t* sorted_ids, int32_t* tile_ranges, int64_t* host_counts,
-             int sync_host, cudaStream_t s) {
-    int grid_x, grid_y, cgrid_x, cgrid_y;
-    cell_grid(width, height, grid_x, grid_y, cgrid_x, cgrid_y);
-    const int n_tiles = grid_x * grid_y, n_cells = cgrid_x * cgrid_y;
-    if (max_pairs >= (int64_t(1) << 30) || max_coarse >= (int64_t(1) << 30)) {
-        set_error("bin_sort: capacity %lld / %lld exceeds 2^30", (long long)max_coarse, (long long)max_pairs);
-        return B200GS_ENOSPACE;
-    }
-    if (n_cells > 65536) {
-        set_error("bin_sort: %d coarse cells exceed 65536 (image too large)", n_cells);
-        return B200GS_ENOSPACE;
-    }
-    if (max_coarse == 0 || n == 0) {   // nothing on screen (or nothing can be stored): empty lists; counts[2] stays 0
-        B200GS_CUDA(cudaMemsetAsync(tile_ranges, 0, sizeof(int32_t) * 2 * (size_t)n_tiles, s));
-        return publish_counts(d_counts, host_counts, sync_host, s);
-    }
-    const WorkspaceA A = carve_a(const_cast<void*>(ws_a), n);
-    const WorkspaceB W = carve_b(ws_b, n, max_coarse, width, height);
-    if (ws_bytes < W.bytes) {
-        set_error("bin_sort: workspace too small (%zu < %zu)", ws_bytes, W.bytes);
-        return B200GS_ENOSPACE;
-    }
-    const uint2* order = A.rec_a;
-    const SplatRec* recs = A.recs;
-    const int64_t* d_visible = d_counts + 3;
-    const int64_t* d_coarse = d_counts + 1;
-
-    // B: coarse entries with their tile masks in depth order; per-cell counts
-    B200GS_CUDA(cudaMemsetAsync(W.cell_hist, 0, W.zero_bytes, s));
-    const int passes = n_cells > sweep::RADIX ? 2 : 1;     // partition passes: one per byte of the cell id
-    CellEntry* emit_dst = passes == 2 ? W.entries : W.entries_in;   // the partitioned entries end in W.entries
-    const int pack = pack_ncells(n, width, height) ? 1 : 0;
-    rank_offsets_kernel<<<(unsigned)W.scan_blocks, 256, 0, s>>>(d_visible, pack, order, recs, W.offsets, W.tickets, W.scan_state);
-    B200GS_LAUNCH_CHECK();
-    static constexpr decltype(&emit_cells_kernel<false>) emit[2] = {emit_cells_kernel<false>, emit_cells_kernel<true>};
-    emit[mode == B200GS_MODE_GSPLAT]<<<(unsigned)W.blocks, 256, 0, s>>>(d_visible, pack, grid_x, grid_y, cgrid_x, cull, max_coarse, order, recs,
-                                                                         W.offsets, emit_dst, n_cells, W.cell_hist);
-    B200GS_LAUNCH_CHECK();
-    cell_table_kernel<<<1, 1024, 0, s>>>(n_cells, W.cell_hist, W.cell_ranges, W.chunk_base, W.chunk_cell, W.digit_hist, n_tiles, W.tile_start);
-    B200GS_LAUNCH_CHECK();
-    // stable partition by cell (the entry carries its cell in .w)
-    CellEntry* src_ent = emit_dst;
-    CellEntry* dst_ent = passes == 2 ? W.entries_in : W.entries;
-    for (int pass = 0; pass < passes; ++pass) {
-        sweep::onesweep_pass_kernel<CellEntry, CELL_IPT><<<(unsigned)W.tiles, sweep::PASS_THREADS, 0, s>>>(
-            src_ent, dst_ent, d_coarse, max_coarse, 8 * pass, W.digit_hist + pass * sweep::RADIX, W.lookback + (size_t)pass * W.tiles * sweep::RADIX,
-            W.tickets + 1 + pass);
-        B200GS_LAUNCH_CHECK();
-        CellEntry* tmp = src_ent; src_ent = dst_ent; dst_ent = tmp;
-    }
-
-    // C: per-chunk tile counts;  D: chunk prefixes, tile starts / ranges / total;  E: ids in place
-    const unsigned chunks = (unsigned)W.max_chunks;
-    chunk_counts_kernel<<<chunks, CHUNK, 0, s>>>(n_cells, cgrid_x, grid_x, grid_y, W.cell_ranges, W.chunk_base, W.chunk_cell, W.entries, W.chunk_cnt,
-                                                 W.tile_start);
-    B200GS_LAUNCH_CHECK();
-    chunk_prefix_kernel<<<(unsigned)n_cells + 1, 1024, 0, s>>>(n_cells, n_tiles, W.chunk_base, W.chunk_cnt, W.chunk_pre, W.tile_start, max_pairs,
-                                                               (int2*)tile_ranges, d_counts);
-    B200GS_LAUNCH_CHECK();
-    scatter_ids_kernel<<<chunks, CHUNK, 0, s>>>(n_cells, cgrid_x, grid_x, grid_y, max_pairs, W.cell_ranges, W.chunk_base, W.chunk_cell, W.entries,
-                                                W.chunk_pre, W.tile_start, sorted_ids);
-    B200GS_LAUNCH_CHECK();
     return publish_counts(d_counts, host_counts, sync_host, s);
 }
 
@@ -1023,10 +956,135 @@ __global__ void __launch_bounds__(256) pack_rows_kernel(int64_t n, const float2*
 
 static size_t pack_scan_state_bytes(int64_t n) { return align_up((size_t)div_up64(n > 0 ? n : 1, 256) * 4 + 64, 256); }
 
-size_t pack_rows_workspace_bytes(int64_t n) { return pack_scan_state_bytes(n) + align_up((size_t)(n > 0 ? n : 1) * 4, 256); }
+static size_t pack_rows_workspace_bytes(int64_t n) { return pack_scan_state_bytes(n) + align_up((size_t)(n > 0 ? n : 1) * 4, 256); }
 
-int pack_rows(int64_t n, const float* xy, const float* depth, const float* conic, const float* comp, const float* opacity,
-              const float* rgb, const int32_t* radii, void* ws, int32_t* row_index, float* rows, int64_t* d_count, cudaStream_t s) {
+}  // namespace b200gs
+
+using namespace b200gs;
+
+extern "C" {
+
+size_t b200gs_bin_count_workspace_bytes(int64_t n) { return n < 0 ? 0 : carve_a(nullptr, n).bytes; }
+
+size_t b200gs_bin_sort_workspace_bytes(int64_t n, int64_t max_coarse, int32_t width, int32_t height) {
+    if (n < 0 || max_coarse < 0 || width <= 0 || height <= 0) return 0;
+    return carve_b(nullptr, n, max_coarse, width, height).bytes;
+}
+
+int b200gs_bin_count(int32_t mode, int32_t width, int32_t height, int64_t n, const float* xy, const float* depth,
+                     const int32_t* radii, const float* cull_conic, const float* cull_opacity, void* workspace, size_t workspace_bytes,
+                     int64_t* d_counts, int64_t* host_counts, int32_t sync_host, void* stream) {
+    B200GS_CHECK_ARG(mode == B200GS_MODE_VANILLA || mode == B200GS_MODE_GSPLAT, "bad mode");
+    B200GS_CHECK_ARG(width > 0 && height > 0 && n >= 0, "bad size");
+    B200GS_CHECK_ARG(workspace && d_counts, "workspace/d_counts must not be NULL");
+    B200GS_CHECK_ARG(n == 0 || (xy && depth && radii), "NULL pointer");
+    B200GS_CHECK_ARG(n < (int64_t(1) << 31), "n >= 2^31");
+    B200GS_CHECK_ARG((cull_conic == nullptr) == (cull_opacity == nullptr), "cull_conic and cull_opacity go together");
+    return bin_count(mode, width, height, n, false, xy, depth, radii, cull_conic, cull_opacity, workspace, workspace_bytes, d_counts,
+                     host_counts, sync_host, (cudaStream_t)stream);
+}
+
+int b200gs_bin_count_rows(int32_t mode, int32_t width, int32_t height, int64_t n, const float* rows, int32_t cull, void* workspace,
+                          size_t workspace_bytes, int64_t* d_counts, int64_t* host_counts, int32_t sync_host, void* stream,
+                          const int64_t* block_counts, int64_t block_rows) {
+    B200GS_CHECK_ARG(mode == B200GS_MODE_VANILLA || mode == B200GS_MODE_GSPLAT, "bad mode");
+    B200GS_CHECK_ARG(width > 0 && height > 0 && n >= 0 && n < (int64_t(1) << 31), "bad size");
+    B200GS_CHECK_ARG(workspace && d_counts && (n == 0 || rows), "NULL pointer");
+    B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(rows) & 15u) == 0, "rows must be 16-byte aligned");
+    return bin_count(mode, width, height, n, true, rows + B200GS_ROW_XY, rows + B200GS_ROW_DEPTH, (const int32_t*)(rows + B200GS_ROW_RADIUS),
+                     rows + B200GS_ROW_CONIC, rows + B200GS_ROW_OPACITY, workspace, workspace_bytes, d_counts, host_counts, sync_host,
+                     (cudaStream_t)stream, block_counts, block_rows);
+}
+
+int b200gs_bin_sort(int32_t mode, int32_t width, int32_t height, int64_t n, int32_t cull, int64_t max_coarse, int64_t max_pairs,
+                    int64_t* d_counts, const void* ws_a, void* ws_b, size_t ws_bytes, int32_t* sorted_ids, int32_t* tile_ranges,
+                    int64_t* host_counts, int32_t sync_host, void* stream) {
+    B200GS_CHECK_ARG(mode == B200GS_MODE_VANILLA || mode == B200GS_MODE_GSPLAT, "bad mode");
+    B200GS_CHECK_ARG(width > 0 && height > 0 && n >= 0 && max_pairs >= 0 && max_coarse >= 0, "bad size");
+    B200GS_CHECK_ARG(d_counts != nullptr, "d_counts must not be NULL");
+    B200GS_CHECK_ARG(ws_a && ws_b && tile_ranges, "workspace/tile_ranges must not be NULL");
+    B200GS_CHECK_ARG(n == 0 || max_coarse == 0 || sorted_ids, "NULL pointer");
+    const cudaStream_t s = (cudaStream_t)stream;
+    int grid_x, grid_y, cgrid_x, cgrid_y;
+    cell_grid(width, height, grid_x, grid_y, cgrid_x, cgrid_y);
+    const int n_tiles = grid_x * grid_y, n_cells = cgrid_x * cgrid_y;
+    if (max_pairs >= (int64_t(1) << 30) || max_coarse >= (int64_t(1) << 30)) {
+        set_error("bin_sort: capacity %lld / %lld exceeds 2^30", (long long)max_coarse, (long long)max_pairs);
+        return B200GS_ENOSPACE;
+    }
+    if (n_cells > 65536) {
+        set_error("bin_sort: %d coarse cells exceed 65536 (image too large)", n_cells);
+        return B200GS_ENOSPACE;
+    }
+    if (max_coarse == 0 || n == 0) {   // nothing on screen (or nothing can be stored): empty lists; counts[2] stays 0
+        B200GS_CUDA(cudaMemsetAsync(tile_ranges, 0, sizeof(int32_t) * 2 * (size_t)n_tiles, s));
+        return publish_counts(d_counts, host_counts, sync_host, s);
+    }
+    const WorkspaceA A = carve_a(const_cast<void*>(ws_a), n);
+    const WorkspaceB W = carve_b(ws_b, n, max_coarse, width, height);
+    if (ws_bytes < W.bytes) {
+        set_error("bin_sort: workspace too small (%zu < %zu)", ws_bytes, W.bytes);
+        return B200GS_ENOSPACE;
+    }
+    const uint2* order = A.rec_a;
+    const SplatRec* recs = A.recs;
+    const int64_t* d_visible = d_counts + 3;
+    const int64_t* d_coarse = d_counts + 1;
+
+    // B: coarse entries with their tile masks in depth order; per-cell counts
+    B200GS_CUDA(cudaMemsetAsync(W.cell_hist, 0, W.zero_bytes, s));
+    const int passes = n_cells > sweep::RADIX ? 2 : 1;     // partition passes: one per byte of the cell id
+    CellEntry* emit_dst = passes == 2 ? W.entries : W.entries_in;   // the partitioned entries end in W.entries
+    const int pack = pack_ncells(n, width, height) ? 1 : 0;
+    rank_offsets_kernel<<<(unsigned)W.scan_blocks, 256, 0, s>>>(d_visible, pack, order, recs, W.offsets, W.tickets, W.scan_state);
+    B200GS_LAUNCH_CHECK();
+    static constexpr decltype(&emit_cells_kernel<false>) emit[2] = {emit_cells_kernel<false>, emit_cells_kernel<true>};
+    emit[mode == B200GS_MODE_GSPLAT]<<<(unsigned)W.blocks, 256, 0, s>>>(d_visible, pack, grid_x, grid_y, cgrid_x, cull, max_coarse, order, recs,
+                                                                         W.offsets, emit_dst, n_cells, W.cell_hist);
+    B200GS_LAUNCH_CHECK();
+    cell_table_kernel<<<1, 1024, 0, s>>>(n_cells, W.cell_hist, W.cell_ranges, W.chunk_base, W.chunk_cell, W.digit_hist, n_tiles, W.tile_start);
+    B200GS_LAUNCH_CHECK();
+    // stable partition by cell (the entry carries its cell in .w)
+    CellEntry* src_ent = emit_dst;
+    CellEntry* dst_ent = passes == 2 ? W.entries_in : W.entries;
+    for (int pass = 0; pass < passes; ++pass) {
+        sweep::onesweep_pass_kernel<CellEntry, CELL_IPT><<<(unsigned)W.tiles, sweep::PASS_THREADS, 0, s>>>(
+            src_ent, dst_ent, d_coarse, max_coarse, 8 * pass, W.digit_hist + pass * sweep::RADIX, W.lookback + (size_t)pass * W.tiles * sweep::RADIX,
+            W.tickets + 1 + pass);
+        B200GS_LAUNCH_CHECK();
+        CellEntry* tmp = src_ent; src_ent = dst_ent; dst_ent = tmp;
+    }
+
+    // C: per-chunk tile counts;  D: chunk prefixes, tile starts / ranges / total;  E: ids in place
+    const unsigned chunks = (unsigned)W.max_chunks;
+    chunk_counts_kernel<<<chunks, CHUNK, 0, s>>>(n_cells, cgrid_x, grid_x, grid_y, W.cell_ranges, W.chunk_base, W.chunk_cell, W.entries, W.chunk_cnt,
+                                                 W.tile_start);
+    B200GS_LAUNCH_CHECK();
+    chunk_prefix_kernel<<<(unsigned)n_cells + 1, 1024, 0, s>>>(n_cells, n_tiles, W.chunk_base, W.chunk_cnt, W.chunk_pre, W.tile_start, max_pairs,
+                                                               (int2*)tile_ranges, d_counts);
+    B200GS_LAUNCH_CHECK();
+    scatter_ids_kernel<<<chunks, CHUNK, 0, s>>>(n_cells, cgrid_x, grid_x, grid_y, max_pairs, W.cell_ranges, W.chunk_base, W.chunk_cell, W.entries,
+                                                W.chunk_pre, W.tile_start, sorted_ids);
+    B200GS_LAUNCH_CHECK();
+    return publish_counts(d_counts, host_counts, sync_host, s);
+}
+
+int b200gs_publish_i64(const int64_t* d_values, int64_t* host_values, int32_t n, void* stream) {
+    B200GS_CHECK_ARG(d_values && host_values && n > 0, "bad argument");
+    return publish_i64(d_values, host_values, n, (cudaStream_t)stream);
+}
+
+// ---- [n,12] row layout (the exchange format of the Gaussian-sharded renderer) -------------------------------------------
+size_t b200gs_pack_rows_workspace_bytes(int64_t n) { return n < 0 ? 0 : pack_rows_workspace_bytes(n); }
+
+int b200gs_pack_rows(int64_t n, const float* xy, const float* depth, const float* conic, const float* comp, const float* opacity,
+                     const float* rgb, const int32_t* radii, void* ws, size_t workspace_bytes, int32_t* row_index, float* rows,
+                     int64_t* d_count, void* stream) {
+    B200GS_CHECK_ARG(n >= 0 && n < (int64_t(1) << 31), "bad n");
+    B200GS_CHECK_ARG(d_count != nullptr, "d_count must not be NULL");
+    B200GS_CHECK_ARG(n == 0 || (xy && depth && conic && opacity && rgb && radii && ws && row_index && rows), "NULL pointer");
+    B200GS_CHECK_ARG(n == 0 || workspace_bytes >= pack_rows_workspace_bytes(n), "workspace too small");
+    const cudaStream_t s = (cudaStream_t)stream;
     if (n == 0) {
         B200GS_CUDA(cudaMemsetAsync(d_count, 0, sizeof(int64_t), s));
         return B200GS_OK;
@@ -1044,4 +1102,4 @@ int pack_rows(int64_t n, const float* xy, const float* depth, const float* conic
     return B200GS_OK;
 }
 
-}  // namespace b200gs
+}  // extern "C"

@@ -1123,10 +1123,12 @@ int feat_bwd_chunk(dim3 grid, int gx, int width, int height, const int32_t* rang
 
 }  // namespace
 
-int launch_blend_fwd(int mode, int width, int height, int channels, const int32_t* ranges, const int32_t* ids, bool rows, const float* xy,
-                     const float* conic, const float* opacity, const float* colors, const float* bg, float* image,
-                     int64_t pix_stride, int64_t ch_stride, float* final_T, int32_t* n_contrib, float* alpha, cudaStream_t s,
-                     uint8_t* hit_any) {
+// The K6 / K7 launch path of the array and the row entry points.  rows: xy, conic, opacity and colors (and the gradient outputs) are
+// columns of 16-byte aligned [n,12] row buffers, channels == 3
+static int launch_blend_fwd(int mode, int width, int height, int channels, const int32_t* ranges, const int32_t* ids, bool rows,
+                            const float* xy, const float* conic, const float* opacity, const float* colors, const float* bg, float* image,
+                            int64_t pix_stride, int64_t ch_stride, float* final_T, int32_t* n_contrib, float* alpha, cudaStream_t s,
+                            uint8_t* hit_any = nullptr) {
     static constexpr decltype(&fwd_dispatch<1, false>) by_channels[4][2] = {
         {fwd_dispatch<1, false>, fwd_dispatch<1, true>}, {fwd_dispatch<2, false>, fwd_dispatch<2, true>},
         {fwd_dispatch<3, false>, fwd_dispatch<3, true>}, {fwd_dispatch<4, false>, fwd_dispatch<4, true>}};
@@ -1138,11 +1140,11 @@ int launch_blend_fwd(int mode, int width, int height, int channels, const int32_
                                                                   pix_stride, ch_stride, final_T, n_contrib, alpha, hit_any, s);
 }
 
-int launch_blend_bwd(int mode, int width, int height, int channels, const int32_t* ranges, const int32_t* ids, bool rows, const float* xy,
-                     const float* conic, const float* opacity, const float* colors, const float* bg, const float* final_T,
-                     const int32_t* n_contrib, const float* v_image, int64_t pix_stride, int64_t ch_stride, const float* v_alpha,
-                     float sx, float sy, float* v_xy, float* v_conic, float* v_opacity, float* v_colors, float* v_xy_abs,
-                     cudaStream_t s) {
+static int launch_blend_bwd(int mode, int width, int height, int channels, const int32_t* ranges, const int32_t* ids, bool rows,
+                            const float* xy, const float* conic, const float* opacity, const float* colors, const float* bg,
+                            const float* final_T, const int32_t* n_contrib, const float* v_image, int64_t pix_stride, int64_t ch_stride,
+                            const float* v_alpha, float sx, float sy, float* v_xy, float* v_conic, float* v_opacity, float* v_colors,
+                            float* v_xy_abs, cudaStream_t s) {
     static constexpr decltype(&bwd_dispatch<1, false>) by_channels[4][2] = {
         {bwd_dispatch<1, false>, bwd_dispatch<1, true>}, {bwd_dispatch<2, false>, bwd_dispatch<2, true>},
         {bwd_dispatch<3, false>, bwd_dispatch<3, true>}, {bwd_dispatch<4, false>, bwd_dispatch<4, true>}};
@@ -1155,11 +1157,72 @@ int launch_blend_bwd(int mode, int width, int height, int channels, const int32_
                                                                   v_opacity, v_colors, v_xy_abs, s);
 }
 
-// Chunks of 32 channels over the same binning; a chunk of cw channels runs the smallest instantiation >= cw.  Only chunk 0 writes
-// final_T / n_contrib / alpha (every chunk computes the same ones).
-int launch_blend_feat_fwd(int width, int height, int channels, const int32_t* ranges, const int32_t* ids, const float* xy, const float* conic,
-                          const float* opacity, const float* features, const float* bg, float* image, float* final_T, int32_t* n_contrib,
-                          float* alpha, cudaStream_t s) {
+}  // namespace b200gs
+
+using namespace b200gs;
+
+extern "C" {
+
+int b200gs_blend_fwd(int32_t mode, int32_t width, int32_t height, int32_t channels, const int32_t* tile_ranges,
+                     const int32_t* sorted_ids, const float* xy, const float* conic, const float* opacity,
+                     const float* colors, const float* bg, float* image, int64_t pix_stride, int64_t ch_stride,
+                     float* final_T, int32_t* n_contrib, float* alpha, uint8_t* hit_any, void* stream) {
+    B200GS_CHECK_ARG(mode == B200GS_MODE_VANILLA || mode == B200GS_MODE_GSPLAT, "bad mode");
+    B200GS_CHECK_ARG(width > 0 && height > 0, "bad size");
+    B200GS_CHECK_ARG(tile_ranges && image && final_T && n_contrib, "NULL output/range pointer");
+    return launch_blend_fwd(mode, width, height, channels, tile_ranges, sorted_ids, false, xy, conic, opacity, colors, bg, image,
+                            pix_stride, ch_stride, final_T, n_contrib, alpha, (cudaStream_t)stream, hit_any);
+}
+
+int b200gs_blend_bwd(int32_t mode, int32_t width, int32_t height, int32_t channels, const int32_t* tile_ranges,
+                     const int32_t* sorted_ids, const float* xy, const float* conic, const float* opacity,
+                     const float* colors, const float* bg, const float* final_T, const int32_t* n_contrib,
+                     const float* v_image, int64_t pix_stride, int64_t ch_stride, const float* v_alpha,
+                     float xy_scale_x, float xy_scale_y, float* v_xy, float* v_conic, float* v_opacity,
+                     float* v_colors, float* v_xy_abs, void* stream) {
+    B200GS_CHECK_ARG(mode == B200GS_MODE_VANILLA || mode == B200GS_MODE_GSPLAT, "bad mode");
+    B200GS_CHECK_ARG(width > 0 && height > 0, "bad size");
+    B200GS_CHECK_ARG(tile_ranges && final_T && n_contrib && v_image, "NULL input pointer");
+    B200GS_CHECK_ARG(v_xy && v_conic && v_opacity && v_colors, "NULL output pointer");
+    return launch_blend_bwd(mode, width, height, channels, tile_ranges, sorted_ids, false, xy, conic, opacity, colors, bg, final_T,
+                            n_contrib, v_image, pix_stride, ch_stride, v_alpha, xy_scale_x, xy_scale_y, v_xy, v_conic,
+                            v_opacity, v_colors, v_xy_abs, (cudaStream_t)stream);
+}
+
+int b200gs_blend_fwd_rows(int32_t mode, int32_t width, int32_t height, const int32_t* tile_ranges, const int32_t* sorted_ids,
+                          const float* rows, const float* bg, float* image, int64_t pix_stride, int64_t ch_stride, float* final_T,
+                          int32_t* n_contrib, float* alpha, void* stream) {
+    B200GS_CHECK_ARG(mode == B200GS_MODE_VANILLA || mode == B200GS_MODE_GSPLAT, "bad mode");
+    B200GS_CHECK_ARG(width > 0 && height > 0 && tile_ranges && image && final_T && n_contrib, "bad argument");
+    B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(rows) & 15u) == 0, "rows must be 16-byte aligned");
+    return launch_blend_fwd(mode, width, height, 3, tile_ranges, sorted_ids, true, rows + B200GS_ROW_XY,
+                            rows + B200GS_ROW_CONIC, rows + B200GS_ROW_OPACITY, rows + B200GS_ROW_RGB, bg, image, pix_stride,
+                            ch_stride, final_T, n_contrib, alpha, (cudaStream_t)stream);
+}
+
+int b200gs_blend_bwd_rows(int32_t mode, int32_t width, int32_t height, const int32_t* tile_ranges, const int32_t* sorted_ids,
+                          const float* rows, const float* bg, const float* final_T, const int32_t* n_contrib, const float* v_image,
+                          int64_t pix_stride, int64_t ch_stride, const float* v_alpha, float grad_scale_x, float grad_scale_y,
+                          float* v_rows, void* stream) {
+    B200GS_CHECK_ARG(mode == B200GS_MODE_VANILLA || mode == B200GS_MODE_GSPLAT, "bad mode");
+    B200GS_CHECK_ARG(width > 0 && height > 0 && tile_ranges && final_T && n_contrib && v_image && v_rows, "bad argument");
+    B200GS_CHECK_ARG(((reinterpret_cast<uintptr_t>(rows) | reinterpret_cast<uintptr_t>(v_rows)) & 15u) == 0, "rows and v_rows must be 16-byte aligned");
+    return launch_blend_bwd(mode, width, height, 3, tile_ranges, sorted_ids, true, rows + B200GS_ROW_XY,
+                            rows + B200GS_ROW_CONIC, rows + B200GS_ROW_OPACITY, rows + B200GS_ROW_RGB, bg, final_T, n_contrib, v_image,
+                            pix_stride, ch_stride, v_alpha, grad_scale_x, grad_scale_y, v_rows + B200GS_ROW_XY, v_rows + B200GS_ROW_CONIC,
+                            v_rows + B200GS_ROW_OPACITY, v_rows + B200GS_ROW_RGB, nullptr, (cudaStream_t)stream);
+}
+
+// gsplat mode, any channel count >= 1: [n, channels] features, [H, W, channels] image.  Chunks of 32 channels over the same binning;
+// a chunk of cw channels runs the smallest instantiation >= cw.  Only chunk 0 writes final_T / n_contrib / alpha (every chunk
+// computes the same ones).
+int b200gs_blend_feat_fwd(int32_t width, int32_t height, int32_t channels, const int32_t* ranges, const int32_t* ids, const float* xy,
+                          const float* conic, const float* opacity, const float* features, const float* bg, float* image, float* final_T,
+                          int32_t* n_contrib, float* alpha, void* stream) {
+    B200GS_CHECK_ARG(width > 0 && height > 0, "bad size");
+    B200GS_CHECK_ARG(channels >= 1, "channels must be >= 1");
+    B200GS_CHECK_ARG(ranges && ids && xy && conic && opacity && features, "NULL input pointer");
+    B200GS_CHECK_ARG(image && final_T && n_contrib, "NULL output pointer");
     const int gx = div_up(width, TILE);
     const dim3 grid(gx * div_up(height, TILE));
     for (int c0 = 0; c0 < channels; c0 += 32) {
@@ -1167,7 +1230,7 @@ int launch_blend_feat_fwd(int width, int height, int channels, const int32_t* ra
         const bool first = c0 == 0;
         const auto by_width = cw <= 8 ? feat_fwd_chunk<8> : cw <= 16 ? feat_fwd_chunk<16> : feat_fwd_chunk<32>;
         const int rc = by_width(grid, gx, width, height, ranges, ids, xy, conic, opacity, features, channels, c0, cw, bg, image,
-                                first ? final_T : nullptr, first ? n_contrib : nullptr, first ? alpha : nullptr, s);
+                                first ? final_T : nullptr, first ? n_contrib : nullptr, first ? alpha : nullptr, (cudaStream_t)stream);
         if (rc) return rc;
     }
     return B200GS_OK;
@@ -1176,10 +1239,17 @@ int launch_blend_feat_fwd(int width, int height, int channels, const int32_t* ra
 // Only chunk 0 takes the alpha cotangent: the geometry gradients are linear in the per-channel terms, so the chunks' sum is the
 // D-channel gradient.  v_xy == NULL selects the features-only kernels.  absgrad (v_xy_abs) is each chunk's |.| summed over chunks:
 // exact for D <= 32, an upper bound of the all-channel value beyond.
-int launch_blend_feat_bwd(int width, int height, int channels, const int32_t* ranges, const int32_t* ids, const float* xy, const float* conic,
-                          const float* opacity, const float* features, const float* bg, const float* final_T, const int32_t* n_contrib,
-                          const float* v_image, const float* v_alpha, float* v_features, float* v_xy, float* v_conic, float* v_opacity,
-                          float* v_xy_abs, cudaStream_t s) {
+int b200gs_blend_feat_bwd(int32_t width, int32_t height, int32_t channels, const int32_t* ranges, const int32_t* ids, const float* xy,
+                          const float* conic, const float* opacity, const float* features, const float* bg, const float* final_T,
+                          const int32_t* n_contrib, const float* v_image, const float* v_alpha, float* v_features, float* v_xy,
+                          float* v_conic, float* v_opacity, float* v_xy_abs, void* stream) {
+    B200GS_CHECK_ARG(width > 0 && height > 0, "bad size");
+    B200GS_CHECK_ARG(channels >= 1, "channels must be >= 1");
+    B200GS_CHECK_ARG(ranges && ids && xy && conic && opacity && features, "NULL input pointer");
+    B200GS_CHECK_ARG(final_T && n_contrib && v_image && v_features, "NULL input/output pointer");
+    B200GS_CHECK_ARG((v_xy == nullptr) == (v_conic == nullptr) && (v_xy == nullptr) == (v_opacity == nullptr),
+                     "v_xy, v_conic and v_opacity are all given or all NULL");
+    B200GS_CHECK_ARG(v_xy_abs == nullptr || v_xy != nullptr, "v_xy_abs needs the geometry gradients");
     const int gx = div_up(width, TILE);
     const dim3 grid(gx * div_up(height, TILE));
     static constexpr decltype(&feat_bwd_chunk<8, false, false>) by_width[3][3] = {
@@ -1192,10 +1262,10 @@ int launch_blend_feat_bwd(int width, int height, int channels, const int32_t* ra
         const int rc = by_width[cw <= 8 ? 0 : cw <= 16 ? 1 : 2][variant](grid, gx, width, height, ranges, ids, xy, conic, opacity, features,
                                                                           channels, c0, cw, bg, final_T, n_contrib, v_image,
                                                                           c0 == 0 ? v_alpha : nullptr, v_features, v_xy, v_conic, v_opacity,
-                                                                          v_xy_abs, s);
+                                                                          v_xy_abs, (cudaStream_t)stream);
         if (rc) return rc;
     }
     return B200GS_OK;
 }
 
-}  // namespace b200gs
+}  // extern "C"

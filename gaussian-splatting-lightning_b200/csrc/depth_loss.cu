@@ -279,7 +279,10 @@ DArgs make_args(int height, int width, const uint8_t* mask, int64_t msy, int64_t
 int stat_blocks(int64_t n) { return int(div_up64(n, STAT_PIXELS) < STAT_MAX_BLOCKS ? div_up64(n, STAT_PIXELS) : STAT_MAX_BLOCKS); }
 int64_t tile_blocks(int height, int width) { return int64_t(div_up(width, LT)) * div_up(height, LT); }
 
-}  // namespace
+// the grid is (ceil(W/LT), ceil(H/LT)): ceil(H/LT) is at most 65535
+bool depth_size_ok(int32_t height, int32_t width) {
+    return height >= 1 && width >= 1 && height <= 65535 * LT && int64_t(height) * width <= INT32_MAX;
+}
 
 size_t depth_loss_workspace_bytes(int height, int width, int loss_type) {
     const int64_t n = int64_t(height) * width;
@@ -288,8 +291,43 @@ size_t depth_loss_workspace_bytes(int height, int width, int loss_type) {
     return size_t(floats) * sizeof(float);
 }
 
-int launch_depth_loss_fwd(int height, int width, const float* pred, const float* gt, const uint8_t* mask, int64_t msy, int64_t msx,
-                          int loss_type, int norm, float median, float w, float* ws, float* loss, float* stats, cudaStream_t st) {
+// pred, gt [H,W] contiguous; mask NULL or uint8 read at mask[msy y + msx x]; loss_type 0 l1, 1 l2, 2 l1+ssim; norm 0 none, 1 min-max,
+// 2 median, 3 mean of gt.  The backward reads the workspace the forward wrote.  Shared by the forward and the backward; returns the
+// error code, or 0 when the arguments are valid
+int check_depth_loss(const char* fn, int32_t height, int32_t width, const float* pred, const float* gt, const uint8_t* mask, int64_t msy,
+                     int64_t msx, int32_t loss_type, int32_t norm, const void* workspace, size_t workspace_bytes) {
+    if (height < 1 || width < 1) return fail(fn, "image size must be >= 1");
+    if (!depth_size_ok(height, width)) return fail(fn, "image too large");
+    if (loss_type < 0 || loss_type > 2) return fail(fn, "loss_type must be 0 (l1), 1 (l2) or 2 (l1+ssim)");
+    if (norm < 0 || norm > 3) return fail(fn, "norm must be 0 (none), 1 (min-max), 2 (median) or 3 (mean)");
+    if (loss_type == 2 && (height < 11 || width < 11)) return fail(fn, "l1+ssim needs an image of at least 11x11");
+    if (loss_type == 2 && mask) return fail(fn, "l1+ssim takes no mask");
+    if (mask && (msy < 0 || msx < 0)) return fail(fn, "negative mask stride");
+    if (!(pred && gt && workspace)) return fail(fn, "NULL pointer");
+    if (workspace_bytes < depth_loss_workspace_bytes(height, width, loss_type)) return workspace_too_small(fn);
+    return 0;
+}
+
+}  // namespace
+
+}  // namespace b200gs
+
+using namespace b200gs;
+
+extern "C" {
+
+size_t b200gs_depth_loss_workspace_bytes(int32_t height, int32_t width, int32_t loss_type) {
+    if (!depth_size_ok(height, width) || loss_type < 0 || loss_type > 2) return 0;
+    return depth_loss_workspace_bytes(height, width, loss_type);
+}
+
+int b200gs_depth_loss_fwd(int32_t height, int32_t width, const float* pred, const float* gt, const uint8_t* mask, int64_t msy, int64_t msx,
+                          int32_t loss_type, int32_t norm, float median, float w, void* workspace, size_t workspace_bytes, float* loss,
+                          float* stats, void* stream) {
+    if (int rc = check_depth_loss(__func__, height, width, pred, gt, mask, msy, msx, loss_type, norm, workspace, workspace_bytes)) return rc;
+    B200GS_CHECK_ARG(loss && stats, "NULL pointer");
+    const cudaStream_t st = (cudaStream_t)stream;
+    float* ws = static_cast<float*>(workspace);
     const DArgs g = make_args(height, width, mask, msy, msx, loss_type, norm, median, w);
     const int64_t n = int64_t(height) * width;
     // l1 and l2 without min-max or mean normalisation use no statistic: one CTA writes an empty partial
@@ -311,17 +349,20 @@ int launch_depth_loss_fwd(int height, int width, const float* pred, const float*
     return B200GS_OK;
 }
 
-int launch_depth_loss_bwd(int height, int width, const float* pred, const float* gt, const uint8_t* mask, int64_t msy, int64_t msx,
-                          int loss_type, int norm, float median, float w, const float* ws, const float* v_loss, float* v_pred,
-                          cudaStream_t st) {
+int b200gs_depth_loss_bwd(int32_t height, int32_t width, const float* pred, const float* gt, const uint8_t* mask, int64_t msy, int64_t msx,
+                          int32_t loss_type, int32_t norm, float median, float w, const void* workspace, size_t workspace_bytes,
+                          const float* v_loss, float* v_pred, void* stream) {
+    if (int rc = check_depth_loss(__func__, height, width, pred, gt, mask, msy, msx, loss_type, norm, workspace, workspace_bytes)) return rc;
+    B200GS_CHECK_ARG(v_pred, "NULL pointer");
+    const float* ws = static_cast<const float*>(workspace);
     const DArgs g = make_args(height, width, mask, msy, msx, loss_type, norm, median, w);
     const int64_t n = int64_t(height) * width;
     const float* maps = ws + HEAD + int64_t(stat_blocks(n)) * STAT + tile_blocks(height, width) * PART;
     const dim3 grid(div_up(width, LT), div_up(height, LT));
-    if (loss_type == 2) depth_bwd_kernel<true><<<grid, LT * LT, 0, st>>>(g, pred, gt, mask, ws, maps, v_loss, v_pred);
-    else depth_bwd_kernel<false><<<grid, LT * LT, 0, st>>>(g, pred, gt, mask, ws, maps, v_loss, v_pred);
+    if (loss_type == 2) depth_bwd_kernel<true><<<grid, LT * LT, 0, (cudaStream_t)stream>>>(g, pred, gt, mask, ws, maps, v_loss, v_pred);
+    else depth_bwd_kernel<false><<<grid, LT * LT, 0, (cudaStream_t)stream>>>(g, pred, gt, mask, ws, maps, v_loss, v_pred);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-}  // namespace b200gs
+}  // extern "C"

@@ -218,7 +218,11 @@ ExpoArgs make_args(int height, int width, int64_t sc, int64_t sy, int64_t sx, in
     return g;
 }
 
-}  // namespace
+// the grid is (ceil(W/BX), ceil(H/BY)): ceil(H/BY) is at most 65535
+bool exposure_size_ok(int32_t height, int32_t width, int32_t shade_size) {
+    return height >= 1 && width >= 1 && height <= 65535 * BY && int64_t(height) * width <= INT32_MAX && shade_size >= 0 &&
+           shade_size <= 4096;
+}
 
 size_t exposure_workspace_bytes(int height, int width, int shade_size, bool backward) {
     int64_t floats = HEAD + int64_t(shade_size) * shade_size;
@@ -226,11 +230,48 @@ size_t exposure_workspace_bytes(int height, int width, int shade_size, bool back
     return size_t(floats) * sizeof(float);
 }
 
-int launch_exposure_fwd(int height, int width, const float* render, int64_t sc, int64_t sy, int64_t sx, int n_app, int n_params,
-                        const float* params, const int64_t* id_dev, int64_t id_host, int s, const float* shade, float max_gray,
-                        float max_gamma, float* ws, float* out, cudaStream_t st) {
-    const ExpoArgs g = make_args(height, width, sc, sy, sx, n_params, s, max_gray, max_gamma);
-    exposure_prep_kernel<<<1, PREP_THREADS, 0, st>>>(n_app, n_params, params, id_dev, id_host, s, shade, ws);
+// render / out / v_out / v_render [3,H,W] through the element strides (sc, sy, sx); params [n_appearances, n_params] (n_params 4 or
+// 7: with bias); the id read from appearance_id when not NULL, else host_appearance_id; shade [s, s] (s = 0: none).  Shared by the
+// forward and the backward; returns the error code, or 0 when the arguments are valid
+int check_exposure(const char* fn, int32_t channels, int32_t height, int32_t width, const float* render, int64_t sc, int64_t sy, int64_t sx,
+                   int32_t n_appearances, int32_t n_params, const float* exposure_params, int32_t shade_size, const float* shade,
+                   const void* workspace, size_t workspace_bytes, bool backward, const void* out) {
+    if (channels != 3) return fail(fn, "channels must be 3");
+    if (height < 1 || width < 1) return fail(fn, "image size must be >= 1");
+    if (shade_size < 0) return fail(fn, "negative shade_size");
+    if (!exposure_size_ok(height, width, shade_size)) return fail(fn, "image or shade map too large");
+    if (sc < 0 || sy < 0 || sx < 0) return fail(fn, "negative stride");
+    if (n_appearances < 1) return fail(fn, "n_appearances must be >= 1");
+    if (n_params != 4 && n_params != 7) return fail(fn, "n_params must be 4 (no bias) or 7 (with bias)");
+    if (!(render && exposure_params && workspace && out) || (shade_size > 0 && !shade)) return fail(fn, "NULL pointer");
+    if (workspace_bytes < exposure_workspace_bytes(height, width, shade_size, backward)) return workspace_too_small(fn);
+    return 0;
+}
+
+}  // namespace
+
+}  // namespace b200gs
+
+using namespace b200gs;
+
+extern "C" {
+
+size_t b200gs_exposure_workspace_bytes(int32_t height, int32_t width, int32_t shade_size, int32_t backward) {
+    if (!exposure_size_ok(height, width, shade_size)) return 0;
+    return exposure_workspace_bytes(height, width, shade_size, backward != 0);
+}
+
+int b200gs_exposure_fwd(int32_t channels, int32_t height, int32_t width, const float* render, int64_t sc, int64_t sy, int64_t sx,
+                        int32_t n_appearances, int32_t n_params, const float* exposure_params, const int64_t* appearance_id,
+                        int64_t host_appearance_id, int32_t s, const float* shade, float max_gray_scale, float max_gamma,
+                        void* workspace, size_t workspace_bytes, float* out, void* stream) {
+    if (int rc = check_exposure(__func__, channels, height, width, render, sc, sy, sx, n_appearances, n_params, exposure_params, s, shade,
+                                workspace, workspace_bytes, false, out))
+        return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    float* ws = static_cast<float*>(workspace);
+    const ExpoArgs g = make_args(height, width, sc, sy, sx, n_params, s, max_gray_scale, max_gamma);
+    exposure_prep_kernel<<<1, PREP_THREADS, 0, st>>>(n_appearances, n_params, exposure_params, appearance_id, host_appearance_id, s, shade, ws);
     B200GS_LAUNCH_CHECK();
     const dim3 grid(div_up(width, BX), div_up(height, BY)), block(BX, BY);
     if (s > 0) exposure_fwd_kernel<true><<<grid, block, 0, st>>>(g, render, ws, out);
@@ -239,12 +280,19 @@ int launch_exposure_fwd(int height, int width, const float* render, int64_t sc, 
     return B200GS_OK;
 }
 
-int launch_exposure_bwd(int height, int width, const float* render, int64_t sc, int64_t sy, int64_t sx, int n_app, int n_params,
-                        const float* params, const int64_t* id_dev, int64_t id_host, int s, const float* shade, float max_gray,
-                        float max_gamma, float* ws, const float* v_out, float* v_render, float* v_params, float* v_shade,
-                        cudaStream_t st) {
-    const ExpoArgs g = make_args(height, width, sc, sy, sx, n_params, s, max_gray, max_gamma);
-    exposure_prep_kernel<<<1, PREP_THREADS, 0, st>>>(n_app, n_params, params, id_dev, id_host, s, shade, ws);
+int b200gs_exposure_bwd(int32_t channels, int32_t height, int32_t width, const float* render, int64_t sc, int64_t sy, int64_t sx,
+                        int32_t n_appearances, int32_t n_params, const float* exposure_params, const int64_t* appearance_id,
+                        int64_t host_appearance_id, int32_t s, const float* shade, float max_gray_scale, float max_gamma,
+                        void* workspace, size_t workspace_bytes, const float* v_out, float* v_render, float* v_params, float* v_shade,
+                        void* stream) {
+    if (int rc = check_exposure(__func__, channels, height, width, render, sc, sy, sx, n_appearances, n_params, exposure_params, s, shade,
+                                workspace, workspace_bytes, true, v_out))
+        return rc;
+    B200GS_CHECK_ARG(v_render && v_params && (s == 0 || v_shade), "NULL pointer");
+    const cudaStream_t st = (cudaStream_t)stream;
+    float* ws = static_cast<float*>(workspace);
+    const ExpoArgs g = make_args(height, width, sc, sy, sx, n_params, s, max_gray_scale, max_gamma);
+    exposure_prep_kernel<<<1, PREP_THREADS, 0, st>>>(n_appearances, n_params, exposure_params, appearance_id, host_appearance_id, s, shade, ws);
     B200GS_LAUNCH_CHECK();
     const int64_t n_blocks = pixel_blocks(height, width);
     float* partials = ws + HEAD + s * s;
@@ -253,10 +301,10 @@ int launch_exposure_bwd(int height, int width, const float* render, int64_t sc, 
     if (s > 0) exposure_bwd_kernel<true><<<grid, block, 0, st>>>(g, render, v_out, ws, v_render, partials, v_m);
     else exposure_bwd_kernel<false><<<grid, block, 0, st>>>(g, render, v_out, ws, v_render, partials, v_m);
     B200GS_LAUNCH_CHECK();
-    exposure_reduce_kernel<<<1 + div_up(s * s, RED_THREADS / 32), RED_THREADS, 0, st>>>(g, int(n_blocks), n_app, ws, partials, v_m, shade,
-                                                                                         v_params, v_shade);
+    exposure_reduce_kernel<<<1 + div_up(s * s, RED_THREADS / 32), RED_THREADS, 0, st>>>(g, int(n_blocks), n_appearances, ws, partials, v_m,
+                                                                                         shade, v_params, v_shade);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-}  // namespace b200gs
+}  // extern "C"

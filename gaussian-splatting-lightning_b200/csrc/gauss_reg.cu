@@ -253,12 +253,44 @@ RArgs make_args(int64_t n, bool has_opac, bool has_scales, bool stats, int flags
 
 int reg_blocks(int64_t n) { return int(div_up64(n, SPAN) < MAX_BLOCKS ? div_up64(n, SPAN) : MAX_BLOCKS); }
 
-}  // namespace
+bool gaussian_reg_size_ok(int64_t n) { return n >= 1 && n <= INT32_MAX; }
 
 size_t gaussian_reg_workspace_bytes(int64_t n) { return size_t(HEAD + int64_t(reg_blocks(n)) * PART) * sizeof(float); }
 
-int launch_gaussian_reg_fwd(int64_t n, const float* opac, const float* scales, int flags, float w_o, float w_s, float max_scale,
-                            float max_ratio, float lam, float lam_r, float* ws, float* terms, float* stats, cudaStream_t st) {
+// opacities [n,1] and scales [n,3] contiguous, either NULL when no term reads it; flags of b200gs.h.  The backward reads the
+// coefficients its forward wrote to the workspace.  Shared by the forward and the backward; returns the error code, or 0 when the
+// arguments are valid
+int check_gaussian_reg(const char* fn, int64_t n, const float* opacities, const float* scales, int32_t flags, bool stats,
+                       const void* workspace, size_t workspace_bytes) {
+    constexpr int32_t all = B200GS_GREG_RAW | B200GS_GREG_OPACITY | B200GS_GREG_SCALE | B200GS_GREG_OVER_SCALE | B200GS_GREG_OVER_RATIO;
+    if (n < 1) return fail(fn, "n must be >= 1");
+    if (!gaussian_reg_size_ok(n)) return fail(fn, "n too large (> 2^31 - 1)");
+    if (flags & ~all) return fail(fn, "unknown flags");
+    if ((flags & B200GS_GREG_OPACITY) && !opacities) return fail(fn, "NULL pointer: opacities");
+    if (((flags & (B200GS_GREG_SCALE | B200GS_GREG_OVER_SCALE | B200GS_GREG_OVER_RATIO)) || stats) && !scales)
+        return fail(fn, "NULL pointer: scales");
+    if (!workspace) return fail(fn, "NULL pointer: workspace");
+    if (workspace_bytes < gaussian_reg_workspace_bytes(n)) return workspace_too_small(fn);
+    return 0;
+}
+
+}  // namespace
+
+}  // namespace b200gs
+
+using namespace b200gs;
+
+extern "C" {
+
+size_t b200gs_gaussian_reg_workspace_bytes(int64_t n) { return gaussian_reg_size_ok(n) ? gaussian_reg_workspace_bytes(n) : 0; }
+
+int b200gs_gaussian_reg_fwd(int64_t n, const float* opac, const float* scales, int32_t flags, float w_o, float w_s, float max_scale,
+                            float max_ratio, float lam, float lam_r, void* workspace, size_t workspace_bytes, float* terms, float* stats,
+                            void* stream) {
+    if (int rc = check_gaussian_reg(__func__, n, opac, scales, flags, stats != nullptr, workspace, workspace_bytes)) return rc;
+    B200GS_CHECK_ARG(terms, "NULL pointer: terms");
+    const cudaStream_t st = (cudaStream_t)stream;
+    float* ws = static_cast<float*>(workspace);
     const RArgs g = make_args(n, opac != nullptr, scales != nullptr, stats != nullptr, flags, w_o, w_s, max_scale, max_ratio, lam, lam_r);
     const int blocks = reg_blocks(n);
     reg_partials_kernel<<<blocks, THREADS, 0, st>>>(g, opac, scales, ws + HEAD);
@@ -268,14 +300,20 @@ int launch_gaussian_reg_fwd(int64_t n, const float* opac, const float* scales, i
     return B200GS_OK;
 }
 
-int launch_gaussian_reg_bwd(int64_t n, const float* opac, const float* scales, int flags, float w_o, float w_s, float max_scale,
-                            float max_ratio, float lam, float lam_r, const float* ws, const float* v_terms, float* v_opac,
-                            float* v_scales, cudaStream_t st) {
+int b200gs_gaussian_reg_bwd(int64_t n, const float* opac, const float* scales, int32_t flags, float w_o, float w_s, float max_scale,
+                            float max_ratio, float lam, float lam_r, const void* workspace, size_t workspace_bytes, const float* v_terms,
+                            float* v_opac, float* v_scales, void* stream) {
+    if (int rc = check_gaussian_reg(__func__, n, opac, scales, flags, false, workspace, workspace_bytes)) return rc;
+    B200GS_CHECK_ARG(v_terms, "NULL pointer: v_terms");
+    B200GS_CHECK_ARG(!opac || v_opac, "NULL pointer: v_opacities");
+    B200GS_CHECK_ARG(!scales || v_scales, "NULL pointer: v_scales");
     // the backward needs the sort only for the ratio term
     const RArgs g = make_args(n, opac != nullptr, scales != nullptr, false, flags, w_o, w_s, max_scale, max_ratio, lam, lam_r);
-    reg_bwd_kernel<<<int(div_up64(n, THREADS)), THREADS, 0, st>>>(g, opac, scales, ws, v_terms, v_opac, v_scales);
+    reg_bwd_kernel<<<int(div_up64(n, THREADS)), THREADS, 0, (cudaStream_t)stream>>>(g, opac, scales, static_cast<const float*>(workspace),
+                                                                                    v_terms, opac ? v_opac : nullptr,
+                                                                                    scales ? v_scales : nullptr);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-}  // namespace b200gs
+}  // extern "C"

@@ -156,31 +156,55 @@ __global__ void __launch_bounds__(GLOSSY_BWD_THREADS) glossy_bwd_kernel(int deg,
         store_grad_rows<MC, 3>(s_warp, lane, i, n, v_shs, sh_stride * 3, 0, ncoef, bs, g);
 }
 
+// shared by the Glossy-Gaussian entry points: the degree, the opacity rest width and, when the colour is on, its layout
+int check_glossy(const char* fn, int32_t degree, int64_t n, const float* means, const float* campos, int32_t op_k_rest, bool colour,
+                 int32_t sh_stride, int32_t sh_split) {
+    if (degree < 0 || degree > 4) return fail(fn, "degree must be 0..4");
+    if (n < 0) return fail(fn, "n < 0");
+    if (op_k_rest < 0 || op_k_rest + 1 < (degree + 1) * (degree + 1)) return fail(fn, "1 + op_k_rest < (degree+1)^2");
+    if (n > 0 && !(means && campos)) return fail(fn, "NULL pointer");
+    if (colour && sh_split != 0 && sh_split != 1) return fail(fn, "sh_split must be 0 or 1");
+    if (colour && sh_stride < (degree + 1) * (degree + 1)) return fail(fn, "sh_stride < (degree+1)^2");
+    return 0;
+}
+
 }  // namespace
 
+}  // namespace b200gs
+
+using namespace b200gs;
+
+extern "C" {
+
 // The instantiation is picked here, by the degree (MC = 25 iff degree 4) and the colour layout.
-int launch_glossy_sh_fwd(int degree, int64_t n, const float* means, const float* campos, const float* op_dc, const float* op_rest,
-                         int op_k_rest, const float* shs, const float* shs_rest, int sh_stride, bool split, const uint8_t* mask,
-                         float* opacity, float* rgb, uint8_t* clamped, cudaStream_t s) {
+int b200gs_glossy_sh_fwd(int32_t degree, int64_t n, const float* means, const float* campos, const float* op_dc, const float* op_rest,
+                         int32_t op_k_rest, const float* shs, const float* shs_rest, int32_t sh_stride, int32_t sh_split,
+                         const uint8_t* mask, float* opacity, float* rgb, uint8_t* clamped, void* stream) {
+    if (int rc = check_glossy(__func__, degree, n, means, campos, op_k_rest, rgb != nullptr, sh_stride, sh_split)) return rc;
+    B200GS_CHECK_ARG(n == 0 || (op_dc && opacity && clamped && (op_k_rest == 0 || op_rest)), "NULL pointer");
+    B200GS_CHECK_ARG(n == 0 || !rgb || (shs && (!sh_split || sh_stride == 1 || shs_rest)), "NULL pointer");
     static constexpr decltype(&glossy_fwd_kernel<false, 16>) kernels[2][2] = {
         {glossy_fwd_kernel<false, 16>, glossy_fwd_kernel<false, 25>}, {glossy_fwd_kernel<true, 16>, glossy_fwd_kernel<true, 25>}};
     if (n == 0) return B200GS_OK;
-    kernels[split][degree > 3]<<<(unsigned)div_up64(n, GLOSSY_FWD_THREADS), GLOSSY_FWD_THREADS, 0, s>>>(
+    kernels[sh_split != 0][degree > 3]<<<(unsigned)div_up64(n, GLOSSY_FWD_THREADS), GLOSSY_FWD_THREADS, 0, (cudaStream_t)stream>>>(
         degree, n, means, campos, op_dc, op_rest, op_k_rest, shs, shs_rest, sh_stride, mask, opacity, rgb, clamped);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-int launch_glossy_sh_bwd(int degree, int64_t n, const float* means, const float* campos, int op_k_rest, int sh_stride, bool split,
-                         const uint8_t* clamped, const float* v_opacity, const float* v_rgb, float* v_op_dc, float* v_op_rest,
-                         float* v_shs, float* v_shs_rest, cudaStream_t s) {
+int b200gs_glossy_sh_bwd(int32_t degree, int64_t n, const float* means, const float* campos, int32_t op_k_rest, int32_t sh_stride,
+                         int32_t sh_split, const uint8_t* clamped, const float* v_opacity, const float* v_rgb, float* v_op_dc,
+                         float* v_op_rest, float* v_shs, float* v_shs_rest, void* stream) {
+    if (int rc = check_glossy(__func__, degree, n, means, campos, op_k_rest, v_rgb != nullptr, sh_stride, sh_split)) return rc;
+    B200GS_CHECK_ARG(n == 0 || (clamped && v_opacity && v_op_dc && (op_k_rest == 0 || v_op_rest)), "NULL pointer");
+    B200GS_CHECK_ARG(n == 0 || !v_rgb || (v_shs && (!sh_split || sh_stride == 1 || v_shs_rest)), "NULL pointer");
     static constexpr decltype(&glossy_bwd_kernel<false, 16>) kernels[2][2] = {
         {glossy_bwd_kernel<false, 16>, glossy_bwd_kernel<false, 25>}, {glossy_bwd_kernel<true, 16>, glossy_bwd_kernel<true, 25>}};
     if (n == 0) return B200GS_OK;
-    kernels[split][degree > 3]<<<(unsigned)div_up64(n, GLOSSY_BWD_THREADS), GLOSSY_BWD_THREADS, 0, s>>>(
+    kernels[sh_split != 0][degree > 3]<<<(unsigned)div_up64(n, GLOSSY_BWD_THREADS), GLOSSY_BWD_THREADS, 0, (cudaStream_t)stream>>>(
         degree, n, means, campos, op_k_rest, sh_stride, clamped, v_opacity, v_rgb, v_op_dc, v_op_rest, v_shs, v_shs_rest);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-}  // namespace b200gs
+}  // extern "C"

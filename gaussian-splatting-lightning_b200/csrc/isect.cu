@@ -45,20 +45,34 @@ __global__ void __launch_bounds__(OFFSETS_THREADS) isect_offsets_kernel(int64_t 
 
 }  // namespace
 
-int launch_isect_keys(int n_tiles, const int32_t* tile_ranges, const int32_t* sorted_ids, int64_t n_pairs, const float* depth, int64_t* keys,
-                      cudaStream_t s) {
+}  // namespace b200gs
+
+using namespace b200gs;
+
+extern "C" {
+
+int b200gs_isect_keys(int32_t n_tiles, const int32_t* tile_ranges, const int32_t* sorted_ids, int64_t n_pairs, const float* depth,
+                      int64_t* keys, void* stream) {
+    B200GS_CHECK_ARG(n_tiles >= 0 && n_pairs >= 0 && n_pairs < (int64_t(1) << 31), "bad size");
+    B200GS_CHECK_ARG(n_tiles == 0 || tile_ranges, "tile_ranges must not be NULL");
+    B200GS_CHECK_ARG(n_pairs == 0 || (sorted_ids && depth && keys), "NULL pointer");
+    B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(tile_ranges) & 7u) == 0, "tile_ranges must be 8-byte aligned");
     if (n_tiles == 0 || n_pairs == 0) return B200GS_OK;
-    isect_keys_kernel<<<(unsigned)div_up64(int64_t(n_tiles) * 32, KEYS_THREADS), KEYS_THREADS, 0, s>>>(
+    isect_keys_kernel<<<(unsigned)div_up64(int64_t(n_tiles) * 32, KEYS_THREADS), KEYS_THREADS, 0, (cudaStream_t)stream>>>(
         n_tiles, reinterpret_cast<const int2*>(tile_ranges), sorted_ids, n_pairs, depth, keys);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-int launch_isect_offsets(int64_t n_pairs, const int64_t* keys, int n_tiles, int32_t* offsets, cudaStream_t s) {
+int b200gs_isect_offsets(int64_t n_pairs, const int64_t* keys, int32_t n_tiles, int32_t* offsets, void* stream) {
+    B200GS_CHECK_ARG(n_tiles >= 0 && n_pairs >= 0 && n_pairs < (int64_t(1) << 31), "bad size");
+    B200GS_CHECK_ARG(n_tiles == 0 || offsets, "offsets must not be NULL");
+    B200GS_CHECK_ARG(n_pairs == 0 || keys, "keys must not be NULL");
     if (n_tiles == 0) return B200GS_OK;
-    isect_offsets_kernel<<<(unsigned)div_up(n_tiles, OFFSETS_THREADS), OFFSETS_THREADS, 0, s>>>(n_pairs, keys, n_tiles, offsets);
+    isect_offsets_kernel<<<(unsigned)div_up(n_tiles, OFFSETS_THREADS), OFFSETS_THREADS, 0, (cudaStream_t)stream>>>(n_pairs, keys, n_tiles,
+                                                                                                                    offsets);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-}  // namespace b200gs
+}  // extern "C"

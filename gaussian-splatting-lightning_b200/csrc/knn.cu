@@ -352,26 +352,42 @@ int launch_record_sort(int64_t n, int bits, uint2* a, uint2* b, void* scratch, c
     return B200GS_OK;
 }
 
-size_t knn_workspace_bytes(int64_t n) { return knn_layout(n).total; }
+}  // namespace b200gs
 
-int launch_knn_mean_dist2(int64_t n, const float* points, float* out, void* ws, size_t ws_bytes, cudaStream_t s) {
+using namespace b200gs;
+
+extern "C" {
+
+// both entry points share the workspace layout knn_layout
+size_t b200gs_knn_workspace_bytes(int64_t n) { return n < 0 ? 0 : knn_layout(n).total; }
+
+int b200gs_knn_mean_dist2(int64_t n, const float* points, float* mean_dist2, void* workspace, size_t workspace_bytes, void* stream) {
+    B200GS_CHECK_ARG(n >= 0, "n < 0");
+    B200GS_CHECK_ARG(n == 0 || (points && mean_dist2 && workspace), "NULL pointer");
     if (n == 0) return B200GS_OK;
-    if (int rc = check_knn_workspace(n, ws_bytes)) return rc;
+    if (int rc = check_knn_workspace(n, workspace_bytes)) return rc;
+    const cudaStream_t s = (cudaStream_t)stream;
     const KnnLayout L = knn_layout(n);
-    char* w = (char*)ws;
+    char* w = (char*)workspace;
     if (int rc = build_grid(n, points, L, w, s)) return rc;
     knn_search_kernel<<<(unsigned)div_up64(n, 128), 128, 0, s>>>(n, (const float4*)(w + L.sorted), (const int*)(w + L.cell_lo),
-                                                                (const int*)(w + L.cell_hi), (const KnnGrid*)(w + L.grid), out);
+                                                                (const int*)(w + L.cell_hi), (const KnnGrid*)(w + L.grid), mean_dist2);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-int launch_knn_points(int64_t s_q, const float* queries, int64_t n, const float* points, int k, float* dists, int64_t* idx, void* ws,
-                      size_t ws_bytes, cudaStream_t s) {
-    if (int rc = check_knn_workspace(n, ws_bytes)) return rc;
+int b200gs_knn_points(int64_t s_q, const float* queries, int64_t n, const float* points, int32_t k, float* dists, int64_t* idx,
+                      void* workspace, size_t workspace_bytes, void* stream) {
+    B200GS_CHECK_ARG(s_q >= 0 && n >= 0, "negative size");
+    B200GS_CHECK_ARG(k >= 1 && k <= 32, "K must be 1..32");
+    B200GS_CHECK_ARG(k <= n, "K exceeds the number of reference points");
+    B200GS_CHECK_ARG(points && workspace, "NULL pointer");
+    B200GS_CHECK_ARG(s_q == 0 || (queries && dists && idx), "NULL pointer");
+    if (int rc = check_knn_workspace(n, workspace_bytes)) return rc;
     if (s_q == 0) return B200GS_OK;
+    const cudaStream_t s = (cudaStream_t)stream;
     const KnnLayout L = knn_layout(n);
-    char* w = (char*)ws;
+    char* w = (char*)workspace;
     if (int rc = build_grid(n, points, L, w, s)) return rc;
     const unsigned blocks = (unsigned)div_up64(s_q, 128);
     const float4* sorted = (const float4*)(w + L.sorted);
@@ -388,4 +404,4 @@ int launch_knn_points(int64_t s_q, const float* queries, int64_t n, const float*
     return B200GS_OK;
 }
 
-}  // namespace b200gs
+}  // extern "C"

@@ -83,23 +83,50 @@ __global__ void __launch_bounds__(LT * LT) loss_bwd_kernel(int width, int height
     v_img[p] = up * inv_n * ((1.f - lambda) * sgn - lambda * ssim_grad(g, a, b));
 }
 
+// the grid is (ceil(W/LT), ceil(H/LT), C): C and ceil(H/LT) are at most 65535, and ceil(W/LT) is computed in int
+bool loss_size_ok(int32_t channels, int32_t width, int32_t height) {
+    return channels >= 1 && width >= 1 && height >= 1 && channels <= 65535 && height <= 65535 * LT && width <= INT32_MAX - (LT - 1);
+}
+
+// shared by the forward and the backward; returns the error code, or 0 when the arguments are valid
+int check_loss(const char* fn, int32_t channels, int32_t width, int32_t height, const void* image, const void* target, const void* maps,
+               const void* out) {
+    if (channels < 1 || width < 1 || height < 1) return fail(fn, "bad size: channels, width and height must be >= 1");
+    if (channels > 65535) return fail(fn, "too many channels (> 65535)");
+    if (height > 65535 * LT) return fail(fn, "image too tall (height > 65535 * 16)");
+    if (width > INT32_MAX - (LT - 1)) return fail(fn, "image too wide (width > 2^31 - 16)");
+    if (!(image && target && maps && out)) return fail(fn, "NULL pointer");
+    return 0;
+}
+
 }  // namespace
 
-int64_t loss_blocks(int channels, int width, int height) { return int64_t(channels) * div_up(width, LT) * div_up(height, LT); }
-
-int launch_loss_fwd(int channels, int width, int height, const float* img, const float* gt, float* dmaps, float* partials, cudaStream_t s) {
-    const dim3 grid(div_up(width, LT), div_up(height, LT), channels);
-    loss_fwd_kernel<<<grid, LT * LT, 0, s>>>(width, height, img, gt, dmaps, partials);
-    B200GS_LAUNCH_CHECK();
-    return B200GS_OK;
-}
-
-int launch_loss_bwd(int channels, int width, int height, const float* img, const float* gt, const float* dmaps, float lambda_dssim,
-                    const float* v_loss, float* v_img, cudaStream_t s) {
-    const dim3 grid(div_up(width, LT), div_up(height, LT), channels);
-    loss_bwd_kernel<<<grid, LT * LT, 0, s>>>(width, height, img, gt, dmaps, lambda_dssim, v_loss, v_img);
-    B200GS_LAUNCH_CHECK();
-    return B200GS_OK;
-}
-
 }  // namespace b200gs
+
+using namespace b200gs;
+
+extern "C" {
+
+int64_t b200gs_loss_blocks(int32_t channels, int32_t width, int32_t height) {
+    return loss_size_ok(channels, width, height) ? int64_t(channels) * div_up(width, LT) * div_up(height, LT) : 0;
+}
+
+int b200gs_loss_fwd(int32_t channels, int32_t width, int32_t height, const float* image, const float* target, float* dmaps,
+                    float* partials, void* stream) {
+    if (int rc = check_loss(__func__, channels, width, height, image, target, dmaps, partials)) return rc;
+    const dim3 grid(div_up(width, LT), div_up(height, LT), channels);
+    loss_fwd_kernel<<<grid, LT * LT, 0, (cudaStream_t)stream>>>(width, height, image, target, dmaps, partials);
+    B200GS_LAUNCH_CHECK();
+    return B200GS_OK;
+}
+
+int b200gs_loss_bwd(int32_t channels, int32_t width, int32_t height, const float* image, const float* target, const float* dmaps,
+                    float lambda_dssim, const float* v_loss, float* v_image, void* stream) {
+    if (int rc = check_loss(__func__, channels, width, height, image, target, dmaps, v_image)) return rc;
+    const dim3 grid(div_up(width, LT), div_up(height, LT), channels);
+    loss_bwd_kernel<<<grid, LT * LT, 0, (cudaStream_t)stream>>>(width, height, image, target, dmaps, lambda_dssim, v_loss, v_image);
+    B200GS_LAUNCH_CHECK();
+    return B200GS_OK;
+}
+
+}  // extern "C"

@@ -62,20 +62,34 @@ __global__ void __launch_bounds__(256) position_noise_kernel(int64_t n, float* _
 
 }  // namespace
 
-int launch_mcmc_relocation(int64_t n, const float* opacities, const float* scales, const int32_t* counts, int n_max, float* new_opacities,
-                           float* new_scales, cudaStream_t s) {
-    if (n == 0) return B200GS_OK;
-    relocation_kernel<<<(unsigned)div_up64(n, 256), 256, 0, s>>>(n, opacities, scales, counts, n_max, new_opacities, new_scales);
-    B200GS_LAUNCH_CHECK();
-    return B200GS_OK;
-}
-
-int launch_mcmc_position_noise(int64_t n, float* means, const float* log_scales, const float* raw_quats, const float* opacity_logits,
-                               float scale, uint64_t seed, uint64_t offset, cudaStream_t s) {
-    if (n == 0) return B200GS_OK;
-    position_noise_kernel<<<(unsigned)div_up64(n, 256), 256, 0, s>>>(n, means, log_scales, raw_quats, opacity_logits, scale, seed, offset);
-    B200GS_LAUNCH_CHECK();
-    return B200GS_OK;
-}
-
 }  // namespace b200gs
+
+using namespace b200gs;
+
+extern "C" {
+
+int b200gs_mcmc_relocation(int64_t n, const float* opacities, const float* scales, const int32_t* counts, const float* binoms, int32_t n_max,
+                           float* new_opacities, float* new_scales, void* stream) {
+    B200GS_CHECK_ARG(n >= 0, "n < 0");
+    B200GS_CHECK_ARG(n_max >= 1, "n_max < 1");
+    B200GS_CHECK_ARG(n == 0 || (opacities && scales && counts && binoms && new_opacities && new_scales), "NULL pointer");
+    if (n == 0) return B200GS_OK;
+    relocation_kernel<<<(unsigned)div_up64(n, 256), 256, 0, (cudaStream_t)stream>>>(n, opacities, scales, counts, n_max, new_opacities,
+                                                                                    new_scales);
+    B200GS_LAUNCH_CHECK();
+    return B200GS_OK;
+}
+
+int b200gs_mcmc_position_noise(int64_t n, float* means, const float* log_scales, const float* raw_quats, const float* opacity_logits,
+                               float scale, uint64_t seed, uint64_t offset, void* stream) {
+    B200GS_CHECK_ARG(n >= 0, "n < 0");
+    B200GS_CHECK_ARG(n == 0 || (means && log_scales && raw_quats && opacity_logits), "NULL pointer");
+    B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(raw_quats) & 15u) == 0, "raw_quats must be 16-byte aligned");
+    if (n == 0) return B200GS_OK;
+    position_noise_kernel<<<(unsigned)div_up64(n, 256), 256, 0, (cudaStream_t)stream>>>(n, means, log_scales, raw_quats, opacity_logits, scale,
+                                                                                        seed, offset);
+    B200GS_LAUNCH_CHECK();
+    return B200GS_OK;
+}
+
+}  // extern "C"

@@ -178,16 +178,57 @@ dim3 tiles(int height, int width) { return dim3(unsigned(div_up(width, T)), unsi
 
 Mat make_mat(const float* m, int64_t s0, int64_t s1, const float* k, int64_t k0, int64_t k1) { return Mat{m, s0, s1, k, k0, k1}; }
 
-}  // namespace
+// the grid is tiles(height, width): its y dimension, ceil(H/T), is at most 65535
+bool size_ok(int32_t height, int32_t width) {
+    return height >= 1 && width >= 1 && height <= 65535 * T && int64_t(height) * width <= INT32_MAX;
+}
 
 size_t normal_reg_workspace_bytes(int height, int width) {
     const dim3 g = tiles(height, width);
     return size_t(HEAD + int64_t(g.x) * g.y) * sizeof(float);
 }
 
-int launch_normal_reg_fwd(int height, int width, const float* normal, int64_t sc, int64_t sy, int64_t sx, const float* depth,
+// depth, alpha [H,W] contiguous; normal [3,H,W] read at normal[c sc + y sy + x sx]; v_normal [3,H,W] and the depth_to_normal output
+// [H,W,3] contiguous; the 4x4 camera matrix (w2c for the loss, c2w for depth_to_normal) at m[i ms0 + j ms1] and K [3,3] at
+// K[i ks0 + j ks1].  Shared by the three entry points; returns the error code, or 0 when the arguments are valid
+int check_normal_maps(const char* fn, int32_t height, int32_t width, const float* depth, const float* cam, int64_t ms0, int64_t ms1,
+                      const float* K, int64_t ks0, int64_t ks1) {
+    if (height < 1 || width < 1) return fail(fn, "image size must be >= 1");
+    if (!size_ok(height, width)) return fail(fn, "image too large");
+    if (ms0 < 0 || ms1 < 0 || ks0 < 0 || ks1 < 0) return fail(fn, "negative matrix stride");
+    if (!(depth && cam && K)) return fail(fn, "NULL pointer");
+    return 0;
+}
+
+// the backward reads the coefficient its forward wrote to the workspace
+int check_normal_reg_workspace(const char* fn, int32_t height, int32_t width, const float* alpha, const void* workspace,
+                               size_t workspace_bytes) {
+    if (!(alpha && workspace)) return fail(fn, "NULL pointer");
+    if (workspace_bytes < normal_reg_workspace_bytes(height, width)) return workspace_too_small(fn);
+    return 0;
+}
+
+}  // namespace
+
+}  // namespace b200gs
+
+using namespace b200gs;
+
+extern "C" {
+
+size_t b200gs_normal_reg_workspace_bytes(int32_t height, int32_t width) {
+    return size_ok(height, width) ? normal_reg_workspace_bytes(height, width) : 0;
+}
+
+int b200gs_normal_reg_fwd(int32_t height, int32_t width, const float* normal, int64_t sc, int64_t sy, int64_t sx, const float* depth,
                           const float* alpha, const float* w2c, int64_t ms0, int64_t ms1, const float* K, int64_t ks0, int64_t ks1,
-                          float weight, float* ws, float* loss, cudaStream_t st) {
+                          float weight, void* workspace, size_t workspace_bytes, float* loss, void* stream) {
+    if (int rc = check_normal_maps(__func__, height, width, depth, w2c, ms0, ms1, K, ks0, ks1)) return rc;
+    if (int rc = check_normal_reg_workspace(__func__, height, width, alpha, workspace, workspace_bytes)) return rc;
+    B200GS_CHECK_ARG(normal && loss, "NULL pointer");
+    B200GS_CHECK_ARG(sc >= 0 && sy >= 0 && sx >= 0, "negative normal stride");
+    const cudaStream_t st = (cudaStream_t)stream;
+    float* ws = static_cast<float*>(workspace);
     const dim3 g = tiles(height, width);
     const Mat mat = make_mat(w2c, ms0, ms1, K, ks0, ks1);
     normal_reg_partials_kernel<<<g, THREADS, 0, st>>>(height, width, depth, alpha, normal, sc, sy, sx, mat, ws + HEAD);
@@ -197,19 +238,26 @@ int launch_normal_reg_fwd(int height, int width, const float* normal, int64_t sc
     return B200GS_OK;
 }
 
-int launch_normal_reg_bwd(int height, int width, const float* depth, const float* alpha, const float* w2c, int64_t ms0, int64_t ms1,
-                          const float* K, int64_t ks0, int64_t ks1, const float* ws, const float* v_loss, float* v_normal, cudaStream_t st) {
-    normal_reg_bwd_kernel<<<tiles(height, width), THREADS, 0, st>>>(height, width, depth, alpha, make_mat(w2c, ms0, ms1, K, ks0, ks1), ws,
-                                                                    v_loss, v_normal);
+int b200gs_normal_reg_bwd(int32_t height, int32_t width, const float* depth, const float* alpha, const float* w2c, int64_t ms0, int64_t ms1,
+                          const float* K, int64_t ks0, int64_t ks1, const void* workspace, size_t workspace_bytes, const float* v_loss,
+                          float* v_normal, void* stream) {
+    if (int rc = check_normal_maps(__func__, height, width, depth, w2c, ms0, ms1, K, ks0, ks1)) return rc;
+    if (int rc = check_normal_reg_workspace(__func__, height, width, alpha, workspace, workspace_bytes)) return rc;
+    B200GS_CHECK_ARG(v_loss && v_normal, "NULL pointer");
+    normal_reg_bwd_kernel<<<tiles(height, width), THREADS, 0, (cudaStream_t)stream>>>(
+        height, width, depth, alpha, make_mat(w2c, ms0, ms1, K, ks0, ks1), static_cast<const float*>(workspace), v_loss, v_normal);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-int launch_depth_to_normal(int height, int width, const float* depth, const float* c2w, int64_t ms0, int64_t ms1, const float* K,
-                           int64_t ks0, int64_t ks1, float* out, cudaStream_t st) {
-    depth_to_normal_kernel<<<tiles(height, width), THREADS, 0, st>>>(height, width, depth, make_mat(c2w, ms0, ms1, K, ks0, ks1), out);
+int b200gs_depth_to_normal(int32_t height, int32_t width, const float* depth, const float* c2w, int64_t ms0, int64_t ms1, const float* K,
+                           int64_t ks0, int64_t ks1, float* normals, void* stream) {
+    if (int rc = check_normal_maps(__func__, height, width, depth, c2w, ms0, ms1, K, ks0, ks1)) return rc;
+    B200GS_CHECK_ARG(normals, "NULL pointer");
+    depth_to_normal_kernel<<<tiles(height, width), THREADS, 0, (cudaStream_t)stream>>>(height, width, depth,
+                                                                                       make_mat(c2w, ms0, ms1, K, ks0, ks1), normals);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-}  // namespace b200gs
+}  // extern "C"

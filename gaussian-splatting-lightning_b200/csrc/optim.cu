@@ -44,21 +44,33 @@ __global__ void __launch_bounds__(256) densify_stats_kernel(int64_t n, const int
 
 }  // namespace
 
-int launch_selective_adam(int64_t rows, int width, float* param, const float* grad, float* exp_avg, float* exp_avg_sq, const uint8_t* visible,
-                          float lr, float b1, float b2, float eps, cudaStream_t s) {
+}  // namespace b200gs
+
+using namespace b200gs;
+
+extern "C" {
+
+int b200gs_selective_adam(int64_t rows, int32_t width, float* param, const float* grad, float* exp_avg, float* exp_avg_sq,
+                          const uint8_t* visible, float lr, float beta1, float beta2, float eps, void* stream) {
+    B200GS_CHECK_ARG(rows >= 0 && width > 0, "bad sizes");
+    B200GS_CHECK_ARG(rows == 0 || (param && grad && exp_avg && exp_avg_sq && visible), "NULL pointer");
     const int64_t total = rows * width;
     if (total == 0) return B200GS_OK;
-    selective_adam_kernel<<<(unsigned)div_up64(total, 256), 256, 0, s>>>(total, width, param, grad, exp_avg, exp_avg_sq, visible, lr, b1, b2, eps);
+    selective_adam_kernel<<<(unsigned)div_up64(total, 256), 256, 0, (cudaStream_t)stream>>>(total, width, param, grad, exp_avg, exp_avg_sq,
+                                                                                            visible, lr, beta1, beta2, eps);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-int launch_densify_stats(int64_t n, const int32_t* radii, const uint8_t* visible, const float* grad, int grad_stride, float sx, float sy,
-                         float* max_radii2d, float* grad_accum, float* denom, cudaStream_t s) {
+int b200gs_densify_stats(int64_t n, const int32_t* radii, const uint8_t* visible, const float* grad, int32_t grad_stride, float scale_x,
+                         float scale_y, float* max_radii2d, float* grad_accum, float* denom, void* stream) {
+    B200GS_CHECK_ARG(n >= 0 && grad_stride >= 2, "bad sizes");
+    B200GS_CHECK_ARG(n == 0 || (radii && grad && max_radii2d && grad_accum && denom), "NULL pointer");
     if (n == 0) return B200GS_OK;
-    densify_stats_kernel<<<(unsigned)div_up64(n, 256), 256, 0, s>>>(n, radii, visible, grad, grad_stride, sx, sy, max_radii2d, grad_accum, denom);
+    densify_stats_kernel<<<(unsigned)div_up64(n, 256), 256, 0, (cudaStream_t)stream>>>(n, radii, visible, grad, grad_stride, scale_x, scale_y,
+                                                                                       max_radii2d, grad_accum, denom);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-}  // namespace b200gs
+}  // extern "C"

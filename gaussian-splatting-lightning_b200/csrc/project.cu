@@ -955,47 +955,156 @@ static int project_bwd_launch(const B200gsView& v, const RawIO& raw, int64_t n, 
     return B200GS_OK;
 }
 
-int launch_project_fwd(const B200gsView& v, int64_t n, const float* means, const float* scales, const float* quats,
+// split = true: coeffs / v_coeffs are dc [n,1,3], rest / v_rest [n,stride-1,3] read and written in place, mask[n] (nullable) zeroes
+// rows, as in sh_fwd_kernel; otherwise rest, mask and v_rest are ignored
+static int launch_sh_fwd(int degree, int stride, int64_t n, const float* dirs, const float* coeffs, float* rgb, cudaStream_t s,
+                         bool split = false, const float* rest = nullptr, const uint8_t* mask = nullptr) {
+    static constexpr decltype(&sh_fwd_kernel<false, 16>) kernels[2][2] = {
+        {sh_fwd_kernel<false, 16>, sh_fwd_kernel<false, 25>}, {sh_fwd_kernel<true, 16>, sh_fwd_kernel<true, 25>}};
+    if (n == 0) return B200GS_OK;
+    kernels[split][degree > 3]<<<(unsigned)div_up64(n, 256), 256, 0, s>>>(degree, stride, n, dirs, coeffs, rest, mask, rgb);
+    B200GS_LAUNCH_CHECK();
+    return B200GS_OK;
+}
+
+static int launch_sh_bwd(int degree, int stride, int64_t n, const float* dirs, const float* coeffs, const float* v_rgb, float* v_coeffs,
+                         float* v_dirs, cudaStream_t s, bool split = false, const float* rest = nullptr, const uint8_t* mask = nullptr,
+                         float* v_rest = nullptr) {
+    static constexpr decltype(&sh_bwd_kernel<false, 16>) kernels[2][2] = {
+        {sh_bwd_kernel<false, 16>, sh_bwd_kernel<false, 25>}, {sh_bwd_kernel<true, 16>, sh_bwd_kernel<true, 25>}};
+    if (n == 0) return B200GS_OK;
+    kernels[split][degree > 3]<<<(unsigned)div_up64(n, 256), 256, 0, s>>>(degree, stride, n, dirs, coeffs, rest, mask, v_rgb, v_coeffs,
+                                                                          v_rest, v_dirs);
+    B200GS_LAUNCH_CHECK();
+    return B200GS_OK;
+}
+
+static int check_view(const B200gsView* v, bool needs_sh) {
+    if (v == nullptr) { set_error("view is NULL"); return B200GS_EINVAL; }
+    if (v->width <= 0 || v->height <= 0) { set_error("bad image size %dx%d", v->width, v->height); return B200GS_EINVAL; }
+    if (v->mode != B200GS_MODE_VANILLA && v->mode != B200GS_MODE_GSPLAT) { set_error("bad mode %d", v->mode); return B200GS_EINVAL; }
+    if (needs_sh) {
+        if (v->sh_degree < 0 || v->sh_degree > 4) { set_error("sh_degree %d unsupported (0..4)", v->sh_degree); return B200GS_EINVAL; }
+        if (v->sh_stride < (v->sh_degree + 1) * (v->sh_degree + 1)) {
+            set_error("sh_stride %d < (sh_degree+1)^2", v->sh_stride);
+            return B200GS_EINVAL;
+        }
+    }
+    return B200GS_OK;
+}
+
+static int check_views(const B200gsView* views, int32_t n_views) {
+    if (views == nullptr) { set_error("views is NULL"); return B200GS_EINVAL; }
+    if (n_views < 1 || n_views > B200GS_MAX_VIEWS) { set_error("n_views %d out of range (1..%d)", n_views, B200GS_MAX_VIEWS); return B200GS_EINVAL; }
+    for (int j = 0; j < n_views; ++j) {
+        int rc = check_view(views + j, true);
+        if (rc) return rc;
+        if (views[j].mode != B200GS_MODE_GSPLAT) { set_error("multi-view projection supports gsplat constants only"); return B200GS_EINVAL; }
+        if (views[j].sh_degree != views[0].sh_degree || views[j].sh_stride != views[0].sh_stride) {
+            set_error("all views of a multi-view launch must share sh_degree / sh_stride");
+            return B200GS_EINVAL;
+        }
+    }
+    return B200GS_OK;
+}
+
+static size_t project_pack_workspace_bytes(int n_views, int64_t n) {
+    return 256 + (size_t)n_views * (size_t)div_up64(n > 0 ? n : 1, PACK_THREADS) * sizeof(uint32_t);
+}
+
+}  // namespace b200gs
+
+using namespace b200gs;
+
+extern "C" {
+
+int b200gs_project_fwd(const B200gsView* view, int64_t n, const float* means, const float* scales, const float* quats,
                        const float* shs, float* xy, float* depth, int32_t* radii, float* conic, float* comp,
-                       int32_t* tiles, float* cov3d, float* rgb, uint8_t* clamped, cudaStream_t s) {
-    return project_fwd_launch<false>(v, RawIO{}, n, means, scales, quats, shs, xy, depth, radii, conic, comp, tiles, cov3d, rgb, clamped,
-                                     nullptr, s);
+                       int32_t* tiles, float* cov3d, float* rgb, uint8_t* clamped, void* stream) {
+    int rc = check_view(view, shs != nullptr);
+    if (rc) return rc;
+    B200GS_CHECK_ARG(n >= 0, "n < 0");
+    if (n > 0) {
+        B200GS_CHECK_ARG(means && scales && quats, "means/scales/quats must not be NULL");
+        B200GS_CHECK_ARG(xy && depth && radii && conic && tiles, "xy/depth/radii/conic/tiles must not be NULL");
+        B200GS_CHECK_ARG(shs == nullptr || (rgb && clamped), "rgb/clamped required when shs is given");
+    }
+    return project_fwd_launch<false>(*view, RawIO{}, n, means, scales, quats, shs, xy, depth, radii, conic, comp, tiles, cov3d, rgb, clamped,
+                                     nullptr, (cudaStream_t)stream);
 }
 
-int launch_project_fwd_rows(const B200gsView& v, int64_t n, const float* means, const float* log_scales, const float* raw_quats,
-                            const float* opac_logits, const float* shs_dc, const float* shs_rest, int anti_aliased, float* rows,
-                            int32_t* radii, uint8_t* clamped, int32_t* tiles, cudaStream_t s) {
-    RawIO raw{};
-    raw.opac_in = opac_logits; raw.shs_rest = shs_rest; raw.anti_aliased = anti_aliased;
-    return project_fwd_launch<true>(v, raw, n, means, log_scales, raw_quats, shs_dc, nullptr, nullptr, radii, nullptr, nullptr, tiles, nullptr,
-                                    nullptr, clamped, rows, s);
-}
-
-int launch_project_bwd(const B200gsView& v, int64_t n, const float* means, const float* scales, const float* quats,
+int b200gs_project_bwd(const B200gsView* view, int64_t n, const float* means, const float* scales, const float* quats,
                        const float* shs, const int32_t* radii, const uint8_t* clamped, const float* v_xy,
                        const float* v_depth, const float* v_conic, const float* v_comp, const float* v_rgb,
-                       float* v_means, float* v_scales, float* v_quats, float* v_shs, cudaStream_t s) {
-    return project_bwd_launch<false>(v, RawIO{}, n, means, scales, quats, shs, radii, clamped, v_xy, v_depth, v_conic, v_comp, v_rgb,
-                                     v_means, v_scales, v_quats, v_shs, s);
+                       float* v_means, float* v_scales, float* v_quats, float* v_shs, void* stream) {
+    int rc = check_view(view, shs != nullptr);
+    if (rc) return rc;
+    B200GS_CHECK_ARG(n >= 0, "n < 0");
+    if (n > 0) {
+        B200GS_CHECK_ARG(means && scales && quats && radii, "means/scales/quats/radii must not be NULL");
+        B200GS_CHECK_ARG(v_xy && v_conic, "v_xy/v_conic must not be NULL");
+        B200GS_CHECK_ARG(v_means && v_scales && v_quats, "v_means/v_scales/v_quats must not be NULL");
+        B200GS_CHECK_ARG((shs == nullptr) == (v_shs == nullptr), "shs and v_shs must be given together");
+        B200GS_CHECK_ARG(shs == nullptr || (clamped && v_rgb), "clamped/v_rgb required when shs is given");
+    }
+    return project_bwd_launch<false>(*view, RawIO{}, n, means, scales, quats, shs, radii, clamped, v_xy, v_depth, v_conic, v_comp, v_rgb,
+                                     v_means, v_scales, v_quats, v_shs, (cudaStream_t)stream);
 }
 
-int launch_project_bwd_rows(const B200gsView& v, int64_t n, const float* means, const float* log_scales, const float* raw_quats,
-                            const float* opac_logits, const float* shs_dc, const float* shs_rest, int anti_aliased, const int32_t* radii,
-                            const uint8_t* clamped, const int32_t* row_offsets, const float* v_rows, int accumulate, float* v_means,
-                            float* v_log_scales, float* v_raw_quats, float* v_opac_logit, float* v_shs_dc, float* v_shs_rest,
-                            float* v_mean2d, int v_mean2d_cols, cudaStream_t s) {
+int b200gs_project_fwd_rows(const B200gsView* view, int64_t n, const float* means, const float* log_scales, const float* raw_quats,
+                            const float* opacity_logits, const float* shs_dc, const float* shs_rest, int32_t anti_aliased, float* rows,
+                            int32_t* radii, uint8_t* clamped, int32_t* tiles, void* stream) {
+    int rc = check_view(view, true);
+    if (rc) return rc;
+    B200GS_CHECK_ARG(n >= 0, "n < 0");
+    if (n > 0) {
+        B200GS_CHECK_ARG(means && log_scales && raw_quats && opacity_logits && shs_dc, "NULL input pointer");
+        B200GS_CHECK_ARG(view->sh_stride == 1 || shs_rest, "shs_rest required when sh_stride > 1");
+        B200GS_CHECK_ARG(rows && radii && clamped, "NULL output pointer");
+        B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(rows) & 15u) == 0, "rows must be 16-byte aligned");
+    }
     RawIO raw{};
-    raw.opac_in = opac_logits; raw.shs_rest = shs_rest; raw.anti_aliased = anti_aliased;
-    raw.v_opac_logit = v_opac_logit; raw.v_shs_rest = v_shs_rest;
-    raw.v_rows = v_rows; raw.row_offsets = row_offsets; raw.accumulate = accumulate;
-    raw.v_mean2d = v_mean2d; raw.v_mean2d_cols = v_mean2d_cols;
-    return project_bwd_launch<true>(v, raw, n, means, log_scales, raw_quats, shs_dc, radii, clamped, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                    v_means, v_log_scales, v_raw_quats, v_shs_dc, s);
+    raw.opac_in = opacity_logits; raw.shs_rest = shs_rest; raw.anti_aliased = anti_aliased;
+    return project_fwd_launch<true>(*view, raw, n, means, log_scales, raw_quats, shs_dc, nullptr, nullptr, radii, nullptr, nullptr, tiles,
+                                    nullptr, nullptr, clamped, rows, (cudaStream_t)stream);
 }
 
-int launch_project_fwd_multi(const B200gsView* views, int n_views, int64_t n, const float* means, const float* scales, const float* quats,
-                             const float* opac_logits, const float* shs_dc, const float* shs_rest, int anti_aliased, float* xy, float* depth,
-                             int32_t* radii, float* conic, float* rgb, uint8_t* clamped, float* opac_out, cudaStream_t s) {
+int b200gs_project_bwd_rows(const B200gsView* view, int64_t n, const float* means, const float* log_scales, const float* raw_quats,
+                            const float* opacity_logits, const float* shs_dc, const float* shs_rest, int32_t anti_aliased,
+                            const int32_t* radii, const uint8_t* clamped, const int32_t* row_offsets, const float* v_rows,
+                            int32_t accumulate, float* v_means, float* v_log_scales, float* v_raw_quats, float* v_opacity_logits,
+                            float* v_shs_dc, float* v_shs_rest, float* v_mean2d, int32_t v_mean2d_cols, void* stream) {
+    int rc = check_view(view, true);
+    if (rc) return rc;
+    B200GS_CHECK_ARG(n >= 0, "n < 0");
+    B200GS_CHECK_ARG(v_mean2d == nullptr || v_mean2d_cols == 2 || v_mean2d_cols == 3, "v_mean2d_cols must be 2 or 3");
+    if (n > 0) {
+        B200GS_CHECK_ARG(means && log_scales && raw_quats && opacity_logits && shs_dc && radii && clamped, "NULL input pointer");
+        B200GS_CHECK_ARG(view->sh_stride == 1 || (shs_rest && v_shs_rest), "shs_rest / v_shs_rest required when sh_stride > 1");
+        B200GS_CHECK_ARG(v_means && v_log_scales && v_raw_quats && v_opacity_logits && v_shs_dc, "NULL output pointer");
+    }
+    static const float dummy = 0.f;   // v_rows may be NULL when no Gaussian of the shard is visible: never dereferenced then
+    RawIO raw{};
+    raw.opac_in = opacity_logits; raw.shs_rest = shs_rest; raw.anti_aliased = anti_aliased;
+    raw.v_opac_logit = v_opacity_logits; raw.v_shs_rest = v_shs_rest;
+    raw.v_rows = v_rows ? v_rows : &dummy; raw.row_offsets = row_offsets; raw.accumulate = accumulate;
+    raw.v_mean2d = v_mean2d; raw.v_mean2d_cols = v_mean2d_cols;
+    return project_bwd_launch<true>(*view, raw, n, means, log_scales, raw_quats, shs_dc, radii, clamped, nullptr, nullptr, nullptr, nullptr,
+                                    nullptr, v_means, v_log_scales, v_raw_quats, v_shs_dc, (cudaStream_t)stream);
+}
+
+int b200gs_project_fwd_raw_multi(const B200gsView* views, int32_t n_views, int64_t n, const float* means, const float* scales,
+                                 const float* quats, const float* opac_logits, const float* shs_dc, const float* shs_rest,
+                                 int32_t anti_aliased, float* xy, float* depth, int32_t* radii, float* conic, float* rgb, uint8_t* clamped,
+                                 float* opac_out, void* stream) {
+    int rc = check_views(views, n_views);
+    if (rc) return rc;
+    B200GS_CHECK_ARG(n >= 0, "n < 0");
+    if (n > 0) {
+        B200GS_CHECK_ARG(means && scales && quats && opac_logits && shs_dc, "NULL input pointer");
+        B200GS_CHECK_ARG(views[0].sh_stride == 1 || shs_rest, "shs_rest required when sh_stride > 1");
+        B200GS_CHECK_ARG(xy && depth && radii && conic && rgb && clamped && opac_out, "NULL output pointer");
+    }
     if (n == 0 || n_views == 0) return B200GS_OK;
     ViewPack vp;
     for (int j = 0; j < n_views; ++j) vp.v[j] = views[j];
@@ -1003,19 +1112,33 @@ int launch_project_fwd_multi(const B200gsView* views, int n_views, int64_t n, co
     RawIO raw{};
     raw.opac_in = opac_logits; raw.shs_rest = shs_rest; raw.opac_out = opac_out; raw.anti_aliased = anti_aliased;
     const auto kernel = views[0].sh_degree > 3 ? project_fwd_multi_kernel<25> : project_fwd_multi_kernel<16>;
-    kernel<<<(unsigned)div_up64(n, 256), 256, 0, s>>>(vp, n_views, raw, n, means, scales, quats, shs_dc, (float2*)xy, depth, radii, conic, rgb, clamped);
+    kernel<<<(unsigned)div_up64(n, 256), 256, 0, (cudaStream_t)stream>>>(vp, n_views, raw, n, means, scales, quats, shs_dc, (float2*)xy, depth,
+                                                                         radii, conic, rgb, clamped);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-size_t project_pack_workspace_bytes(int n_views, int64_t n) {
-    return 256 + (size_t)n_views * (size_t)div_up64(n > 0 ? n : 1, PACK_THREADS) * sizeof(uint32_t);
-}
+size_t b200gs_project_pack_workspace_bytes(int32_t n_views, int64_t n) { return project_pack_workspace_bytes(n_views, n); }
 
-int launch_project_pack_multi(const B200gsView* views, int n_views, int64_t n, const float* means, const float* scales, const float* quats,
-                              const float* opac_logits, const float* shs_dc, const float* shs_rest, int anti_aliased, float* xy, int32_t* radii,
-                              uint8_t* clamped, int32_t* row_index, float* const* dst_rows, int64_t cap, void* workspace, size_t workspace_bytes,
-                              int64_t* d_count, cudaStream_t s) {
+int b200gs_project_pack_multi(const B200gsView* views, int32_t n_views, int64_t n, const float* means, const float* scales, const float* quats,
+                              const float* opac_logits, const float* shs_dc, const float* shs_rest, int32_t anti_aliased, float* xy,
+                              int32_t* radii, uint8_t* clamped, int32_t* row_index, void* const* dst_rows, int64_t cap, void* workspace,
+                              size_t workspace_bytes, int64_t* d_count, void* stream) {
+    B200GS_CHECK_ARG(views && n_views >= 1 && n_views <= B200GS_MAX_VIEWS, "n_views must be 1..B200GS_MAX_VIEWS");
+    B200GS_CHECK_ARG(n >= 0 && n < (int64_t(1) << 30) && cap > 0 && cap < (int64_t(1) << 30), "bad size");
+    for (int j = 0; j < n_views; ++j) {
+        int rc = check_view(views + j, true);
+        if (rc) return rc;
+        B200GS_CHECK_ARG(views[j].mode == B200GS_MODE_GSPLAT, "multi-view launches use the gsplat constant set");
+        B200GS_CHECK_ARG(dst_rows && dst_rows[j] && (reinterpret_cast<uintptr_t>(dst_rows[j]) & 15u) == 0, "dst_rows: NULL or misaligned");
+    }
+    if (n > 0) {
+        B200GS_CHECK_ARG(means && scales && quats && opac_logits && shs_dc, "NULL input pointer");
+        B200GS_CHECK_ARG(views[0].sh_stride == 1 || shs_rest, "shs_rest required when sh_stride > 1");
+        B200GS_CHECK_ARG(xy && radii && clamped && row_index && workspace, "NULL output pointer");
+    }
+    B200GS_CHECK_ARG(d_count, "NULL d_count");
+    const cudaStream_t s = (cudaStream_t)stream;
     if (n_views == 0) return B200GS_OK;
     if (n == 0) {
         B200GS_CUDA(cudaMemsetAsync(d_count, 0, sizeof(int64_t) * (size_t)n_views, s));
@@ -1030,7 +1153,7 @@ int launch_project_pack_multi(const B200gsView* views, int n_views, int64_t n, c
     PackDst dst;
     for (int j = 0; j < B200GS_MAX_VIEWS; ++j) {
         vp.v[j] = views[j < n_views ? j : 0];
-        dst.p[j] = j < n_views ? dst_rows[j] : nullptr;
+        dst.p[j] = j < n_views ? (float*)dst_rows[j] : nullptr;
     }
     RawIO raw{};
     raw.opac_in = opac_logits; raw.shs_rest = shs_rest; raw.anti_aliased = anti_aliased;
@@ -1058,10 +1181,19 @@ int launch_project_pack_multi(const B200gsView* views, int n_views, int64_t n, c
     return B200GS_OK;
 }
 
-int launch_project_bwd_multi(const B200gsView* views, int n_views, int64_t n, const float* means, const float* scales, const float* quats,
-                             const float* opac_logits, const float* shs_rest, int anti_aliased, const int32_t* radii, const uint8_t* clamped,
-                             const int32_t* row_index, const float* const* v_rows, float* v_means, float* v_scales, float* v_quats,
-                             float* v_opac_logit, float* v_shs_dc, float* v_shs_rest, cudaStream_t s) {
+int b200gs_project_bwd_rows_multi(const B200gsView* views, int32_t n_views, int64_t n, const float* means, const float* scales,
+                                  const float* quats, const float* opac_logits, const float* shs_dc, const float* shs_rest,
+                                  int32_t anti_aliased, const int32_t* radii, const uint8_t* clamped, const int32_t* row_index,
+                                  const float* const* v_rows, float* v_means, float* v_scales, float* v_quats, float* v_opac_logit,
+                                  float* v_shs_dc, float* v_shs_rest, void* stream) {
+    int rc = check_views(views, n_views);
+    if (rc) return rc;
+    B200GS_CHECK_ARG(n >= 0, "n < 0");
+    if (n > 0) {
+        B200GS_CHECK_ARG(means && scales && quats && opac_logits && shs_dc && radii && clamped && row_index && v_rows, "NULL input pointer");
+        B200GS_CHECK_ARG(views[0].sh_stride == 1 || (shs_rest && v_shs_rest), "shs_rest / v_shs_rest required when sh_stride > 1");
+        B200GS_CHECK_ARG(v_means && v_scales && v_quats && v_opac_logit && v_shs_dc, "NULL output pointer");
+    }
     if (n == 0 || n_views == 0) return B200GS_OK;
     ViewPack vp;
     RowSources src;
@@ -1079,32 +1211,46 @@ int launch_project_bwd_multi(const B200gsView* views, int n_views, int64_t n, co
         return B200GS_EINVAL;
     }
     const auto kernel = views[0].sh_degree > 3 || views[0].sh_stride > 16 ? project_bwd_multi_kernel<25> : project_bwd_multi_kernel<16>;
-    kernel<<<(unsigned)div_up64(n, BWD_THREADS), BWD_THREADS, 0, s>>>(vp, n_views, raw, src, n, means, scales, quats, radii, clamped, row_index,
-                                                                      v_means, v_scales, (float4*)v_quats, v_shs_dc);
+    kernel<<<(unsigned)div_up64(n, BWD_THREADS), BWD_THREADS, 0, (cudaStream_t)stream>>>(vp, n_views, raw, src, n, means, scales, quats, radii,
+                                                                                         clamped, row_index, v_means, v_scales,
+                                                                                         (float4*)v_quats, v_shs_dc);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-// split: coeffs = dc, rest / v_rest as in sh_fwd_kernel; otherwise rest, mask and v_rest are ignored
-int launch_sh_fwd(int degree, int stride, int64_t n, const float* dirs, const float* coeffs, float* rgb, cudaStream_t s, bool split,
-                  const float* rest, const uint8_t* mask) {
-    static constexpr decltype(&sh_fwd_kernel<false, 16>) kernels[2][2] = {
-        {sh_fwd_kernel<false, 16>, sh_fwd_kernel<false, 25>}, {sh_fwd_kernel<true, 16>, sh_fwd_kernel<true, 25>}};
-    if (n == 0) return B200GS_OK;
-    kernels[split][degree > 3]<<<(unsigned)div_up64(n, 256), 256, 0, s>>>(degree, stride, n, dirs, coeffs, rest, mask, rgb);
-    B200GS_LAUNCH_CHECK();
-    return B200GS_OK;
+int b200gs_sh_fwd(int32_t degree, int32_t sh_stride, int64_t n, const float* dirs, const float* coeffs, float* rgb, void* stream) {
+    B200GS_CHECK_ARG(degree >= 0 && degree <= 4, "degree must be 0..4");
+    B200GS_CHECK_ARG(sh_stride >= (degree + 1) * (degree + 1), "sh_stride < (degree+1)^2");
+    B200GS_CHECK_ARG(n >= 0, "n < 0");
+    B200GS_CHECK_ARG(n == 0 || (dirs && coeffs && rgb), "NULL pointer");
+    return launch_sh_fwd(degree, sh_stride, n, dirs, coeffs, rgb, (cudaStream_t)stream);
 }
 
-int launch_sh_bwd(int degree, int stride, int64_t n, const float* dirs, const float* coeffs, const float* v_rgb,
-                  float* v_coeffs, float* v_dirs, cudaStream_t s, bool split, const float* rest, const uint8_t* mask, float* v_rest) {
-    static constexpr decltype(&sh_bwd_kernel<false, 16>) kernels[2][2] = {
-        {sh_bwd_kernel<false, 16>, sh_bwd_kernel<false, 25>}, {sh_bwd_kernel<true, 16>, sh_bwd_kernel<true, 25>}};
-    if (n == 0) return B200GS_OK;
-    kernels[split][degree > 3]<<<(unsigned)div_up64(n, 256), 256, 0, s>>>(degree, stride, n, dirs, coeffs, rest, mask, v_rgb, v_coeffs,
-                                                                          v_rest, v_dirs);
-    B200GS_LAUNCH_CHECK();
-    return B200GS_OK;
+int b200gs_sh_bwd(int32_t degree, int32_t sh_stride, int64_t n, const float* dirs, const float* coeffs, const float* v_rgb,
+                  float* v_coeffs, float* v_dirs, void* stream) {
+    B200GS_CHECK_ARG(degree >= 0 && degree <= 4, "degree must be 0..4");
+    B200GS_CHECK_ARG(sh_stride >= (degree + 1) * (degree + 1), "sh_stride < (degree+1)^2");
+    B200GS_CHECK_ARG(n >= 0, "n < 0");
+    B200GS_CHECK_ARG(n == 0 || (dirs && coeffs && v_rgb && v_coeffs), "NULL pointer");
+    return launch_sh_bwd(degree, sh_stride, n, dirs, coeffs, v_rgb, v_coeffs, v_dirs, (cudaStream_t)stream);
 }
 
-}  // namespace b200gs
+int b200gs_sh_split_fwd(int32_t degree, int32_t k_rest, int64_t n, const float* dirs, const float* dc, const float* rest, const uint8_t* mask,
+                        float* rgb, void* stream) {
+    B200GS_CHECK_ARG(degree >= 0 && degree <= 4, "degree must be 0..4");
+    B200GS_CHECK_ARG(k_rest >= 0 && k_rest + 1 >= (degree + 1) * (degree + 1), "1 + k_rest < (degree+1)^2");
+    B200GS_CHECK_ARG(n >= 0, "n < 0");
+    B200GS_CHECK_ARG(n == 0 || (dirs && dc && rgb && (k_rest == 0 || rest)), "NULL pointer");
+    return launch_sh_fwd(degree, k_rest + 1, n, dirs, dc, rgb, (cudaStream_t)stream, true, rest, mask);
+}
+
+int b200gs_sh_split_bwd(int32_t degree, int32_t k_rest, int64_t n, const float* dirs, const float* dc, const float* rest, const uint8_t* mask,
+                        const float* v_rgb, float* v_dc, float* v_rest, float* v_dirs, void* stream) {
+    B200GS_CHECK_ARG(degree >= 0 && degree <= 4, "degree must be 0..4");
+    B200GS_CHECK_ARG(k_rest >= 0 && k_rest + 1 >= (degree + 1) * (degree + 1), "1 + k_rest < (degree+1)^2");
+    B200GS_CHECK_ARG(n >= 0, "n < 0");
+    B200GS_CHECK_ARG(n == 0 || (dirs && dc && v_rgb && v_dc && (k_rest == 0 || (rest && v_rest))), "NULL pointer");
+    return launch_sh_bwd(degree, k_rest + 1, n, dirs, dc, v_rgb, v_dc, v_dirs, (cudaStream_t)stream, true, rest, mask, v_rest);
+}
+
+}  // extern "C"

@@ -237,14 +237,44 @@ SimLayout sim_bwd_layout(int64_t n, int64_t s, int k, int d) {
     return L;
 }
 
-}  // namespace
-
+// features [N,D] contiguous, idx [S,K] int64, dists [S,K]; kind 0 Cosine, 1 Euclidean
 size_t similarity_reg_workspace_bytes(int64_t n, int64_t s, int k, int d, bool backward) {
     return backward ? sim_bwd_layout(n, s, k, d).total : sim_fwd_bytes(s);
 }
 
-int launch_similarity_reg_fwd(int64_t n, int d, const float* features, int64_t s, int k, const int64_t* idx, const float* dists, int kind,
-                              float decay, float lambda, float* ws, float* out, float* weights, cudaStream_t st) {
+// shared by the similarity entry points; returns the error code, or 0 when the arguments are valid
+int check_similarity(const char* fn, int64_t n, int32_t d, const float* features, int64_t s, int32_t k, const int64_t* idx, const float* dists,
+                     int32_t kind, const void* workspace, size_t workspace_bytes, bool backward) {
+    if (kind != 0 && kind != 1) return fail(fn, "kind must be 0 (Cosine) or 1 (Euclidean)");
+    if (d < 1 || d > 256) return fail(fn, "feature dimension must be 1..256");
+    if (k < 2 || k > 32) return fail(fn, "K must be 2..32");
+    if (s < 1 || n < 1) return fail(fn, "S and N must be >= 1");
+    if (n >= (int64_t(1) << 30) || s * k >= (int64_t(1) << 30)) return fail(fn, "N and S K must be < 2^30");
+    if (!(features && idx && dists && workspace)) return fail(fn, "NULL pointer");
+    if (workspace_bytes < similarity_reg_workspace_bytes(n, s, k, d, backward)) return workspace_too_small(fn);
+    return 0;
+}
+
+}  // namespace
+
+}  // namespace b200gs
+
+using namespace b200gs;
+
+extern "C" {
+
+size_t b200gs_similarity_reg_workspace_bytes(int64_t n, int64_t s, int32_t k, int32_t d, int32_t backward) {
+    const bool ok = n >= 1 && n < (int64_t(1) << 30) && s >= 1 && k >= 2 && k <= 32 && s * k < (int64_t(1) << 30) && d >= 1 && d <= 256;
+    return ok ? similarity_reg_workspace_bytes(n, s, k, d, backward != 0) : 0;
+}
+
+int b200gs_similarity_reg_fwd(int64_t n, int32_t d, const float* features, int64_t s, int32_t k, const int64_t* idx, const float* dists,
+                              int32_t kind, float decay, float lambda, void* workspace, size_t workspace_bytes, float* out, float* weights,
+                              void* stream) {
+    if (int rc = check_similarity(__func__, n, d, features, s, k, idx, dists, kind, workspace, workspace_bytes, false)) return rc;
+    B200GS_CHECK_ARG(out, "NULL pointer");
+    const cudaStream_t st = (cudaStream_t)stream;
+    float* ws = static_cast<float*>(workspace);
     const int wpc = warps_per_cta(k, d, false);
     similarity_fwd_kernel<<<(unsigned)div_up64(s, wpc), wpc * 32, (size_t)wpc * warp_floats(k, d, false) * 4, st>>>(
         n, d, features, s, k, idx, dists, kind == 0, decay, ws, weights);
@@ -254,10 +284,14 @@ int launch_similarity_reg_fwd(int64_t n, int d, const float* features, int64_t s
     return B200GS_OK;
 }
 
-int launch_similarity_reg_bwd(int64_t n, int d, const float* features, int64_t s, int k, const int64_t* idx, const float* dists, int kind,
-                              float decay, float lambda, float* ws, const float* v_loss, float* v_features, cudaStream_t st) {
+int b200gs_similarity_reg_bwd(int64_t n, int32_t d, const float* features, int64_t s, int32_t k, const int64_t* idx, const float* dists,
+                              int32_t kind, float decay, float lambda, void* workspace, size_t workspace_bytes, const float* v_loss,
+                              float* v_features, void* stream) {
+    if (int rc = check_similarity(__func__, n, d, features, s, k, idx, dists, kind, workspace, workspace_bytes, true)) return rc;
+    B200GS_CHECK_ARG(v_loss && v_features, "NULL pointer");
+    const cudaStream_t st = (cudaStream_t)stream;
     const SimLayout L = sim_bwd_layout(n, s, k, d);
-    char* w = (char*)ws;
+    char* w = (char*)workspace;
     const int64_t e = s * k;
     B200GS_CUDA(cudaMemsetAsync(w + L.zero, 0, L.zero_bytes, st));
     const int wpc = warps_per_cta(k, d, true);
@@ -280,4 +314,4 @@ int launch_similarity_reg_bwd(int64_t n, int d, const float* features, int64_t s
     return B200GS_OK;
 }
 
-}  // namespace b200gs
+}  // extern "C"

@@ -287,22 +287,79 @@ __global__ void __launch_bounds__(LT * LT) vis_loss_bwd_kernel(int width, int he
     }
 }
 
-}  // namespace
-
 int64_t uv_grid_params(const B200gsUvGrid& g) { return 2 * int64_t(grid_levels(g).total); }
 
-int launch_uv_grid_fwd(const B200gsUvGrid& grid, int width, int height, const float* uv, int64_t n, const float* const* grids, int n_grids,
-                       const int64_t* id_dev, int64_t id_host, float* enc, cudaStream_t s) {
+bool uv_grid_ok(const B200gsUvGrid* g) {
+    return g && g->n_levels >= 1 && g->n_levels <= 16 && g->base_resolution >= 1 && g->per_level_scale >= 1.f &&
+           std::isfinite(g->per_level_scale) && uv_grid_params(*g) <= INT32_MAX;
+}
+
+// shared by the forward and the backward; returns the error code, or 0 when the arguments are valid
+int check_uv_grid(const char* fn, const B200gsUvGrid* grid, int32_t width, int32_t height, const float* uv, int64_t n) {
+    if (!uv_grid_ok(grid)) return fail(fn, "bad grid: n_levels 1..16, base_resolution >= 1, per_level_scale >= 1");
+    if (uv == nullptr) {
+        if (width < 2 || height < 2) return fail(fn, "the pixel grid needs width and height >= 2 (u = x / (width - 1))");
+        if (int64_t(width) * height > INT32_MAX) return fail(fn, "image too large");
+    } else if (n < 0 || n > INT32_MAX) {
+        return fail(fn, "n out of range");
+    }
+    return 0;
+}
+
+// the grid is (ceil(W/LT), ceil(H/LT), 3): ceil(H/LT) is at most 65535
+bool vis_loss_size_ok(int32_t width, int32_t height) {
+    return width >= 1 && height >= 1 && height <= 65535 * LT && int64_t(width) * height <= INT32_MAX / 4;
+}
+
+int64_t vis_loss_blocks(int width, int height) { return 3 * int64_t(div_up(width, LT)) * div_up(height, LT); }
+
+// the workspace holds the derivative maps, then the per-CTA partials
+size_t vis_loss_workspace_bytes(int width, int height, bool vis_grad) {
+    return (size_t(vis_grad ? 4 : 3) * 3 * size_t(width) * height + 3 * size_t(vis_loss_blocks(width, height))) * sizeof(float);
+}
+
+// shared by the forward and the backward; returns the error code, or 0 when the arguments are valid
+int check_vis_loss(const char* fn, int32_t width, int32_t height, const float* image, const float* gt, const float* visibility,
+                   const void* workspace, size_t workspace_bytes, bool vis_grad) {
+    if (width < 1 || height < 1) return fail(fn, "image size must be >= 1");
+    if (!vis_loss_size_ok(width, height)) return fail(fn, "image too large");
+    if (!(image && gt && visibility && workspace)) return fail(fn, "NULL pointer");
+    if (workspace_bytes < vis_loss_workspace_bytes(width, height, vis_grad)) return workspace_too_small(fn);
+    return 0;
+}
+
+}  // namespace
+
+}  // namespace b200gs
+
+using namespace b200gs;
+
+extern "C" {
+
+int64_t b200gs_uv_grid_params(const B200gsUvGrid* grid) { return uv_grid_ok(grid) ? uv_grid_params(*grid) : 0; }
+
+int b200gs_uv_grid_fwd(const B200gsUvGrid* grid, int32_t width, int32_t height, const float* uv, int64_t n, const float* const* grids,
+                       int32_t n_grids, const int64_t* appearance_id, int64_t host_appearance_id, float* enc, void* stream) {
+    if (int rc = check_uv_grid(__func__, grid, width, height, uv, n)) return rc;
+    B200GS_CHECK_ARG(n_grids >= 1, "n_grids must be >= 1");
+    B200GS_CHECK_ARG(grids && enc, "NULL pointer");
+    B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(enc) & 7u) == 0, "enc must be 8-byte aligned");
     if (!uv) n = int64_t(width) * height;
     if (n == 0) return B200GS_OK;
-    uv_grid_fwd_kernel<<<unsigned(div_up64(n, 256)), 256, 0, s>>>(grid_levels(grid), width, height, uv, n, grids, n_grids, id_dev, id_host, enc);
+    uv_grid_fwd_kernel<<<unsigned(div_up64(n, 256)), 256, 0, (cudaStream_t)stream>>>(grid_levels(*grid), width, height, uv, n, grids, n_grids,
+                                                                                     appearance_id, host_appearance_id, enc);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-int launch_uv_grid_bwd(const B200gsUvGrid& grid, int width, int height, const float* uv, int64_t n, const float* v_enc, float* v_grid,
-                       cudaStream_t s) {
-    const GridLevels g = grid_levels(grid);
+int b200gs_uv_grid_bwd(const B200gsUvGrid* grid, int32_t width, int32_t height, const float* uv, int64_t n, const float* v_enc,
+                       float* v_grid, void* stream) {
+    if (int rc = check_uv_grid(__func__, grid, width, height, uv, n)) return rc;
+    B200GS_CHECK_ARG(v_enc && v_grid, "NULL pointer");
+    B200GS_CHECK_ARG(((reinterpret_cast<uintptr_t>(v_enc) | reinterpret_cast<uintptr_t>(v_grid)) & 7u) == 0,
+                     "v_enc and v_params must be 8-byte aligned");
+    const cudaStream_t s = (cudaStream_t)stream;
+    const GridLevels g = grid_levels(*grid);
     if (uv) {
         B200GS_CUDA(cudaMemsetAsync(v_grid, 0, size_t(g.total) * 2 * sizeof(float), s));
         if (n == 0) return B200GS_OK;
@@ -314,27 +371,35 @@ int launch_uv_grid_bwd(const B200gsUvGrid& grid, int width, int height, const fl
     return B200GS_OK;
 }
 
-int64_t vis_loss_blocks(int width, int height) { return 3 * int64_t(div_up(width, LT)) * div_up(height, LT); }
+int64_t b200gs_vis_loss_blocks(int32_t width, int32_t height) { return vis_loss_size_ok(width, height) ? vis_loss_blocks(width, height) : 0; }
 
-size_t vis_loss_workspace_bytes(int width, int height, bool vis_grad) {
-    return (size_t(vis_grad ? 4 : 3) * 3 * size_t(width) * height + 3 * size_t(vis_loss_blocks(width, height))) * sizeof(float);
+size_t b200gs_vis_loss_workspace_bytes(int32_t width, int32_t height, int32_t vis_grad) {
+    return vis_loss_size_ok(width, height) ? vis_loss_workspace_bytes(width, height, vis_grad != 0) : 0;
 }
 
-int launch_vis_loss_fwd(int width, int height, const float* img, const float* gt, const float* vis, const uint8_t* mask, bool vis_grad,
-                        float* ws, cudaStream_t s) {
+int b200gs_vis_loss_fwd(int32_t width, int32_t height, const float* image, const float* gt, const float* visibility, const uint8_t* mask,
+                        int32_t vis_grad, void* workspace, size_t workspace_bytes, void* stream) {
+    if (int rc = check_vis_loss(__func__, width, height, image, gt, visibility, workspace, workspace_bytes, vis_grad != 0)) return rc;
+    float* ws = static_cast<float*>(workspace);
     const dim3 grid(div_up(width, LT), div_up(height, LT), 3);
     float* partials = ws + size_t(vis_grad ? 4 : 3) * 3 * size_t(width) * height;
-    vis_loss_fwd_kernel<<<grid, LT * LT, 0, s>>>(width, height, img, gt, vis, mask, vis_grad, ws, partials);
+    vis_loss_fwd_kernel<<<grid, LT * LT, 0, (cudaStream_t)stream>>>(width, height, image, gt, visibility, mask, vis_grad != 0, ws, partials);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-int launch_vis_loss_bwd(int width, int height, const float* img, const float* gt, const float* vis, const uint8_t* mask, const float* ws,
-                        float lambda_dssim, float vis_reg_factor, const float* v_loss, float* v_img, float* v_vis, cudaStream_t s) {
+int b200gs_vis_loss_bwd(int32_t width, int32_t height, const float* image, const float* gt, const float* visibility, const uint8_t* mask,
+                        const void* workspace, size_t workspace_bytes, float lambda_dssim, float vis_reg_factor, const float* v_loss,
+                        float* v_image, float* v_visibility, void* stream) {
+    if (int rc = check_vis_loss(__func__, width, height, image, gt, visibility, workspace, workspace_bytes, v_visibility != nullptr))
+        return rc;
+    B200GS_CHECK_ARG(v_image, "NULL v_image");
     const dim3 grid(div_up(width, LT), div_up(height, LT));
-    vis_loss_bwd_kernel<<<grid, LT * LT, 0, s>>>(width, height, img, gt, vis, mask, ws, lambda_dssim, vis_reg_factor, v_loss, v_img, v_vis);
+    vis_loss_bwd_kernel<<<grid, LT * LT, 0, (cudaStream_t)stream>>>(width, height, image, gt, visibility, mask,
+                                                                    static_cast<const float*>(workspace), lambda_dssim, vis_reg_factor,
+                                                                    v_loss, v_image, v_visibility);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
-}  // namespace b200gs
+}  // extern "C"
