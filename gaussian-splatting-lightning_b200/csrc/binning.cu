@@ -991,6 +991,8 @@ int b200gs_bin_count_rows(int32_t mode, int32_t width, int32_t height, int64_t n
     B200GS_CHECK_ARG(width > 0 && height > 0 && n >= 0 && n < (int64_t(1) << 31), "bad size");
     B200GS_CHECK_ARG(workspace && d_counts && (n == 0 || rows), "NULL pointer");
     B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(rows) & 15u) == 0, "rows must be 16-byte aligned");
+    // the count kernel indexes the blocks in int (BinSrc::blk_rows)
+    B200GS_CHECK_ARG(block_counts == nullptr || (block_rows > 0 && block_rows <= INT32_MAX), "block_rows must be 1..2^31-1 with block_counts");
     return bin_count(mode, width, height, n, true, rows + B200GS_ROW_XY, rows + B200GS_ROW_DEPTH, (const int32_t*)(rows + B200GS_ROW_RADIUS),
                      rows + B200GS_ROW_CONIC, rows + B200GS_ROW_OPACITY, workspace, workspace_bytes, d_counts, host_counts, sync_host,
                      (cudaStream_t)stream, block_counts, block_rows);

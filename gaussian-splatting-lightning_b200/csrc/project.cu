@@ -1126,6 +1126,7 @@ int b200gs_project_pack_multi(const B200gsView* views, int32_t n_views, int64_t 
                               size_t workspace_bytes, int64_t* d_count, void* stream) {
     B200GS_CHECK_ARG(views && n_views >= 1 && n_views <= B200GS_MAX_VIEWS, "n_views must be 1..B200GS_MAX_VIEWS");
     B200GS_CHECK_ARG(n >= 0 && n < (int64_t(1) << 30) && cap > 0 && cap < (int64_t(1) << 30), "bad size");
+    B200GS_CHECK_ARG(int64_t(n_views - 1) * cap + cap <= INT32_MAX, "n_views * block_rows exceeds the int32 range of row_index");
     for (int j = 0; j < n_views; ++j) {
         int rc = check_view(views + j, true);
         if (rc) return rc;

@@ -612,6 +612,8 @@ B200GS_API int b200gs_loss_bwd(int32_t channels, int32_t width, int32_t height, 
  *     blend_fwd_rows / blend_bwd_rows read rows (and blend_bwd_rows accumulates into v_rows) with 16-byte accesses: both buffers
  *     must be 16-byte aligned (an allocation base is), or the call fails with B200GS_EINVAL. */
 #define B200GS_MAX_VIEWS 8      /* cameras per multi-view launch / destination ranks per peer-mode pack (one NVSwitch box) */
+/* b200gs_project_pack_multi numbers camera j's rows j*block_rows + k in an int32 row_index: it requires
+ * n_views * block_rows <= 2^31 - 1 (with B200GS_MAX_VIEWS views, block_rows <= 268435455) and returns B200GS_EINVAL otherwise. */
 #define B200GS_ROW_FLOATS 12
 #define B200GS_ROW_XY 0
 #define B200GS_ROW_DEPTH 2
@@ -659,6 +661,8 @@ B200GS_API int b200gs_project_fwd_raw_multi(const B200gsView* views, int32_t n_v
  *     pointers: block of block_rows rows in the receive buffer of the rank that owns camera j — peer memory over NVLink — or in a local
  *     send buffer); rows past block_rows are dropped.  d_count[j] = visible splats of camera j (compare with block_rows).  Kept locally
  *     for K8 and the renderer contract, camera-major ([j*n + i]): xy (mean2D), radii, clamped, row_index (j*block_rows + k, -1 = dropped).
+ *     Sizes: 1 <= n_views <= B200GS_MAX_VIEWS, 0 <= n < 2^30, 1 <= block_rows < 2^30, n_views * block_rows <= 2^31 - 1, dst_rows[j]
+ *     16-byte aligned, workspace_bytes >= b200gs_project_pack_workspace_bytes when n > 0; B200GS_EINVAL otherwise, before any CUDA call.
  *     Replaces b200gs_project_fwd_raw_multi + b200gs_pack_rows (gsplat_distributed_renderer.py:127-217: project, then all-to-all). */
 B200GS_API size_t b200gs_project_pack_workspace_bytes(int32_t n_views, int64_t n);
 B200GS_API int b200gs_project_pack_multi(const B200gsView* views, int32_t n_views, int64_t n, const float* means, const float* log_scales,
@@ -686,7 +690,7 @@ B200GS_API int b200gs_pack_rows(int64_t n, const float* xy, const float* depth, 
  *     argument of b200gs_bin_sort decides whether the tiles are culled.
  * block_counts / block_rows (optional; NULL / 0 = every row counts): the rows arrive in blocks of block_rows rows of which only the first
  *     block_counts[b] are valid (the fixed-capacity exchange of the sharded renderer) — the rest reads as culled, so the receive buffer
- *     needs no padding pass. */
+ *     needs no padding pass.  With block_counts, block_rows must be 1..2^31 - 1 (B200GS_EINVAL otherwise). */
 B200GS_API int b200gs_bin_count_rows(int32_t mode, int32_t width, int32_t height, int64_t n, const float* rows, int32_t cull,
                                      void* workspace_a, size_t workspace_a_bytes, int64_t* d_counts, int64_t* host_counts,
                                      int32_t sync_host, void* stream, const int64_t* block_counts, int64_t block_rows);

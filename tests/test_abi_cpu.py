@@ -73,6 +73,16 @@ def test_argument_validation_without_gpu(lib):
         assert b"aligned" in L.b200gs_last_error()
     assert L.b200gs_bin_count_rows(0, 64, 64, 1, d8, 1, d16, 1 << 20, d16, None, 0, None, None, 0) == -1
     assert b"aligned" in L.b200gs_last_error()
+    # blocked rows: the count kernel indexes the blocks in int
+    for block_rows in (0, -1, 1 << 31):
+        assert L.b200gs_bin_count_rows(0, 64, 64, 1, d16, 1, d16, 1 << 20, d16, None, 0, None, d16, block_rows) == -1
+        assert b"block_rows" in L.b200gs_last_error()
+    # the pack kernel's int32 row_index: n_views * block_rows must stay <= 2^31 - 1
+    views = (lib.B200gsView * 8)()
+    dst = (ctypes.c_void_p * 8)(*[16 * (j + 1) for j in range(8)])
+    for n_views, cap in ((3, (1 << 30) - 1), (8, (1 << 28))):
+        assert L.b200gs_project_pack_multi(views, n_views, 256, *([d16] * 6), 1, *([d16] * 4), dst, cap, d16, 1 << 20, d16, None) == -1
+        assert b"int32" in L.b200gs_last_error()
     # n = 0 is a valid no-op everywhere that takes a count
     v.sh_stride = 16
     assert L.b200gs_project_fwd(ctypes.byref(v), 0, *([None] * 13), None) == 0
