@@ -32,18 +32,30 @@ struct GridLevels {
     int res[UV_MAX_LEVELS], size[UV_MAX_LEVELS], offset[UV_MAX_LEVELS];   // offset in vertices
 };
 
-GridLevels grid_levels(const B200gsUvGrid& g) {
-    GridLevels L{};
+// The level table of g (n_levels 1..16, base_resolution >= 1, per_level_scale >= 1, checked by the caller), or false when the grid
+// cannot be addressed: a scale that is not finite, a grid of more than INT32_MAX floats, or a corner cx + cy res_l (cx, cy <= res_l)
+// past K32/K33's uint32 vertex arithmetic.  The sizes are summed in int64_t: in int, res_l^2 and the total wrap for large grids, and
+// a wrapped total can pass the cap while the size table no longer describes the allocation.
+bool grid_levels(const B200gsUvGrid& g, GridLevels& L) {
+    L = GridLevels{};
     L.n = g.n_levels;
     const float lg = std::log2(g.per_level_scale);
+    int64_t total = 0;
     for (int l = 0; l < g.n_levels; ++l) {
-        L.scale[l] = std::exp2(float(l) * lg) * float(g.base_resolution) - 1.f;
-        L.res[l] = int(std::ceil(L.scale[l])) + 1;
-        L.size[l] = (L.res[l] * L.res[l] + 7) / 8 * 8;
-        L.offset[l] = L.total;
-        L.total += L.size[l];
+        const float scale = std::exp2(float(l) * lg) * float(g.base_resolution) - 1.f;
+        if (!std::isfinite(scale) || scale >= 32768.f) return false;        // res_l^2 alone would pass the float cap
+        const int64_t res = int64_t(std::ceil(scale)) + 1;
+        const int64_t size = (res * res + 7) / 8 * 8;
+        if (res + res * res > int64_t(UINT32_MAX)) return false;            // implied by the cap below; kept as the kernels' bound
+        L.scale[l] = scale;
+        L.res[l] = int(res);
+        L.size[l] = int(size);
+        L.offset[l] = int(total);
+        total += size;
+        if (2 * total > INT32_MAX) return false;
     }
-    return L;
+    L.total = int(total);
+    return true;
 }
 
 // the pixel's coordinate along one axis, as the reference's fp32 arange / (n - 1)
@@ -287,16 +299,16 @@ __global__ void __launch_bounds__(LT * LT) vis_loss_bwd_kernel(int width, int he
     }
 }
 
-int64_t uv_grid_params(const B200gsUvGrid& g) { return 2 * int64_t(grid_levels(g).total); }
-
-bool uv_grid_ok(const B200gsUvGrid* g) {
-    return g && g->n_levels >= 1 && g->n_levels <= 16 && g->base_resolution >= 1 && g->per_level_scale >= 1.f &&
-           std::isfinite(g->per_level_scale) && uv_grid_params(*g) <= INT32_MAX;
+// the level table of a supported grid into L; false for any other
+bool uv_grid_ok(const B200gsUvGrid* g, GridLevels& L) {
+    return g && g->n_levels >= 1 && g->n_levels <= UV_MAX_LEVELS && g->base_resolution >= 1 && g->per_level_scale >= 1.f &&
+           std::isfinite(g->per_level_scale) && grid_levels(*g, L);
 }
 
-// shared by the forward and the backward; returns the error code, or 0 when the arguments are valid
-int check_uv_grid(const char* fn, const B200gsUvGrid* grid, int32_t width, int32_t height, const float* uv, int64_t n) {
-    if (!uv_grid_ok(grid)) return fail(fn, "bad grid: n_levels 1..16, base_resolution >= 1, per_level_scale >= 1");
+// shared by the forward and the backward; returns the error code, or 0 when the arguments are valid and L holds the level table
+int check_uv_grid(const char* fn, const B200gsUvGrid* grid, int32_t width, int32_t height, const float* uv, int64_t n, GridLevels& L) {
+    if (!uv_grid_ok(grid, L))
+        return fail(fn, "bad grid: n_levels 1..16, base_resolution >= 1, per_level_scale >= 1, at most INT32_MAX floats");
     if (uv == nullptr) {
         if (width < 2 || height < 2) return fail(fn, "the pixel grid needs width and height >= 2 (u = x / (width - 1))");
         if (int64_t(width) * height > INT32_MAX) return fail(fn, "image too large");
@@ -336,30 +348,34 @@ using namespace b200gs;
 
 extern "C" {
 
-int64_t b200gs_uv_grid_params(const B200gsUvGrid* grid) { return uv_grid_ok(grid) ? uv_grid_params(*grid) : 0; }
+int64_t b200gs_uv_grid_params(const B200gsUvGrid* grid) {
+    GridLevels g;
+    return uv_grid_ok(grid, g) ? 2 * int64_t(g.total) : 0;
+}
 
 int b200gs_uv_grid_fwd(const B200gsUvGrid* grid, int32_t width, int32_t height, const float* uv, int64_t n, const float* const* grids,
                        int32_t n_grids, const int64_t* appearance_id, int64_t host_appearance_id, float* enc, void* stream) {
-    if (int rc = check_uv_grid(__func__, grid, width, height, uv, n)) return rc;
+    GridLevels g;
+    if (int rc = check_uv_grid(__func__, grid, width, height, uv, n, g)) return rc;
     B200GS_CHECK_ARG(n_grids >= 1, "n_grids must be >= 1");
     B200GS_CHECK_ARG(grids && enc, "NULL pointer");
     B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(enc) & 7u) == 0, "enc must be 8-byte aligned");
     if (!uv) n = int64_t(width) * height;
     if (n == 0) return B200GS_OK;
-    uv_grid_fwd_kernel<<<unsigned(div_up64(n, 256)), 256, 0, (cudaStream_t)stream>>>(grid_levels(*grid), width, height, uv, n, grids, n_grids,
-                                                                                     appearance_id, host_appearance_id, enc);
+    uv_grid_fwd_kernel<<<unsigned(div_up64(n, 256)), 256, 0, (cudaStream_t)stream>>>(g, width, height, uv, n, grids, n_grids, appearance_id,
+                                                                                     host_appearance_id, enc);
     B200GS_LAUNCH_CHECK();
     return B200GS_OK;
 }
 
 int b200gs_uv_grid_bwd(const B200gsUvGrid* grid, int32_t width, int32_t height, const float* uv, int64_t n, const float* v_enc,
                        float* v_grid, void* stream) {
-    if (int rc = check_uv_grid(__func__, grid, width, height, uv, n)) return rc;
+    GridLevels g;
+    if (int rc = check_uv_grid(__func__, grid, width, height, uv, n, g)) return rc;
     B200GS_CHECK_ARG(v_enc && v_grid, "NULL pointer");
     B200GS_CHECK_ARG(((reinterpret_cast<uintptr_t>(v_enc) | reinterpret_cast<uintptr_t>(v_grid)) & 7u) == 0,
                      "v_enc and v_params must be 8-byte aligned");
     const cudaStream_t s = (cudaStream_t)stream;
-    const GridLevels g = grid_levels(*grid);
     if (uv) {
         B200GS_CUDA(cudaMemsetAsync(v_grid, 0, size_t(g.total) * 2 * sizeof(float), s));
         if (n == 0) return B200GS_OK;

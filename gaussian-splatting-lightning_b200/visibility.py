@@ -123,12 +123,21 @@ def _linears(net: _Network):
 
 
 def _dense_grid_floats(n_levels, base_resolution, per_level_scale):
-    """floats of a DenseGrid by tcnn's rule, in Python integers (also for grids too large for the library)"""
+    """floats of a DenseGrid by tcnn's rule, in Python integers (also for grids too large for the library; inf when a scale is
+    not finite).  The scale is fp32, as tcnn and the library compute it: in float64, level 3 of (12, 16, 1.5) has the scale
+    53.00000000000001 instead of 53, which would add a row and a column of vertices."""
     import math
+    import numpy as np
+    f32 = np.float32
+    lg = f32(math.log2(float(f32(per_level_scale))))
     total = 0
-    for l in range(int(n_levels)):
-        res = math.ceil(2.0 ** (l * math.log2(per_level_scale)) * base_resolution - 1) + 1
-        total += (res * res + 7) // 8 * 8
+    with np.errstate(over="ignore"):
+        for l in range(int(n_levels)):
+            scale = f32(f32(np.exp2(np.float64(f32(f32(l) * lg)))) * f32(base_resolution)) - f32(1.0)
+            if not math.isfinite(scale):
+                return math.inf
+            res = math.ceil(float(scale)) + 1
+            total += (res * res + 7) // 8 * 8
     return 2 * total
 
 

@@ -221,7 +221,8 @@ B200GS_API int b200gs_appearance_mlp_bwd(const B200gsAppearanceMlp* mlp, int64_t
  * B200gsUvGrid (host struct): tiny-cuda-nn's 2-D DenseGrid encoding, linear interpolation, 2 features per level:
  *     n_levels 1..16, base_resolution >= 1, per_level_scale >= 1.  Level l: scale_l = exp2f(l log2f(per_level_scale)) base - 1 (fp32,
  *     on the host), res_l = ceil(scale_l) + 1, size_l = res_l^2 rounded up to a multiple of 8 vertices of 2 floats; a grid is the
- *     levels in order (b200gs_uv_grid_params floats; 121760 for 8 / 16 / 1.405).  Coordinate (u, v): pos = fmaf(scale_l, u, 0.5f),
+ *     levels in order (b200gs_uv_grid_params floats; 121760 for 8 / 16 / 1.405; a grid of more than INT32_MAX floats, or with a
+ *     scale that is not finite, is not supported and gives 0).  Coordinate (u, v): pos = fmaf(scale_l, u, 0.5f),
  *     cell = floor(pos), frac = pos - cell per axis; corners k = 0..3 (bit 0: x) with weight (frac or 1 - frac in x) * (.. in y) at
  *     vertex ((cell_x + k&1) + (cell_y + k>>1) res_l) % size_l; enc[row, 2 l + f] = the weighted sum in corner order.
  * b200gs_uv_grid_fwd: enc float[n, 2 n_levels] (8-byte aligned).  uv NULL: the pixel grid of one image, n = width * height rows in

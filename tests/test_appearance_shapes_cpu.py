@@ -98,6 +98,31 @@ def test_restated_layout_is_the_accept_set_and_the_workspace(L):
     assert n_ok > 0 and pairs == {(8, 8), (8, 4), (4, 4), (4, 2), (2, 2), (2, 1), (1, 1)}
 
 
+def visibility_accepted(feat_dim, n_neurons, n_layers):
+    """the visibility network: an appearance network with no view direction and one output, on 8, 16, 24 or 32 grid features"""
+    return feat_dim in (8, 16, 24, 32) and n_neurons in (64, 128) and 2 <= n_layers <= 4 and warps_of((feat_dim, -1, n_neurons, n_layers, 1), True) > 0
+
+
+VISIBILITY_GRID = [(f, h, l) for f in range(0, 49, 4) for h in (32, 64, 96, 128) for l in range(1, 6)]
+
+
+def test_restated_layout_is_the_visibility_accept_set_and_workspace(L):
+    """the one-output layout keeps the output layer as 8 rows, so its tiles are those of the same network with 3 or 4 outputs; the
+    workspace holds the one-output parameter count per persistent CTA"""
+    n_ok = 0
+    for f, h, l in VISIBILITY_GRID:
+        got = int(L.b200gs_visibility_mlp_workspace_bytes(f, h, l))
+        if visibility_accepted(f, h, l):
+            s = (f, -1, h, l, 1)
+            assert got == MAX_CTAS * n_params(*s) * 4, s
+            assert launch(s, False) == launch((f, -1, h, l, 3), False) and launch(s, True) == launch((f, -1, h, l, 3), True), s
+            assert warps_of(s, False) >= warps_of(s, True) > 0, s
+            n_ok += 1
+        else:
+            assert got == 0, (f, h, l)
+    assert n_ok == 4 * 2 * 3
+
+
 def test_restated_layout_examples():
     """the warp counts the kernels' comments and DESIGN.md quote, and the widest accepted first layers"""
     assert (warps_of((64, -1, 64, 3, 3), False), warps_of((64, -1, 64, 3, 3), True)) == (8, 8)

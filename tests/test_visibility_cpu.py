@@ -81,6 +81,79 @@ def test_uv_grid_entry_points_validate_before_any_cuda_call(L):
     assert L.b200gs_uv_grid_bwd(g, 8, 8, None, 0, None, D, None) != 0
 
 
+# grids whose float count overflows int: (2, 46341, 1.0) and (2, 1, 70000.0) hold about 8.6e9 and 9.8e9 floats, (1, 46341, 1.0)
+# 4.3e9; summed in int their counts wrap to 18,560, 1,210,345,440 and a negative number.  Then a per_level_scale whose level-1 scale
+# is infinite in fp32.
+OVERFLOW = [(2, 46341, 1.0), (2, 1, 70000.0), (1, 46341, 1.0), (2, 16, 3e38), (16, 16, 2.0)]
+
+# the grid configurations the GPU boundary tests sweep (tests/test_gpu_visibility_boundaries.py), with the levels whose last pixel
+# column and row reach corner res_l and wrap through the %: the fp32 scale has a fractional part >= 0.5, or none
+SWEEP_WRAPS = {
+    (4, 16, 1.405): [0, 2],
+    (8, 16, 1.405): [0, 2, 5, 7],
+    (12, 16, 1.405): [0, 2, 5, 7, 8, 10, 11],
+    (16, 16, 1.405): [0, 2, 5, 7, 8, 10, 11, 12, 14, 15],
+    (8, 16, 2.0): list(range(8)),
+    (8, 1, 2.0): list(range(8)),
+    (4, 1, 1.5): [0, 1],
+    (12, 16, 1.5): [0, 1, 2, 3, 4, 10, 11],
+    (16, 4, 1.5): [0, 1, 2, 3, 6, 8, 9, 10, 11, 12, 14, 15],
+}
+
+
+@pytest.mark.parametrize("cfg", OVERFLOW)
+def test_grids_past_the_float_cap_are_refused(L, cfg):
+    from b200gs import _lib
+    from b200gs.visibility import UVGridEncoding, _dense_grid_floats
+    g = ctypes.byref(_lib.B200gsUvGrid(*cfg))
+    assert L.b200gs_uv_grid_params(g) == 0
+    assert _dense_grid_floats(*cfg) > 2 ** 31 - 1
+    # both entry points, on the pixel grid and on given coordinates, refuse it before any CUDA call (D is never dereferenced)
+    assert L.b200gs_uv_grid_fwd(g, 8, 8, None, 0, D, 1, None, 0, D, None) != 0
+    assert L.b200gs_uv_grid_fwd(g, 0, 0, D, 4, D, 1, None, 0, D, None) != 0
+    assert L.b200gs_uv_grid_bwd(g, 8, 8, None, 0, D, D, None) != 0
+    assert L.b200gs_uv_grid_bwd(g, 0, 0, D, 4, D, D, None) != 0
+    with pytest.raises(NotImplementedError, match="at most 2"):
+        UVGridEncoding(*cfg)
+
+
+def test_grid_just_under_the_float_cap_is_counted_exactly(L):
+    """one level of res 32767 holds 2 * 1,073,676,296 = 2,147,352,592 floats, under INT32_MAX; res 32768 is over it"""
+    from b200gs import _lib
+    assert L.b200gs_uv_grid_params(ctypes.byref(_lib.B200gsUvGrid(1, 32767, 1.0))) == 2 * ((32767 * 32767 + 7) // 8 * 8) == V.n_params(1, 32767, 1.0)
+    assert L.b200gs_uv_grid_params(ctypes.byref(_lib.B200gsUvGrid(1, 32768, 1.0))) == 0
+
+
+@pytest.mark.parametrize("cfg", list(SWEEP_WRAPS), ids=str)
+def test_sweep_grid_sizes_agree(L, cfg):
+    from b200gs import _lib, ops
+    from b200gs.visibility import _dense_grid_floats
+    n = L.b200gs_uv_grid_params(ctypes.byref(_lib.B200gsUvGrid(*cfg)))
+    assert n > 0 and n == V.n_params(*cfg) == _dense_grid_floats(*cfg) == ops.uv_grid_params(*cfg)
+
+
+@pytest.mark.parametrize("cfg", list(SWEEP_WRAPS), ids=str)
+def test_wrapping_levels(cfg):
+    lv = V.levels(*cfg)
+    frac_wraps = [l for l, (s, _, _, _) in enumerate(lv) if float(s) - np.floor(float(s)) >= 0.5 or float(s) == np.floor(float(s))]
+    last_wraps = [l for l, (s, res, _, _) in enumerate(lv) if int(np.floor(np.float32(s) + np.float32(0.5))) + 1 == res]
+    assert frac_wraps == last_wraps == SWEEP_WRAPS[cfg]
+
+
+def test_wrapping_levels_near_a_half():
+    """fp32 scales two ulp under a half do not wrap although exact arithmetic would; an exact half and an integer do"""
+    under = lambda x: float(np.float32(x) - 2 * np.spacing(np.float32(x)))
+    s = [float(x[0]) for x in V.levels(12, 16, 1.5)]
+    assert s[5] == under(120.5) == 120.49998474121094 and 5 not in SWEEP_WRAPS[(12, 16, 1.5)]
+    s = [float(x[0]) for x in V.levels(16, 4, 1.5)]
+    assert s[3] == 12.5 and 3 in SWEEP_WRAPS[(16, 4, 1.5)]
+    assert s[5] == under(29.375) and 5 not in SWEEP_WRAPS[(16, 4, 1.5)]
+    lv = V.levels(8, 1, 2.0)
+    assert (float(lv[0][0]), lv[0][1], lv[0][2]) == (0.0, 1, 8)           # every pixel in one cell with frac 0.5
+    assert [float(x[0]) for x in V.levels(8, 16, 2.0)] == [16.0 * 2 ** l - 1 for l in range(8)]
+    assert V.levels(8, 16, 1.405)[0][0] == 15.0 and abs(float(V.levels(8, 16, 1.405)[1][0]) % 1 - 0.48) < 1e-5
+
+
 def mlp(feat=16, n_freq=-1, neurons=64, layers=3, n_out=1, flags=(0, 0, 0), null_weight=False):
     from b200gs import _lib
     m = _lib.B200gsAppearanceMlp(feat, n_freq, neurons, layers, n_out, *flags, feat + 128, feat + 128)
