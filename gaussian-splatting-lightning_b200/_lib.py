@@ -38,6 +38,11 @@ class B200gsUvGrid(ctypes.Structure):
     _fields_ = [("n_levels", c_int32), ("base_resolution", c_int32), ("per_level_scale", c_float)]
 
 
+class B200gsHashGrid(ctypes.Structure):
+    _fields_ = [("n_levels", c_int32), ("n_features_per_level", c_int32), ("log2_hashmap_size", c_int32), ("base_resolution", c_int32),
+                ("per_level_scale", c_float)]
+
+
 class B200gsError(RuntimeError):
     pass
 
@@ -98,6 +103,14 @@ _SIGNATURES = {
     "b200gs_similarity_reg_bwd": (c_int32, [c_int64, c_int32, _P, c_int64, c_int32, _P, _P, c_int32, c_float, c_float, _P, c_size_t, _P, _P, _P]),
     "b200gs_glossy_sh_fwd": (c_int32, [c_int32, c_int64, _P, _P, _P, _P, c_int32, _P, _P, c_int32, c_int32, _P, _P, _P, _P, _P]),
     "b200gs_glossy_sh_bwd": (c_int32, [c_int32, c_int64, _P, _P, c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "b200gs_hash_grid_params": (c_int64, [POINTER(B200gsHashGrid)]),
+    "b200gs_swag_inputs_fwd": (c_int32, [POINTER(B200gsHashGrid), c_int32, c_int64] + [_P] * 4 + [c_int32, c_int32] + [_P, _P, c_int32, _P, _P, _P]),
+    "b200gs_swag_inputs_bwd": (c_int32, [POINTER(B200gsHashGrid), c_int32, c_int64] + [_P] * 4 + [c_int32, c_int32] + [_P, _P, _P, c_int32]
+                               + [_P] * 4 + [_P]),
+    "b200gs_swag_mlp_workspace_bytes": (c_size_t, [c_int32] * 3),
+    "b200gs_swag_mlp_fwd": (c_int32, [POINTER(B200gsAppearanceMlp), c_int32, c_int64, _P, _P, _P, c_float, c_float, _P, _P, _P]),
+    "b200gs_swag_mlp_bwd": (c_int32, [POINTER(B200gsAppearanceMlp), c_int32, c_int64, _P, _P, _P, c_float, c_float] + [_P] * 5
+                            + [c_size_t, _P, _P]),
     "b200gs_sh_fwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P]),
     "b200gs_sh_bwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P, _P, _P]),
     "b200gs_sh_split_fwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P, _P, _P]),

@@ -80,7 +80,8 @@ def install(force: bool = False):
         sys.modules["fused_ssim"] = _fused_ssim_module()
     elif "fused_ssim" not in sys.modules and not any(isinstance(f, _OnImport) and f.name == "fused_ssim" for f in sys.meta_path):
         sys.meta_path.insert(0, _OnImport("fused_ssim", _fused_ssim_module))
-    # tinycudann.Encoding, 2-D DenseGrid only (gsplat_appearance_embedding_visibility_map_renderer.py:4,114-124), the same way
+    # tinycudann.Encoding, 2-D DenseGrid (gsplat_appearance_embedding_visibility_map_renderer.py:4,114-124) and 3-D HashGrid
+    # (swag_model.py:82-86), the same way
     if force:
         sys.modules["tinycudann"] = _tcnn_module()
     elif "tinycudann" not in sys.modules and not any(isinstance(f, _OnImport) and f.name == "tinycudann" for f in sys.meta_path):
@@ -169,8 +170,18 @@ def _tcnn_module():
     from ..visibility import UVGridEncoding
 
     class Encoding(UVGridEncoding):
-        """tinycudann.Encoding for n_input_dims 2 and otype DenseGrid with linear interpolation and 2 features per level, on K32/K33;
-        anything else raises.  The initial values are uniform(-1e-4, 1e-4) from torch's generator, not tcnn's pcg32 stream."""
+        """tinycudann.Encoding for n_input_dims 2 and otype DenseGrid with linear interpolation and 2 features per level, on K32/K33,
+        and for n_input_dims 3 and otype HashGrid (swag.HashGridEncoding, K49/K50; the grids swag.grid_kwargs accepts); anything
+        else raises.  The initial values are uniform(-1e-4, 1e-4) from torch's generator, not tcnn's pcg32 stream, and a hash grid
+        is float32, not half."""
+
+        def __new__(cls, n_input_dims, encoding_config, seed=1337, dtype=None):
+            if n_input_dims == 3 and str(dict(encoding_config).get("otype", "")).lower() == "hashgrid":
+                from ..swag import HashGridEncoding
+                if dtype not in (None, torch.float32):
+                    raise NotImplementedError(f"b200gs provides tinycudann.Encoding for float32 grids only, got dtype={dtype}")
+                return HashGridEncoding(encoding_config)       # not an Encoding: __init__ below is not called
+            return super().__new__(cls)
 
         def __init__(self, n_input_dims, encoding_config, seed=1337, dtype=None):
             c = dict(encoding_config)
@@ -183,7 +194,7 @@ def _tcnn_module():
 
     def refuse(name):
         def init(self, *args, **kwargs):
-            raise NotImplementedError(f"b200gs provides no tinycudann.{name}: only Encoding with a 2-D DenseGrid")
+            raise NotImplementedError(f"b200gs provides no tinycudann.{name}: only Encoding with a 2-D DenseGrid or a 3-D HashGrid")
         return type(name, (), {"__init__": init})
 
     m = types.ModuleType("tinycudann")

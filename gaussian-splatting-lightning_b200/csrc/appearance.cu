@@ -18,7 +18,13 @@
 //     the order of every sum is fixed), the bias gradient as column sums, and each warp's dh_{l-1} = dpre_l W_l, masked by
 //     the ReLU, in place over h_{l-1}.  The last step writes v_features (through the normalisation Jacobian when on).
 //   * K22 appearance_reduce_kernel adds the CTAs' partial blocks in block order.
+// Epilogue 2 is SWAG's (swag_renderer.py:47-56; the rows come from K49, swag.cu): no output activation on o_3, and
+//     colour = sigmoid(o_{0..2}),  z = (1 / temperature) ((log(|o_3| + eps) + log(u + eps)) - log(1 - u + eps)),
+//     opacity = clamp_min(base_opacity - sigmoid(z), 0)
+// with u read through a device pointer.  Only W_0's first w0_cols columns are read, the rest of its first F are zero: SWAG's rows are
+// 35 real columns padded to 40, and the caller's W_0 has the image embedding in columns 35..58.
 #include <algorithm>
+#include <cmath>
 
 #include "common.cuh"
 
@@ -79,7 +85,8 @@ struct AppParams {
     int normalize, normalize_dirs, epilogue;
     const float* features; const uint8_t* mask; const float* base_rgb; const float* dirs; const float* cam; const float* raw_opacity;
     const float* W[APP_MAX_LAYERS]; const float* b[APP_MAX_LAYERS];
-    int w0_stride, w0_pe_col;
+    int w0_stride, w0_pe_col, w0_cols;
+    const float* u; float inv_temp, eps;                                                    // epilogue 2
     float* out; float* opacity_offsets; float* opacities;                                   // forward
     const float* v_out; const float* v_opacities; const float* v_opacity_offsets;           // backward
     float* v_base_rgb; float* v_features; float* v_raw_opacity; float* partials;
@@ -179,7 +186,7 @@ __device__ void load_weights(const AppParams& p, const AppLayout& lay, float* sm
             float v = 0.f;
             if (r < real && c < in) {
                 if (l == 0) {
-                    if (c < s.F) v = __ldg(p.W[0] + int64_t(r) * p.w0_stride + c);
+                    if (c < s.F) v = c < p.w0_cols ? __ldg(p.W[0] + int64_t(r) * p.w0_stride + c) : 0.f;
                     else if (c < s.F + s.pe()) v = __ldg(p.W[0] + int64_t(r) * p.w0_stride + p.w0_pe_col + (c - s.F));
                 } else {
                     v = __ldg(p.W[l] + r * in + c);
@@ -276,16 +283,22 @@ __device__ int hidden_layers(const Tile& T) {
     return prev;
 }
 
-// sigmoid outputs of this warp's rows: z[0..1] = channels 2t, 2t+1 of row g, z[2..3] of row g + 8
-__device__ __forceinline__ void output_layer(const Tile& T, int hbuf, float (&sg)[4]) {
+// output pre-activations of this warp's rows: z[0..1] = channels 2t, 2t+1 of row g, z[2..3] of row g + 8
+__device__ __forceinline__ void output_layer(const Tile& T, int hbuf, float (&z)[4]) {
     const AppShape& s = T.p.s;
     const int t = T.lane & 3, l = s.L - 1, SH = s.H + 4;
     float acc[1][4];
     zero_acc(acc);
     warp_gemm<false>(T.Hb(hbuf) + T.warp * 16 * SH, SH, s.H, T.sm + T.lay.W[l], SH, 0, 1, acc, T.lane);
     const float b0 = T.sm[T.lay.b[l] + 2 * t], b1 = T.sm[T.lay.b[l] + 2 * t + 1];
-    sg[0] = sigmoidf(acc[0][0] + b0); sg[1] = sigmoidf(acc[0][1] + b1);
-    sg[2] = sigmoidf(acc[0][2] + b0); sg[3] = sigmoidf(acc[0][3] + b1);
+    z[0] = acc[0][0] + b0; z[1] = acc[0][1] + b1;
+    z[2] = acc[0][2] + b0; z[3] = acc[0][3] + b1;
+}
+
+// epilogue 2: sigmoid(z) of the Gumbel-sigmoid opacity term for output o_3 = o
+__device__ __forceinline__ float swag_sigmoid_z(const AppParams& p, float o) {
+    const float u = __ldg(p.u);
+    return sigmoidf(p.inv_temp * ((logf(fabsf(o) + p.eps) + logf(u + p.eps)) - logf(1.f - u + p.eps)));
 }
 
 // Append the visible rows of chunk [base, base + blockDim.x) to the ring; returns how many.  `vis` tells the caller whether this
@@ -322,8 +335,8 @@ __device__ void fwd_tile(const Tile& T, int head, int count) {
     tile_rows(T, head, count);
     load_inputs(T);
     const int hb = hidden_layers<true>(T);
-    float sg[4];
-    output_layer(T, hb, sg);
+    float zo[4];
+    output_layer(T, hb, zo);
     const int g = T.lane >> 2, t = T.lane & 3;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -332,9 +345,16 @@ __device__ void fwd_tile(const Tile& T, int head, int count) {
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
             const int c = 2 * t + e;
-            const float v = sg[2 * h + e];
+            const float v = sigmoidf(zo[2 * h + e]);
             if (c >= s.O) continue;
-            if (!p.epilogue) {
+            if (p.epilogue == 2) {
+                if (c < 3) {
+                    p.out[int64_t(row) * 3 + c] = v;
+                } else {
+                    const float o = __ldg(p.raw_opacity + row) - swag_sigmoid_z(p, zo[2 * h + e]);
+                    p.opacities[row] = o < 0.f ? 0.f : o;           // NaN stays NaN, as in torch.clamp_min
+                }
+            } else if (!p.epilogue) {
                 p.out[int64_t(row) * s.O + c] = v;
             } else if (c < 3) {
                 const float base = __ldg(p.base_rgb + int64_t(row) * 3 + c) + 0.5f;
@@ -430,8 +450,8 @@ __device__ void bwd_tile(const Tile& T, int head, int count, float* partial) {
     tile_rows(T, head, count);
     load_inputs(T);
     const int hb = hidden_layers<false>(T);
-    float sg[4];
-    output_layer(T, hb, sg);
+    float zo[4];
+    output_layer(T, hb, zo);
     // the epilogue's gradient: dz of this thread's two channels of rows g and g + 8
     float* DZ = T.sm + T.lay.DZ;
 #pragma unroll
@@ -440,9 +460,19 @@ __device__ void bwd_tile(const Tile& T, int head, int count, float* partial) {
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
             const int c = 2 * t + e;
-            const float v = sg[2 * h + e];
-            float ds = 0.f;
-            if (row >= 0 && c < s.O) {
+            const float v = sigmoidf(zo[2 * h + e]);
+            float ds = 0.f, dz_raw = 0.f;
+            if (row >= 0 && c < s.O && p.epilogue == 2) {
+                if (c < 3) {
+                    ds = __ldg(p.v_out + int64_t(row) * 3 + c);
+                } else {        // o_3 has no activation: its gradient goes to DZ as it is
+                    const float o = zo[2 * h + e], sz = swag_sigmoid_z(p, o);
+                    const float gb = (__ldg(p.raw_opacity + row) - sz >= 0.f && p.v_opacities) ? __ldg(p.v_opacities + row) : 0.f;
+                    p.v_raw_opacity[row] = gb;
+                    const float ga = -gb * (sz * (1.f - sz)) * p.inv_temp / (fabsf(o) + p.eps);
+                    dz_raw = o > 0.f ? ga : (o < 0.f ? -ga : 0.f);
+                }
+            } else if (row >= 0 && c < s.O) {
                 if (!p.epilogue) {
                     ds = __ldg(p.v_out + int64_t(row) * s.O + c);
                 } else if (c < 3) {
@@ -457,7 +487,7 @@ __device__ void bwd_tile(const Tile& T, int head, int count, float* partial) {
                     ds = go + (p.v_opacity_offsets ? __ldg(p.v_opacity_offsets + row) : 0.f);
                 }
             }
-            DZ[r * 12 + c] = ds * v * (1.f - v);
+            DZ[r * 12 + c] = (p.epilogue == 2 && c == 3) ? dz_raw : ds * v * (1.f - v);
         }
     }
     __syncthreads();
@@ -577,11 +607,24 @@ AppParams app_params(const B200gsAppearanceMlp& m, int64_t n, const float* featu
     AppParams p{};
     p.s = AppShape{m.feat_dim, m.n_freq, m.n_neurons, m.n_layers, m.n_out};
     p.n = n;
-    p.normalize = m.normalize; p.normalize_dirs = m.normalize_dirs; p.epilogue = m.epilogue;
+    p.normalize = m.normalize; p.normalize_dirs = m.normalize_dirs; p.epilogue = m.epilogue ? 1 : 0;
     p.features = features; p.mask = mask; p.base_rgb = base_rgb; p.dirs = dirs; p.cam = cam; p.raw_opacity = raw_opacity;
     for (int l = 0; l < m.n_layers; ++l) { p.W[l] = m.weights[l]; p.b[l] = m.biases[l]; }
-    p.w0_stride = m.w0_stride; p.w0_pe_col = m.w0_pe_col;
+    p.w0_stride = m.w0_stride; p.w0_pe_col = m.w0_pe_col; p.w0_cols = m.feat_dim;
     return p;
+}
+
+// SWAG's epilogue (2) and the real width of its padded rows
+struct SwagEpilogue {
+    int in_dim;
+    const float* u;
+    float inv_temp, eps;
+};
+
+void set_swag(AppParams& p, const SwagEpilogue* e) {
+    if (e == nullptr) return;
+    p.epilogue = 2;
+    p.w0_cols = e->in_dim; p.u = e->u; p.inv_temp = e->inv_temp; p.eps = e->eps;
 }
 
 template <typename K>
@@ -601,8 +644,9 @@ int app_launch(K kernel, const AppParams& p, bool bwd, int* grid_out, cudaStream
 // epilogue.  The shape of m has been validated.
 int launch_appearance_mlp_fwd(const B200gsAppearanceMlp& m, int64_t n, const float* features, const uint8_t* mask, const float* base_rgb,
                               const float* dirs, const float* cam, const float* raw_opacity, float* out, float* opacity_offsets,
-                              float* opacities, cudaStream_t s) {
+                              float* opacities, cudaStream_t s, const SwagEpilogue* swag = nullptr) {
     AppParams p = app_params(m, n, features, mask, base_rgb, dirs, cam, raw_opacity);
+    set_swag(p, swag);
     p.out = out; p.opacity_offsets = opacity_offsets; p.opacities = opacities;
     int grid;
     return n > 0 ? app_launch(appearance_mlp_fwd_kernel, p, false, &grid, s) : B200GS_OK;
@@ -611,8 +655,9 @@ int launch_appearance_mlp_fwd(const B200gsAppearanceMlp& m, int64_t n, const flo
 int launch_appearance_mlp_bwd(const B200gsAppearanceMlp& m, int64_t n, const float* features, const uint8_t* mask, const float* base_rgb,
                               const float* dirs, const float* cam, const float* raw_opacity, const float* v_out, const float* v_opacities,
                               const float* v_opacity_offsets, float* v_base_rgb, float* v_features, float* v_raw_opacity, float* workspace,
-                              float* v_params, cudaStream_t s) {
+                              float* v_params, cudaStream_t s, const SwagEpilogue* swag = nullptr) {
     AppParams p = app_params(m, n, features, mask, base_rgb, dirs, cam, raw_opacity);
+    set_swag(p, swag);
     p.v_out = v_out; p.v_opacities = v_opacities; p.v_opacity_offsets = v_opacity_offsets;
     p.v_base_rgb = v_base_rgb; p.v_features = v_features; p.v_raw_opacity = v_raw_opacity; p.partials = workspace;
     int grid = 0;
@@ -668,6 +713,29 @@ int check_visibility(const char* fn, const B200gsAppearanceMlp* m, int64_t n, co
     for (int l = 0; l < m->n_layers; ++l)
         if (!m->weights[l] || !m->biases[l]) return fail(fn, "NULL weight or bias pointer");
     if (n > 0 && !enc) return fail(fn, "NULL enc");
+    return B200GS_OK;
+}
+
+bool swag_shape_ok(int32_t feat_dim, int32_t n_neurons, int32_t n_layers) {
+    return feat_dim >= 8 && feat_dim % 8 == 0 && feat_dim <= 1024 && (n_neurons == 64 || n_neurons == 128) && n_layers >= 2 &&
+           n_layers <= B200GS_APPEARANCE_MAX_LAYERS && appearance_mlp_fits(feat_dim, -1, n_neurons, n_layers, 4);
+}
+
+int check_swag(const char* fn, const B200gsAppearanceMlp* m, int32_t in_dim, int64_t n, const float* x0, const float* base_opacity,
+               const float* u, float temperature, float eps) {
+    if (m == nullptr) return fail(fn, "mlp is NULL");
+    if (m->n_freq != -1 || m->n_out != 4 || m->normalize || m->normalize_dirs || m->epilogue != 2)
+        return fail(fn, "a SWAG network has n_freq -1, n_out 4, no normalisation and epilogue 2");
+    if (!swag_shape_ok(m->feat_dim, m->n_neurons, m->n_layers))
+        return fail(fn, "feat_dim must be a positive multiple of 8 that fits shared memory, n_neurons 64 or 128, n_layers 2..4");
+    if (in_dim > m->feat_dim || in_dim <= m->feat_dim - 8) return fail(fn, "in_dim must satisfy feat_dim - 8 < in_dim <= feat_dim");
+    if (m->w0_stride < in_dim) return fail(fn, "w0_stride < in_dim");
+    if (!(temperature > 0.f) || !std::isfinite(temperature) || !(eps >= 0.f) || !std::isfinite(eps))
+        return fail(fn, "temperature must be positive and eps non-negative, both finite");
+    if (n < 0 || n > INT32_MAX) return fail(fn, "n out of range");
+    for (int l = 0; l < m->n_layers; ++l)
+        if (!m->weights[l] || !m->biases[l]) return fail(fn, "NULL weight or bias pointer");
+    if (n > 0 && !(x0 && base_opacity && u)) return fail(fn, "NULL x0, base_opacity or u");
     return B200GS_OK;
 }
 
@@ -731,6 +799,34 @@ int b200gs_visibility_mlp_bwd(const B200gsAppearanceMlp* mlp, int64_t n, const f
         return workspace_too_small(__func__);
     return launch_appearance_mlp_bwd(*mlp, n, enc, nullptr, nullptr, nullptr, nullptr, nullptr, v_out, nullptr, nullptr, nullptr, v_enc,
                                      nullptr, static_cast<float*>(workspace), v_params, (cudaStream_t)stream);
+}
+
+size_t b200gs_swag_mlp_workspace_bytes(int32_t feat_dim, int32_t n_neurons, int32_t n_layers) {
+    if (!swag_shape_ok(feat_dim, n_neurons, n_layers)) return 0;
+    return appearance_mlp_workspace_bytes(feat_dim, -1, n_neurons, n_layers, 4);
+}
+
+int b200gs_swag_mlp_fwd(const B200gsAppearanceMlp* mlp, int32_t in_dim, int64_t n, const float* x0, const float* base_opacity, const float* u,
+                        float temperature, float eps, float* colour, float* opacity, void* stream) {
+    if (int rc = check_swag(__func__, mlp, in_dim, n, x0, base_opacity, u, temperature, eps)) return rc;
+    B200GS_CHECK_ARG(n == 0 || (colour && opacity), "NULL colour or opacity");
+    const SwagEpilogue e{in_dim, u, float(1.0 / double(temperature)), eps};
+    return launch_appearance_mlp_fwd(*mlp, n, x0, nullptr, nullptr, nullptr, nullptr, base_opacity, colour, nullptr, opacity,
+                                     (cudaStream_t)stream, &e);
+}
+
+int b200gs_swag_mlp_bwd(const B200gsAppearanceMlp* mlp, int32_t in_dim, int64_t n, const float* x0, const float* base_opacity, const float* u,
+                        float temperature, float eps, const float* v_colour, const float* v_opacity, float* v_x0, float* v_base_opacity,
+                        void* workspace, size_t workspace_bytes, float* v_params, void* stream) {
+    if (int rc = check_swag(__func__, mlp, in_dim, n, x0, base_opacity, u, temperature, eps)) return rc;
+    B200GS_CHECK_ARG(v_params, "NULL v_params");
+    B200GS_CHECK_ARG(n == 0 || (v_colour && v_base_opacity && workspace), "NULL v_colour, v_base_opacity or workspace");
+    B200GS_CHECK_ARG((reinterpret_cast<uintptr_t>(v_x0) & 15u) == 0, "v_x0 must be 16-byte aligned");
+    if (n > 0 && workspace_bytes < appearance_mlp_workspace_bytes(mlp->feat_dim, -1, mlp->n_neurons, mlp->n_layers, 4))
+        return workspace_too_small(__func__);
+    const SwagEpilogue e{in_dim, u, float(1.0 / double(temperature)), eps};
+    return launch_appearance_mlp_bwd(*mlp, n, x0, nullptr, nullptr, nullptr, nullptr, base_opacity, v_colour, v_opacity, nullptr, nullptr,
+                                     v_x0, v_base_opacity, static_cast<float*>(workspace), v_params, (cudaStream_t)stream, &e);
 }
 
 }  // extern "C"

@@ -1400,3 +1400,192 @@ def visibility_l1_ssim_loss(image, gt, visibility, mask=None, lambda_dssim: floa
             raise ValueError(f"mask must be bool or uint8 [H,W] on the image's device, got {mask.dtype} {tuple(mask.shape)}")
         mask = (mask != 0).contiguous().view(torch.uint8)
     return _VisibilityLoss.apply(image, gt, vis, mask, float(lambda_dssim), float(vis_reg_factor))
+
+
+# ---- SWAG in-the-wild appearance (csrc/swag.cu K49/K50; the MLP runs on the appearance kernels with epilogue 2) -------------------
+HASH_GRID_FWD_LAUNCHES = 1      # library launches of one hash_grid_encode forward (K49 without colour)
+HASH_GRID_BWD_LAUNCHES = 1      # and of its backward (K50; the table gradient is zeroed with a memset)
+SWAG_FWD_LAUNCHES = 2           # swag_colours_and_opacities forward: K49, K20
+SWAG_BWD_LAUNCHES = 3           # and backward: K21, K22, K50
+HASH_GRID_DEFAULTS = dict(n_levels=8, n_features_per_level=4, log2_hashmap_size=19, base_resolution=16, per_level_scale=2.0)
+HASH_GRID_SUPPORTED = ("n_levels 1..16, n_features_per_level 2 or 4, log2_hashmap_size 1..24, base_resolution >= 1 and "
+                       "per_level_scale >= 1 (every level's scale below 2^30)")
+
+
+def _hash_grid(n_levels=8, n_features_per_level=4, log2_hashmap_size=19, base_resolution=16, per_level_scale=2.0) -> _lib.B200gsHashGrid:
+    return _lib.B200gsHashGrid(int(n_levels), int(n_features_per_level), int(log2_hashmap_size), int(base_resolution),
+                               float(per_level_scale))
+
+
+def hash_grid_params(**grid) -> int:
+    """Floats of one 3-D hash grid (tiny-cuda-nn's ``n_params``; 11681792 for the defaults), 0 when the grid is not supported."""
+    return int(lib().b200gs_hash_grid_params(ctypes.byref(_hash_grid(**grid))))
+
+
+def _check_table(table: torch.Tensor, grid: _lib.B200gsHashGrid) -> int:
+    n = int(lib().b200gs_hash_grid_params(ctypes.byref(grid)))
+    if n == 0:
+        raise NotImplementedError(f"b200gs HashGrid supports {HASH_GRID_SUPPORTED}")
+    if table.dtype != torch.float32 or not table.is_cuda or not table.is_contiguous() or table.numel() != n:
+        raise ValueError(f"the grid table must be a contiguous float32 CUDA tensor of {n} floats")
+    return n
+
+
+class _HashGridEncode(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, grid, table, x):
+        n, width = x.shape[0], grid.n_levels * grid.n_features_per_level
+        enc = torch.empty(n, width, dtype=torch.float32, device=x.device)
+        check(lib().b200gs_swag_inputs_fwd(ctypes.byref(grid), 0, n, ptr(x), None, None, None, 0, 0, None, ptr(table), width, ptr(enc),
+                                           None, _stream()), "b200gs_swag_inputs_fwd")
+        ctx.grid = grid
+        ctx.save_for_backward(x, table)
+        return enc
+
+    @staticmethod
+    def backward(ctx, v_enc):
+        x, table = ctx.saved_tensors
+        v_enc = _f32c(v_enc, "grad")
+        v_table = torch.empty_like(table)
+        check(lib().b200gs_swag_inputs_bwd(ctypes.byref(ctx.grid), 0, x.shape[0], ptr(x), None, None, None, 0, 0, None, None, ptr(v_enc),
+                                           v_enc.shape[1], None, None, None, ptr(v_table), _stream()), "b200gs_swag_inputs_bwd")
+        return None, v_table, None
+
+
+def hash_grid_encode(params: torch.Tensor, x: torch.Tensor, **grid) -> torch.Tensor:
+    """tiny-cuda-nn's 3-D ``HashGrid`` encoding (linear interpolation) of the points ``x`` [n, 3] (any values: points outside [0, 1]
+    wrap as in tcnn) with the flat table ``params`` (tcnn layout, ``hash_grid_params(**grid)`` floats): enc [n, n_levels F].  The
+    gradient reaches ``params`` only (tcnn's input gradient is not provided), scattered with vector float atomics: not
+    bit-reproducible.  ``grid``: n_levels, n_features_per_level, log2_hashmap_size, base_resolution, per_level_scale."""
+    g = _hash_grid(**{**HASH_GRID_DEFAULTS, **grid})
+    _check_table(params, g)
+    x = _f32c(x.detach(), "x")
+    if x.dim() != 2 or x.shape[1] != 3:
+        raise ValueError("x must be [n, 3]")
+    return _HashGridEncode.apply(g, params, x)
+
+
+def swag_supported(in_dim: int, n_neurons: int, n_layers: int) -> bool:
+    """Whether the SWAG MLP kernels take a network on ``in_dim`` real input columns (no device needed)."""
+    return int(lib().b200gs_swag_mlp_workspace_bytes((in_dim + 7) // 8 * 8, n_neurons, n_layers)) > 0
+
+
+class _SwagColoursAndOpacities(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, cfg, means, campos, shs, shs_rest, bbox, table, base_opacity, u, *params):
+        grid, degree, split, stride, in_dim, row, temperature, eps = cfg
+        n, dev, L_ = means.shape[0], means.device, lib()
+        weights, biases = params[0::2], params[1::2]
+        x0 = torch.empty(n, row, dtype=torch.float32, device=dev)
+        clamped = torch.empty(n, dtype=torch.uint8, device=dev)
+        check(L_.b200gs_swag_inputs_fwd(ctypes.byref(grid), degree, n, ptr(means), ptr(campos), ptr(shs), ptr(shs_rest), stride, int(split),
+                                        ptr(bbox), ptr(table), row, ptr(x0), ptr(clamped), _stream()), "b200gs_swag_inputs_fwd")
+        m = _lib.B200gsAppearanceMlp(row, -1, weights[0].shape[0], len(weights), 4, 0, 0, 2, weights[0].shape[1], weights[0].shape[1])
+        for l in range(len(weights)):
+            m.weights[l], m.biases[l] = weights[l].data_ptr(), biases[l].data_ptr()
+        colour = torch.empty(n, 3, dtype=torch.float32, device=dev)
+        opacity = torch.empty(n, dtype=torch.float32, device=dev)
+        check(L_.b200gs_swag_mlp_fwd(ctypes.byref(m), in_dim, n, ptr(x0), ptr(base_opacity), ptr(u), temperature, eps, ptr(colour),
+                                     ptr(opacity), _stream()), "b200gs_swag_mlp_fwd")
+        ctx.cfg, ctx.m = cfg, m
+        ctx.save_for_backward(means, campos, shs, shs_rest, bbox, table, base_opacity, u, x0, clamped, *params)
+        return colour, opacity
+
+    @staticmethod
+    def backward(ctx, v_colour, v_opacity):
+        means, campos, shs, shs_rest, bbox, table, base_opacity, u, x0, clamped, *params = ctx.saved_tensors
+        grid, degree, split, stride, in_dim, row, temperature, eps = ctx.cfg
+        m, L_ = ctx.m, lib()
+        n, dev = means.shape[0], means.device
+        v_colour = _f32c(v_colour, "grad") if v_colour is not None else torch.zeros(n, 3, dtype=torch.float32, device=dev)
+        v_opacity = _f32c(v_opacity, "grad") if v_opacity is not None else None
+        ws, bs, total = _appearance_offsets(row, -1, m.n_neurons, m.n_layers, 4)
+        v_x0 = torch.empty_like(x0)
+        v_base = torch.empty_like(base_opacity)
+        ws_bytes = int(L_.b200gs_swag_mlp_workspace_bytes(row, m.n_neurons, m.n_layers))
+        workspace = torch.empty(ws_bytes // 4, dtype=torch.float32, device=dev)
+        v_params = torch.empty(total, dtype=torch.float32, device=dev)
+        check(L_.b200gs_swag_mlp_bwd(ctypes.byref(m), in_dim, n, ptr(x0), ptr(base_opacity), ptr(u), temperature, eps, ptr(v_colour),
+                                     ptr(v_opacity), ptr(v_x0), ptr(v_base), ptr(workspace), ws_bytes, ptr(v_params), _stream()),
+              "b200gs_swag_mlp_bwd")
+        v_shs, v_shs_rest = torch.empty_like(shs), (torch.empty_like(shs_rest) if split else None)
+        v_means = torch.empty_like(means)
+        v_table = torch.empty_like(table)
+        check(L_.b200gs_swag_inputs_bwd(ctypes.byref(grid), degree, n, ptr(means), ptr(campos), ptr(shs), ptr(shs_rest), stride, int(split),
+                                        ptr(bbox), ptr(clamped), ptr(v_x0), row, ptr(v_shs), ptr(v_shs_rest), ptr(v_means), ptr(v_table),
+                                        _stream()), "b200gs_swag_inputs_bwd")
+        grads = []
+        for l, ((wo, r, c), (bo, _)) in enumerate(zip(ws, bs)):
+            v_w = v_params[wo:wo + r * c].view(r, c)
+            if l == 0:      # the row's real columns; the embedding's get theirs through biases[0]
+                full = torch.zeros_like(params[0])
+                full[:, :in_dim] = v_w[:, :in_dim]
+                v_w = full
+            grads += [v_w, v_params[bo:bo + r]]
+        return (None, v_means, None, v_shs, v_shs_rest, None, v_table, v_base, None, *grads)
+
+
+def swag_colours_and_opacities(degree: int, means: torch.Tensor, campos: torch.Tensor, base_opacity: torch.Tensor, u: torch.Tensor,
+                               table: torch.Tensor, embedding: torch.Tensor, weights, biases, *, bbox: Optional[torch.Tensor] = None,
+                               shs_dc: Optional[torch.Tensor] = None, shs_rest: Optional[torch.Tensor] = None,
+                               features: Optional[torch.Tensor] = None, temperature: float = 0.1, eps: float = 1e-8,
+                               **grid) -> Tuple[torch.Tensor, torch.Tensor]:
+    """SWAG's image-conditioned colours and opacities (swag_renderer.py:47-56) as one autograd node: returns ``(colours [N, 3],
+    opacities [N])``.
+
+    Per Gaussian: rgb = clamp_min(SH_degree(colour; normalize(means - campos)) + 0.5, 0) from ``shs_dc`` [N,1,3] with ``shs_rest``
+    [N,K-1,3] or ``features`` [N,K,3]; enc = the hash grid ``table`` (``hash_grid_params(**grid)`` floats) at ``(means - bbox[:3]) /
+    bbox[3:]`` (``bbox`` 6 floats on the device: the box's minimum and size; None: the means themselves); o = the network
+    ``weights`` / ``biases`` (Linear layers, ReLU between them, no output activation, ``weights[0]`` [H, 3 + enc + E]) on
+    ``[rgb | enc | embedding]``, the image ``embedding`` [E] folded into the first bias; colours = sigmoid(o[:3]) and opacities =
+    clamp_min(base_opacity - sigmoid((log(|o3| + eps) + log(u + eps) - log(1 - u + eps)) / temperature), 0), ``base_opacity`` [N] the
+    activated opacity and ``u`` a one-element device tensor (no host read).  Forward K49 + K20, backward K21 + K22 + K50: no host
+    synchronisation.  Gradients reach the SH coefficients, ``means`` (through the view direction only, as in the reference), the
+    table, ``base_opacity``, the embedding and every weight and bias."""
+    degree = int(degree)
+    if not 0 <= degree <= 4:
+        raise ValueError(f"degree must be 0..4, got {degree}")
+    g = _hash_grid(**{**HASH_GRID_DEFAULTS, **grid})
+    _check_table(table, g)
+    n, need = means.shape[0], (degree + 1) ** 2
+    if means.dim() != 2 or means.shape[1] != 3:
+        raise ValueError("means must be [N, 3]")
+    if features is not None and (shs_dc is not None or shs_rest is not None):
+        raise ValueError("pass either features or shs_dc and shs_rest, not both")
+    split = shs_dc is not None
+    if split:
+        if shs_rest is None or shs_dc.shape != (n, 1, 3) or shs_rest.dim() != 3 or shs_rest.shape[0] != n or shs_rest.shape[2] != 3:
+            raise ValueError("expected shs_dc [N,1,3] and shs_rest [N,K-1,3]")
+        stride = 1 + shs_rest.shape[1]
+        shs, shs_rest = _f32_in_place(shs_dc, "shs_dc"), _f32_in_place(shs_rest, "shs_rest")
+    else:
+        if features is None or features.dim() != 3 or features.shape[0] != n or features.shape[2] != 3:
+            raise ValueError("expected features [N,K,3] (or shs_dc and shs_rest)")
+        stride = features.shape[1]
+        shs, shs_rest = _f32_in_place(features, "features"), None
+    if stride < need:
+        raise ValueError(f"the SH colour has {stride} coefficients, degree {degree} needs {need}")
+    enc_dim = g.n_levels * g.n_features_per_level
+    in_dim, e = 3 + enc_dim, embedding.shape[0]
+    row = (in_dim + 7) // 8 * 8
+    if weights[0].shape[1] != in_dim + e or weights[-1].shape[0] != 4:
+        raise ValueError(f"weights[0] must be [H, {in_dim + e}] (3 colour + {enc_dim} encoding + {e} embedding columns) and the output 4 wide")
+    if not swag_supported(in_dim, weights[0].shape[0], len(weights)):
+        raise NotImplementedError(f"b200gs SWAG network: {len(weights)} layers of {weights[0].shape[0]} neurons on {in_dim} inputs is not "
+                                  "supported (n_neurons 64 or 128, n_layers 2..4)")
+    means = _f32_in_place(means, "means")
+    campos = _f32c(campos, "campos").reshape(-1)
+    base_opacity = _f32c(base_opacity.reshape(-1), "base_opacity")
+    u = _f32c(u.reshape(-1), "u")
+    if campos.numel() != 3 or u.numel() != 1 or base_opacity.numel() != n:
+        raise ValueError("campos must be 3 floats, u one float and base_opacity [N]")
+    if bbox is not None:
+        bbox = _f32c(bbox.reshape(-1), "bbox")
+        if bbox.numel() != 6:
+            raise ValueError("bbox must be 6 floats: the minimum, then the size")
+    b0 = torch.addmv(biases[0], weights[0][:, in_dim:in_dim + e], embedding)
+    params = []
+    for l, (w, b) in enumerate(zip(weights, biases)):
+        params += [_f32c(w, "weight"), _f32c(b0 if l == 0 else b, "bias")]
+    cfg = (g, degree, split, stride, in_dim, row, float(temperature), float(eps))
+    return _SwagColoursAndOpacities.apply(cfg, means, campos, shs, shs_rest, bbox, table, base_opacity, u, *params)

@@ -477,6 +477,60 @@ B200GS_API int b200gs_glossy_sh_bwd(int32_t degree, int64_t n, const float* mean
                                     int32_t sh_stride, int32_t sh_split, const uint8_t* clamped, const float* v_opacity,
                                     const float* v_rgb, float* v_op_dc, float* v_op_rest, float* v_shs, float* v_shs_rest, void* stream);
 
+/* ---- K49 / K50 and the SWAG MLP: in-the-wild appearance of SWAGRenderer.forward (swag_renderer.py:32-66, swag_model.py) ---------
+ * B200gsHashGrid (host struct): tiny-cuda-nn's 3-D HashGrid encoding, linear interpolation: n_levels 1..16, n_features_per_level
+ *     F = 2 | 4, log2_hashmap_size 1..24, base_resolution >= 1, per_level_scale >= 1.  Level l (fp32, on the host): scale_l =
+ *     exp2f(l log2f(per_level_scale)) base - 1 (< 2^30), res_l = ceil(scale_l) + 1, size_l = min(next_multiple(res_l^3, 8),
+ *     2^log2_hashmap_size) vertices of F floats, the levels in order: b200gs_hash_grid_params floats (11681792 for 8 / 4 / 19 / 16 /
+ *     2.0; 0 for a grid outside that set).  Point x: pos = fmaf(scale_l, x, 0.5f), cell = (uint32)(int)floor(pos), frac = pos -
+ *     floor(pos) per axis; corner k = 0..7 (bit d: axis d) weighs prod_d (bit ? frac_d : 1 - frac_d) and reads vertex tcnn
+ *     grid_index(cell + bits) (dense strides while they fit size_l, else the coherent prime hash 1 / 2654435761 / 805459861 xor-ed)
+ *     % size_l.  Points outside [0, 1] follow the same uint32 arithmetic.
+ * b200gs_swag_inputs_fwd (K49): x0 float[n, row_stride] <- [rgb | enc | 0 ..], row_stride <= 72.  With shs (colour on):
+ *     rgb = clamp_min(SH_degree(colour; dir_i) + 0.5, 0), dir_i = (means[i] - campos) / max(|.|, 1e-12), colour sh_split = 1:
+ *     shs = dc [n,1,3], shs_rest = rest [n,sh_stride-1,3]; sh_split = 0: shs = [n,sh_stride,3]; sh_stride >= (degree+1)^2, degree 0..4;
+ *     clamped uint8[n] <- bit c set where channel c failed x >= 0 (NaN included).  shs NULL: no colour columns, enc from column 0.
+ *     enc = the grid of table float[b200gs_hash_grid_params] (aligned to one vertex) at (means[i] - bbox[0..2]) / bbox[3..5]
+ *     (IEEE division; bbox float[6] on the device, NULL: means[i] itself).
+ * b200gs_swag_inputs_bwd (K50): from v_x0 float[n, row_stride]: colour on: v_shs (and v_shs_rest) in the forward's layout, every
+ *     row written in full, and v_means float[n,3] through the view direction, after the clamp bits; v_table float[params] zeroed
+ *     here and then accumulated with vector float atomics (one per corner): not bit-reproducible.  Pad columns are not read.
+ * Launches: K49 1, K50 1 (0 when n == 0) and one cudaMemsetAsync.
+ * Algorithmic bytes per Gaussian, degree 3, default grid, row_stride 40: fwd 204 in + 161 out + 64 gathers of 16 B; bwd 365 in +
+ *     204 out + 64 vector atomics of 16 B.  FLOPs: ~900 fwd, ~1300 bwd (SH basis and gradient, 64 weights and corner indices).
+ * SWAG MLP (K20/K21 with epilogue 2): mlp as for b200gs_appearance_mlp_* with n_freq = -1, n_out = 4, normalize = normalize_dirs = 0,
+ *     epilogue = 2; feat_dim = row_stride of x0, in_dim the real columns (feat_dim - 8 < in_dim <= feat_dim): the kernels read W_0's
+ *     columns [0, in_dim) and treat [in_dim, feat_dim) as zero, so the caller may pass the reference's [n_neurons, in_dim + E] W_0
+ *     (w0_stride >= in_dim) with the image embedding folded into biases[0].  With o the 4 outputs of a row and u (float[1] on the
+ *     device, in (0, 1) or 0.5 in evaluation):
+ *         colour[i] = sigmoid(o[0..2]),  z = float(1 / temperature) ((log(|o3| + eps) + log(u + eps)) - log(1 - u + eps)),
+ *         opacity[i] = clamp_min(base_opacity[i] - sigmoid(z), 0)                      base_opacity float[n] (activated)
+ *     bwd: torch's rules (abs has gradient 0 at 0; clamp_min passes where its argument >= 0); v_colour float[n,3] and v_opacity float[n]
+ *     (nullable: zero); writes v_x0 float[n, feat_dim] (16-byte aligned), v_base_opacity float[n] and v_params as
+ *     b200gs_appearance_mlp_bwd's (W_0's block [n_neurons, feat_dim]; columns at or past in_dim are zero).  temperature > 0, eps >= 0.
+ * Launches: forward 1, backward 2.  Bytes per row: fwd 4 feat_dim + 4 in, 16 out; bwd 4 feat_dim + 20 in, 4 feat_dim + 4 out.
+ *     FLOPs per row: 2 x (feat_dim n_neurons + (n_layers - 2) n_neurons^2 + 8 n_neurons) forward (~13 K for the defaults), three
+ *     times that backward. */
+typedef struct B200gsHashGrid {
+    int32_t n_levels, n_features_per_level, log2_hashmap_size, base_resolution;
+    float per_level_scale;
+} B200gsHashGrid;
+B200GS_API int64_t b200gs_hash_grid_params(const B200gsHashGrid* grid);
+B200GS_API int b200gs_swag_inputs_fwd(const B200gsHashGrid* grid, int32_t degree, int64_t n, const float* means, const float* campos,
+                                      const float* shs, const float* shs_rest, int32_t sh_stride, int32_t sh_split, const float* bbox,
+                                      const float* table, int32_t row_stride, float* x0, uint8_t* clamped, void* stream);
+B200GS_API int b200gs_swag_inputs_bwd(const B200gsHashGrid* grid, int32_t degree, int64_t n, const float* means, const float* campos,
+                                      const float* shs, const float* shs_rest, int32_t sh_stride, int32_t sh_split, const float* bbox,
+                                      const uint8_t* clamped, const float* v_x0, int32_t row_stride, float* v_shs, float* v_shs_rest,
+                                      float* v_means, float* v_table, void* stream);
+B200GS_API size_t b200gs_swag_mlp_workspace_bytes(int32_t feat_dim, int32_t n_neurons, int32_t n_layers);
+B200GS_API int b200gs_swag_mlp_fwd(const B200gsAppearanceMlp* mlp, int32_t in_dim, int64_t n, const float* x0, const float* base_opacity,
+                                   const float* u, float temperature, float eps, float* colour, float* opacity, void* stream);
+B200GS_API int b200gs_swag_mlp_bwd(const B200gsAppearanceMlp* mlp, int32_t in_dim, int64_t n, const float* x0, const float* base_opacity,
+                                   const float* u, float temperature, float eps, const float* v_colour, const float* v_opacity,
+                                   float* v_x0, float* v_base_opacity, void* workspace, size_t workspace_bytes, float* v_params,
+                                   void* stream);
+
 /* ---- K2-K5: tile binning ------------------------------------------------------------------------------------------
  * replaces dgr InclusiveSum + duplicateWithKeys + SortPairs + identifyTileRanges / gsplat isect_tiles + isect_offset_encode.
  * Result order is exactly that of a stable sort of (tile_id << 32 | float_bits(depth)) keys emitted Gaussian-major:
