@@ -43,6 +43,11 @@ class B200gsHashGrid(ctypes.Structure):
                 ("per_level_scale", c_float)]
 
 
+class B200gsGs4d(ctypes.Structure):
+    _fields_ = [("n_levels", c_int32), ("channels", c_int32), ("net_width", c_int32), ("defor_depth", c_int32), ("flags", c_int32),
+                ("resolution", (c_int32 * 4) * 4), ("weights", c_void_p * 10), ("biases", c_void_p * 10)]
+
+
 class B200gsError(RuntimeError):
     pass
 
@@ -111,6 +116,9 @@ _SIGNATURES = {
     "b200gs_swag_mlp_fwd": (c_int32, [POINTER(B200gsAppearanceMlp), c_int32, c_int64, _P, _P, _P, c_float, c_float, _P, _P, _P]),
     "b200gs_swag_mlp_bwd": (c_int32, [POINTER(B200gsAppearanceMlp), c_int32, c_int64, _P, _P, _P, c_float, c_float] + [_P] * 5
                             + [c_size_t, _P, _P]),
+    "b200gs_gs4d_plane_floats": (c_int64, [POINTER(B200gsGs4d)]),
+    "b200gs_gs4d_repack_planes": (c_int32, [POINTER(B200gsGs4d), POINTER(c_void_p), _P, _P]),
+    "b200gs_gs4d_deform_fwd": (c_int32, [POINTER(B200gsGs4d), c_int64] + [_P] * 13 + [_P]),
     "b200gs_sh_fwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P]),
     "b200gs_sh_bwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P, _P, _P]),
     "b200gs_sh_split_fwd": (c_int32, [c_int32, c_int32, c_int64, _P, _P, _P, _P, _P, _P]),

@@ -9,8 +9,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libb200gs.so")
-SOURCES = ["api.cu", "project.cu", "binning.cu", "blend.cu", "loss.cu", "optim.cu", "knn.cu", "mcmc.cu", "isect.cu", "bilagrid.cu", "appearance.cu", "exposure.cu", "depth_loss.cu", "visibility.cu", "gauss_reg.cu", "normal_reg.cu", "similarity_reg.cu", "glossy.cu", "swag.cu"]
-HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "geometry.cuh"), os.path.join(CSRC, "onesweep.cuh"), os.path.join(CSRC, "knn_grid.h"), os.path.join(CSRC, "ssim.cuh"), os.path.join(CSRC, "sh.cuh"),
+SOURCES = ["api.cu", "project.cu", "binning.cu", "blend.cu", "loss.cu", "optim.cu", "knn.cu", "mcmc.cu", "isect.cu", "bilagrid.cu", "appearance.cu", "exposure.cu", "depth_loss.cu", "visibility.cu", "gauss_reg.cu", "normal_reg.cu", "similarity_reg.cu", "glossy.cu", "swag.cu", "gs4d.cu"]
+HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "geometry.cuh"), os.path.join(CSRC, "onesweep.cuh"), os.path.join(CSRC, "knn_grid.h"), os.path.join(CSRC, "ssim.cuh"), os.path.join(CSRC, "sh.cuh"), os.path.join(CSRC, "warp_mma.cuh"),
            os.path.join(os.path.dirname(HERE), "include", "b200gs.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]

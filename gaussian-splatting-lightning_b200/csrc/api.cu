@@ -28,7 +28,7 @@ using namespace b200gs;
 extern "C" {
 
 const char* b200gs_last_error(void) { return g_error; }
-int b200gs_version(void) { return 236; }
+int b200gs_version(void) { return 237; }
 int64_t b200gs_launch_count(void) { return (int64_t)g_launches.load(std::memory_order_relaxed); }
 
 int b200gs_ipc_alloc(size_t bytes, void** dev_ptr, unsigned char* handle64) {

@@ -1589,3 +1589,164 @@ def swag_colours_and_opacities(degree: int, means: torch.Tensor, campos: torch.T
         params += [_f32c(w, "weight"), _f32c(b0 if l == 0 else b, "bias")]
     cfg = (g, degree, split, stride, in_dim, row, float(temperature), float(eps))
     return _SwagColoursAndOpacities.apply(cfg, means, campos, shs, shs_rest, bbox, table, base_opacity, u, *params)
+
+
+# ---- 4DGS deformation (csrc/gs4d.cu K51/K52): forward only ------------------------------------------------------------------------
+GS4D_FWD_LAUNCHES = 1           # library launches of one gs4d_deform (K51)
+GS4D_HEADS = ("dx", "ds", "dr", "dshs")
+GS4D_HEAD_OUT = {"dx": 3, "ds": 3, "dr": 4, "dshs": 48}
+GS4D_SUPPORTED = ("grid_dimensions 2 and input_coordinate_dim 4, output_coordinate_dim 16 or 32, 1..4 levels (multires), every plane "
+                  "resolution 1..16384 with each plane below 2^31 floats, net_width 64 or 128, defor_depth 0..2, any combination of "
+                  "no_dx / no_ds / no_dr / no_dshs / apply_rotation, and no_grid, static_mlp and empty_voxel off with grid_pe 0")
+
+
+def _gs4d_struct(n_levels, channels, net_width, defor_depth, flags, resolution) -> _lib.B200gsGs4d:
+    g = _lib.B200gsGs4d()
+    g.n_levels, g.channels, g.net_width, g.defor_depth, g.flags = int(n_levels), int(channels), int(net_width), int(defor_depth), int(flags)
+    for l, r in enumerate(resolution[:4]):
+        for d in range(4):
+            g.resolution[l][d] = int(r[d])
+    return g
+
+
+def gs4d_supported(n_levels: int, channels: int, net_width: int, defor_depth: int, resolution=None) -> bool:
+    """Whether K51 takes this HexPlane field and network (no device needed).  ``resolution``: per level the (x, y, z, t) nodes
+    (None: 64, 64, 64, 25 at every level)."""
+    if resolution is None:
+        resolution = [(64, 64, 64, 25)] * max(int(n_levels), 0)
+    if len(resolution) != int(n_levels):
+        return False
+    return int(lib().b200gs_gs4d_plane_floats(ctypes.byref(_gs4d_struct(n_levels, channels, net_width, defor_depth, 0, resolution)))) > 0
+
+
+class Gs4dPlanes:
+    """A HexPlane field repacked channel-last by K52: ``planes`` float32 [b200gs_gs4d_plane_floats], ``resolution`` the (x, y, z, t)
+    nodes of each level, ``channels`` C.  Made by ``gs4d_repack_planes``; read by every ``gs4d_deform`` call."""
+
+    def __init__(self, planes: torch.Tensor, resolution, channels: int):
+        self.planes, self.resolution, self.channels = planes, [tuple(r) for r in resolution], int(channels)
+
+    @property
+    def n_levels(self) -> int:
+        return len(self.resolution)
+
+
+def gs4d_repack_planes(grids) -> Gs4dPlanes:
+    """Repack the reference's ``HexPlaneField.grids`` (L levels of 6 planes [1, C, res_b, res_a], plane k = (a, b) of (0,1), (0,2),
+    (0,3), (1,2), (1,3), (2,3)) into K51's channel-last layout, once per model (K52, one launch).  The planes are only read."""
+    grids = [list(level) for level in grids]
+    if not 1 <= len(grids) <= 4:
+        raise NotImplementedError(f"{len(grids)} HexPlane levels (multires) is not supported: b200gs 4DGS takes {GS4D_SUPPORTED}")
+    channels, resolution, flat = None, [], []
+    for level in grids:
+        if len(level) != 6:
+            raise NotImplementedError(f"a level of {len(level)} planes is not supported (grid_dimensions 2, input_coordinate_dim 4 give 6)")
+        if any(p.dim() != 4 or p.shape[0] != 1 for p in level):
+            raise ValueError("every plane must be [1, C, res_b, res_a]")
+        c = int(level[0].shape[1])
+        channels = c if channels is None else channels
+        r = (int(level[0].shape[3]), int(level[0].shape[2]), int(level[1].shape[2]), int(level[2].shape[2]))
+        for (a, b), p in zip(((0, 1), (0, 2), (0, 3), (1, 2), (1, 3), (2, 3)), level):
+            if tuple(p.shape[1:]) != (channels, r[b], r[a]):
+                raise ValueError(f"plane ({a},{b}) is {tuple(p.shape)}, expected [1, {channels}, {r[b]}, {r[a]}]")
+            flat.append(_f32c(p.detach(), "plane"))
+        resolution.append(r)
+    g = _gs4d_struct(len(grids), channels, 64, 0, 0, resolution)
+    total = int(lib().b200gs_gs4d_plane_floats(ctypes.byref(g)))
+    if total == 0:
+        raise NotImplementedError(f"HexPlane field with output_coordinate_dim {channels} and resolutions {resolution} is not supported: "
+                                  f"b200gs 4DGS takes {GS4D_SUPPORTED}")
+    planes = torch.empty(total, dtype=torch.float32, device=flat[0].device)
+    src = (ctypes.c_void_p * len(flat))(*[p.data_ptr() for p in flat])
+    check(lib().b200gs_gs4d_repack_planes(ctypes.byref(g), src, ptr(planes), _stream()), "b200gs_gs4d_repack_planes")
+    return Gs4dPlanes(planes, resolution, channels)
+
+
+def _aligned16(t: torch.Tensor) -> torch.Tensor:
+    return t if t.data_ptr() % 16 == 0 else t.clone()
+
+
+def gs4d_deform(means: torch.Tensor, log_scales: torch.Tensor, quats: torch.Tensor, time, planes: Gs4dPlanes, aabb: torch.Tensor,
+                trunk, heads, *, shs_dc: Optional[torch.Tensor] = None, shs_rest: Optional[torch.Tensor] = None,
+                apply_rotation: bool = False):
+    """The 4DGS deformation of VanillaGS4DRenderer.forward (Deformation.forward_dynamic with mask 1) in one kernel (K51), forward only:
+    returns ``(means', log_scales', quats', shs_dc', shs_rest')`` of the raw parameters ``means`` / ``log_scales`` [N,3] and ``quats``
+    [N,4] (not normalised) at time ``time`` (a float or a one-element tensor, used as given).
+
+    ``planes``: the repacked HexPlane field (``gs4d_repack_planes``); ``aabb`` [2, 3]: the reference's ``grid.aabb`` (row 0 xyz_max,
+    row 1 xyz_min).  ``trunk``: the (weight, bias) of ``feature_out``'s Linear layers (one, or two for defor_depth 2); ``heads``: for
+    each enabled head of ``GS4D_HEADS`` its ((hidden weight, bias), (output weight, bias)).  A head left out is off (no_dx ...): its
+    parameter passes through.  With ``dshs`` on, ``shs_dc`` [N,1,3] and ``shs_rest`` [N,15,3] get dshs; otherwise they are returned
+    as they are.  ``apply_rotation``: quats' = normalize(quats * dr) instead of quats + dr.
+
+    There is no autograd node: while grad is enabled, an input that requires grad raises.  Shapes outside ``GS4D_SUPPORTED`` raise
+    NotImplementedError."""
+    heads = dict(heads)
+    unknown = set(heads) - set(GS4D_HEADS)
+    if unknown:
+        raise ValueError(f"unknown heads {sorted(unknown)}: the heads are {GS4D_HEADS}")
+    trunk = list(trunk)
+    tensors = [means, log_scales, quats, aabb, shs_dc, shs_rest, planes.planes, time] + [t for wb in trunk for t in wb] + \
+        [t for h in heads.values() for wb in h for t in wb]
+    if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in tensors):
+        raise RuntimeError("ops.gs4d_deform is forward only (the 4DGS deformation has no autograd node) and an input requires grad: "
+                           "call it under torch.no_grad() or pass detached tensors")
+    n = means.shape[0]
+    if means.dim() != 2 or means.shape[1] != 3 or log_scales.shape != (n, 3) or quats.shape != (n, 4):
+        raise ValueError("expected means [N,3], log_scales [N,3] and quats [N,4]")
+    if not 1 <= len(trunk) <= 2:
+        raise NotImplementedError(f"a trunk of {len(trunk)} Linear layers is not supported (defor_depth 0..2): b200gs 4DGS takes "
+                                  f"{GS4D_SUPPORTED}")
+    width, k0 = int(trunk[0][0].shape[0]), planes.channels * planes.n_levels
+    if width not in (64, 128):
+        raise NotImplementedError(f"net_width {width} is not supported: b200gs 4DGS takes {GS4D_SUPPORTED}")
+    g = _gs4d_struct(planes.n_levels, planes.channels, width, len(trunk), 0, planes.resolution)
+    keep = []
+
+    def layer(i, wb, rows, cols, what):
+        w, b = wb
+        if tuple(w.shape) != (rows, cols) or tuple(b.shape) != (rows,):
+            raise ValueError(f"{what} must be a Linear({cols}, {rows}), got weight {tuple(w.shape)} and bias {tuple(b.shape)}")
+        w, b = _aligned16(_f32c(w.detach(), what)), _f32c(b.detach(), what)
+        keep.extend((w, b))
+        g.weights[i], g.biases[i] = w.data_ptr(), b.data_ptr()
+
+    layer(0, trunk[0], width, k0, "the first trunk layer")
+    if len(trunk) == 2:
+        layer(1, trunk[1], width, width, "the second trunk layer")
+    for h, name in enumerate(GS4D_HEADS):
+        if name in heads:
+            g.flags |= 1 << h
+            hidden, out = heads[name]
+            layer(2 + 2 * h, hidden, width, width, f"the {name} head's hidden layer")
+            layer(3 + 2 * h, out, GS4D_HEAD_OUT[name], width, f"the {name} head's output layer")
+    if apply_rotation:
+        g.flags |= 16
+    if int(lib().b200gs_gs4d_plane_floats(ctypes.byref(g))) != planes.planes.numel():
+        raise NotImplementedError(f"net_width {width} with defor_depth {len(trunk)} on {planes.n_levels} levels of "
+                                  f"{planes.channels} channels is not supported: b200gs 4DGS takes {GS4D_SUPPORTED}")
+    dev = means.device
+    means, log_scales = _f32c(means.detach(), "means"), _f32c(log_scales.detach(), "log_scales")
+    quats = _aligned16(_f32c(quats.detach(), "quats"))
+    aabb = _f32c(aabb.detach().reshape(-1), "aabb")
+    if aabb.numel() != 6:
+        raise ValueError("aabb must be [2, 3]: xyz_max, then xyz_min")
+    t = time.detach().reshape(-1).to(device=dev, dtype=torch.float32) if isinstance(time, torch.Tensor) else \
+        torch.tensor([float(time)], dtype=torch.float32).to(dev, non_blocking=True)
+    if t.numel() != 1:
+        raise ValueError("time must be one value")
+    if planes.planes.device != dev:
+        raise ValueError("planes must be on the means' device")
+    dshs = "dshs" in heads
+    if dshs:
+        if shs_dc is None or shs_rest is None or shs_dc.shape != (n, 1, 3) or shs_rest.shape != (n, 15, 3):
+            raise ValueError("the dshs head needs shs_dc [N,1,3] and shs_rest [N,15,3] (SH degree 3: 16 coefficients)")
+        shs_dc, shs_rest = _f32c(shs_dc.detach(), "shs_dc"), _f32c(shs_rest.detach(), "shs_rest")
+    means_out, scales_out = torch.empty_like(means), torch.empty_like(log_scales)
+    quats_out = torch.empty_like(quats)
+    dc_out, rest_out = (torch.empty_like(shs_dc), torch.empty_like(shs_rest)) if dshs else (shs_dc, shs_rest)
+    check(lib().b200gs_gs4d_deform_fwd(ctypes.byref(g), n, ptr(planes.planes), ptr(aabb), ptr(t), ptr(means), ptr(log_scales), ptr(quats),
+                                       ptr(shs_dc) if dshs else None, ptr(shs_rest) if dshs else None, ptr(means_out), ptr(scales_out),
+                                       ptr(quats_out), ptr(dc_out) if dshs else None, ptr(rest_out) if dshs else None, _stream()),
+          "b200gs_gs4d_deform_fwd")
+    return means_out, scales_out, quats_out, dc_out, rest_out

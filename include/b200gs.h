@@ -531,6 +531,52 @@ B200GS_API int b200gs_swag_mlp_bwd(const B200gsAppearanceMlp* mlp, int32_t in_di
                                    float* v_x0, float* v_base_opacity, void* workspace, size_t workspace_bytes, float* v_params,
                                    void* stream);
 
+/* ---- K51 / K52: 4DGS deformation of VanillaGS4DRenderer.forward (vanilla_gs4d_renderer.py, gs4d_deformation.py, gs4d_hexplane.py) --
+ * Forward only (the reference renders trained 4DGaussians checkpoints and never trains this network).
+ * B200gsGs4d (host struct): the HexPlane field and the network.  n_levels L 1..4, channels C (output_coordinate_dim) 16 | 32,
+ *     net_width W 64 | 128, defor_depth D 0..2 (0 and 1: one trunk Linear), flags any of B200GS_GS4D_*; resolution[l] = (x, y, z, t)
+ *     nodes of level l, each 1..B200GS_GS4D_MAX_RES, every plane below 2^31 floats.  Plane k = (a, b) of (0,1), (0,2), (0,3), (1,2),
+ *     (1,3), (2,3) is [C, res_b, res_a] in torch (coordinate a indexes the width).  weights[i] [rows, K] row-major (16-byte aligned)
+ *     and biases[i] [rows], as torch.nn.Linear holds them: i = 0 the trunk's first Linear [W, C L], 1 its second [W, W] (D = 2
+ *     only), then for head h = 0 dx, 1 ds, 2 dr, 3 dshs: 2 + 2h its hidden Linear [W, W] and 3 + 2h its output Linear [3 | 3 | 4 |
+ *     48, W].  Pointers of layers not in use are not read.
+ * b200gs_gs4d_plane_floats: floats of the repacked planes (the buffer b200gs_gs4d_repack_planes fills); 0 for a grid or network
+ *     outside the supported set.  No CUDA call: it is also the support query.
+ * b200gs_gs4d_repack_planes (K52): host_planes = 6 L device pointers (level-major, then plane order) to the torch planes; writes
+ *     planes float[b200gs_gs4d_plane_floats] channel-last: each plane [res_b, res_a, C], at the plane's offset in that order.
+ * b200gs_gs4d_deform_fwd (K51): n Gaussians (0 <= n <= INT32_MAX), all device pointers: aabb float[6] = (xyz_max, xyz_min) as the
+ *     reference's set_aabb stores it, time float[1] (t as given), means / log_scales float[n,3] and quats float[n,4] (raw, 16-byte
+ *     aligned), shs_dc float[n,1,3] and shs_rest float[n,15,3] (read with B200GS_GS4D_DSHS only).  With p = (means - xyz_max) *
+ *     (2 / (xyz_min - xyz_max)) - 1 (fp32, IEEE, not clamped) and f = the levels' products of the six bilinear plane samples of
+ *     (p, t) (align_corners, border padding, in plane order from 1), h = the trunk on f with ReLU between its layers, and each
+ *     enabled head Linear relu Linear relu h:
+ *         means_out = means + dx,  log_scales_out = log_scales + ds,  quats_out = quats + dr (B200GS_GS4D_APPLY_ROTATION: the
+ *         Hamilton product quats dr divided by its norm),  shs_*_out = shs_* + dshs reshaped [16, 3]
+ *     A disabled dx / ds / dr head copies its input to the output; with dshs off the SH outputs are not written (may be NULL).
+ *     Weights run as 3xTF32 mma.sync with fp32 accumulation (~fp32 accuracy).  No workspace; launches: one.  Bytes per Gaussian:
+ *     40 in + 40 out (+ 192 in + 192 out with dshs) plus 24 L corner rows of 4 C bytes gathered; FLOPs per Gaussian 2 (C L W +
+ *     (D' - 1) W^2 + sum over enabled heads (W^2 + W out_h)).
+ * Both refuse with B200GS_EINVAL before any CUDA call. */
+#define B200GS_GS4D_DX 1
+#define B200GS_GS4D_DS 2
+#define B200GS_GS4D_DR 4
+#define B200GS_GS4D_DSHS 8
+#define B200GS_GS4D_APPLY_ROTATION 16
+#define B200GS_GS4D_FLAGS 31
+#define B200GS_GS4D_MAX_RES 16384
+typedef struct B200gsGs4d {
+    int32_t n_levels, channels, net_width, defor_depth, flags;
+    int32_t resolution[4][4];
+    const float* weights[10];
+    const float* biases[10];
+} B200gsGs4d;
+B200GS_API int64_t b200gs_gs4d_plane_floats(const B200gsGs4d* grid);
+B200GS_API int b200gs_gs4d_repack_planes(const B200gsGs4d* grid, const float* const* host_planes, float* planes, void* stream);
+B200GS_API int b200gs_gs4d_deform_fwd(const B200gsGs4d* grid, int64_t n, const float* planes, const float* aabb, const float* time,
+                                      const float* means, const float* log_scales, const float* quats, const float* shs_dc,
+                                      const float* shs_rest, float* means_out, float* log_scales_out, float* quats_out,
+                                      float* shs_dc_out, float* shs_rest_out, void* stream);
+
 /* ---- K2-K5: tile binning ------------------------------------------------------------------------------------------
  * replaces dgr InclusiveSum + duplicateWithKeys + SortPairs + identifyTileRanges / gsplat isect_tiles + isect_offset_encode.
  * Result order is exactly that of a stable sort of (tile_id << 32 | float_bits(depth)) keys emitted Gaussian-major:
